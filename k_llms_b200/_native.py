@@ -23,12 +23,62 @@ F64_ABSENT_BITS = 0x7FF8C0DF00000000
 FLAG_HAS_VALUE, FLAG_SINGLE, FLAG_TIE, FLAG_NO_FINITE = 1, 2, 4, 8
 OUT_LOCAL, OUT_MULTIMEM, OUT_PEERS = 0, 1, 2
 
-EXPORTS = (
-    "kc_version", "kc_last_error", "kc_device_count", "kc_sm_count", "kc_set_device", "kc_vote_i32", "kc_numeric_f64", "kc_vote_i32_ex", "kc_numeric_f64_ex", "kc_vote_i8", "kc_consensus_host_i8", "kc_consolidate_json", "kc_free_strings", "kc_levenshtein", "kc_medoid_str", "kc_medoid_str_host", "kc_align_json", "kc_debug_similarity_json", "kc_debug_lsap", "kc_json_plan", "kc_json_inputs", "kc_json_emit", "kc_json_free", "kc_vote_i32_peers", "kc_numeric_f64_peers", "kc_vote_i32_peers_packed",
-    "kc_confidence_f64", "kc_logprob_sum_f32", "kc_weighted_vote_i32", "kc_consensus_host", "kc_host_alloc", "kc_host_free",
-    "kc_consolidate_json_packed", "kc_json_result_view", "kc_json_result_free", "kc_debug_jsongpu_plan", "kc_debug_jsongpu_inputs",
-    "kc_debug_jsongpu_emit", "kc_debug_jsongpu_medoid_inputs", "kc_debug_jsongpu_set_medoid", "kc_debug_jsongpu_free", "kc_debug_parse_doubles", "kc_debug_float_reprs", "kc_debug_round5", "kc_debug_s32_texts", "kc_push_results", "kc_vote_i32_wire", "kc_medoid_str_method",
-)
+_vp, _i32, _i64, _u32, _u64, _f64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64, ctypes.c_uint32, ctypes.c_uint64, ctypes.c_double
+_int, _str, _pp = ctypes.c_int, ctypes.c_char_p, ctypes.POINTER(ctypes.c_void_p)
+_CONSENSUS_HOST = [_vp, _i32, _vp, _vp, _i32, _i64, _i32, _f64, _f64, _vp, _vp, _vp, _vp, _int, _vp]
+
+# Every function of the C ABI (include/kllms_b200.h): name -> (restype, argtypes).  None is void.
+_SIGNATURES = {
+    "kc_version": (_int, []),
+    "kc_last_error": (_str, []),
+    "kc_device_count": (_int, []),
+    "kc_sm_count": (_int, [_int]),
+    "kc_set_device": (_int, [_int]),
+    "kc_vote_i32": (_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "kc_vote_i32_ex": (_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _u32, _vp]),
+    "kc_vote_i32_peers": (_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _i32, _vp, _vp]),
+    "kc_vote_i32_peers_packed": (_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "kc_vote_i32_wire": (_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp]),
+    "kc_vote_i8": (_int, [_vp, _i64, _i32, _vp, _i32, _vp, _vp, _vp]),
+    "kc_numeric_f64": (_int, [_vp, _i64, _i32, _f64, _f64, _vp, _vp, _vp]),
+    "kc_numeric_f64_ex": (_int, [_vp, _i64, _i32, _f64, _f64, _vp, _vp, _u32, _vp]),
+    "kc_numeric_f64_peers": (_int, [_vp, _i64, _i32, _f64, _f64, _vp, _vp, _i32, _vp, _vp]),
+    "kc_push_results": (_int, [_vp, _vp, _i64, _vp, _vp, _i64, _vp, _vp, _vp, _i32, _i32, _vp, _vp, _i32, _vp]),
+    "kc_confidence_f64": (_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
+    "kc_logprob_sum_f32": (_int, [_vp, _vp, _i64, _vp, _vp]),
+    "kc_weighted_vote_i32": (_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "kc_consensus_host": (_int, _CONSENSUS_HOST),
+    "kc_consensus_host_i8": (_int, _CONSENSUS_HOST),
+    "kc_host_alloc": (_vp, [_u64]),
+    "kc_host_free": (None, [_vp]),
+    "kc_medoid_str": (_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp]),
+    "kc_medoid_str_method": (_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
+    "kc_medoid_str_host": (_int, [_vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _int]),
+    "kc_levenshtein": (_int, [_str, _i32, _str, _i32]),
+    "kc_consolidate_json": (_int, [_vp, _vp, _i64, _i32, _f64, _f64, _int, _i32, _vp, _vp, _vp]),
+    "kc_free_strings": (None, [_vp, _i64]),
+    "kc_align_json": (_int, [ctypes.POINTER(_str), _vp, _i32, _f64, ctypes.POINTER(_str)]),
+    "kc_json_plan": (_int, [_vp, _vp, _i64, _i32, _i32, _pp]),
+    "kc_json_inputs": (_int, [_vp] * 10),
+    "kc_json_emit": (_int, [_vp] * 9),
+    "kc_json_free": (None, [_vp]),
+    "kc_consolidate_json_packed": (_int, [_vp, _vp, _i64, _i32, _f64, _f64, _int, _i32, _u32, _pp]),
+    "kc_json_result_view": (_int, [_vp] + [_pp] * 7 + [_vp]),
+    "kc_json_result_free": (None, [_vp]),
+    "kc_debug_similarity_json": (_int, [_str, _str, ctypes.POINTER(_f64)]),
+    "kc_debug_lsap": (_int, [_i32, _i32, _vp, _vp, _vp]),
+    "kc_debug_jsongpu_plan": (_int, [_vp, _vp, _i64, _i32, _pp]),
+    "kc_debug_jsongpu_inputs": (_int, [_vp] * 6),
+    "kc_debug_jsongpu_emit": (_int, [_vp, _vp, _vp, _vp] + [_pp] * 4),
+    "kc_debug_jsongpu_medoid_inputs": (_int, [_vp] + [_pp] * 3 + [ctypes.POINTER(_i64)]),
+    "kc_debug_jsongpu_set_medoid": (_int, [_vp, _vp, _vp]),
+    "kc_debug_jsongpu_free": (None, [_vp]),
+    "kc_debug_parse_doubles": (_int, [_vp, _vp, _i64, _vp, _vp]),
+    "kc_debug_float_reprs": (_int, [_vp, _i64, _vp, _vp]),
+    "kc_debug_round5": (_int, [_vp, _i64, _vp]),
+    "kc_debug_s32_texts": (_int, [_u64, _i64, _i32, _i32, _vp, _i64, _vp]),
+}
+EXPORTS = tuple(_SIGNATURES)
 
 
 class NativeError(RuntimeError):
@@ -50,82 +100,11 @@ def load() -> ctypes.CDLL:
             f"{LIB_PATH} not found: build the sm_90a library first (make -C k_llms_b200/csrc, or "
             "__graft_entry__.build()).  k_llms_b200 has no CPU fallback for the consensus hot path.")
     lib = ctypes.CDLL(LIB_PATH)
-    c = ctypes
-    vp, i32, i64, f64 = c.c_void_p, c.c_int32, c.c_int64, c.c_double
-    lib.kc_version.restype = c.c_int
-    lib.kc_last_error.restype = c.c_char_p
-    lib.kc_device_count.restype = c.c_int
-    lib.kc_sm_count.argtypes = [c.c_int]
-    lib.kc_set_device.argtypes = [c.c_int]
-    lib.kc_vote_i32.argtypes = [vp, i64, i32, vp, i32, vp, vp, vp]
-    lib.kc_numeric_f64.argtypes = [vp, i64, i32, f64, f64, vp, vp, vp]
-    lib.kc_vote_i32_ex.argtypes = [vp, i64, i32, vp, i32, vp, vp, c.c_uint32, vp]
-    lib.kc_numeric_f64_ex.argtypes = [vp, i64, i32, f64, f64, vp, vp, c.c_uint32, vp]
-    lib.kc_confidence_f64.argtypes = [vp, i64, i32, vp, vp, vp]
-    lib.kc_logprob_sum_f32.argtypes = [vp, vp, i64, vp, vp]
-    lib.kc_weighted_vote_i32.argtypes = [vp, vp, i64, i32, i32, vp, vp, vp, vp, vp]
-    lib.kc_consensus_host.argtypes = [vp, i32, vp, vp, i32, i64, i32, f64, f64, vp, vp, vp, vp, c.c_int, vp]
-    lib.kc_consensus_host_i8.argtypes = lib.kc_consensus_host.argtypes
-    lib.kc_vote_i8.argtypes = [vp, i64, i32, vp, i32, vp, vp, vp]
-    lib.kc_consolidate_json.argtypes = [vp, vp, i64, i32, f64, f64, c.c_int, i32, vp, vp, vp]
-    lib.kc_consolidate_json.restype = c.c_int
-    lib.kc_vote_i32_peers.argtypes = [vp, i64, i32, vp, i32, vp, vp, i32, vp, vp]
-    lib.kc_numeric_f64_peers.argtypes = [vp, i64, i32, f64, f64, vp, vp, i32, vp, vp]
-    lib.kc_vote_i32_peers_packed.argtypes = [vp, i64, i32, vp, i32, vp, vp, vp, i32, vp, vp, vp]
-    lib.kc_vote_i32_peers.restype = lib.kc_numeric_f64_peers.restype = lib.kc_vote_i32_peers_packed.restype = c.c_int
-    lib.kc_json_plan.argtypes = [vp, vp, i64, i32, i32, c.POINTER(vp)]
-    lib.kc_json_inputs.argtypes = [vp] + [vp] * 9
-    lib.kc_json_emit.argtypes = [vp, vp, vp, vp, vp, vp, vp, vp, vp]
-    lib.kc_json_plan.restype = lib.kc_json_inputs.restype = lib.kc_json_emit.restype = c.c_int
-    lib.kc_json_free.argtypes = [vp]
-    lib.kc_json_free.restype = None
-    lib.kc_align_json.argtypes = [c.POINTER(c.c_char_p), vp, i32, f64, c.POINTER(c.c_char_p)]
-    lib.kc_align_json.restype = c.c_int
-    lib.kc_debug_similarity_json.argtypes = [c.c_char_p, c.c_char_p, c.POINTER(c.c_double)]
-    lib.kc_debug_lsap.argtypes = [i32, i32, vp, vp, vp]
-    lib.kc_debug_similarity_json.restype = lib.kc_debug_lsap.restype = c.c_int
-    lib.kc_medoid_str_host.argtypes = [vp, i64, vp, vp, i64, i32, vp, vp, c.c_int]
-    lib.kc_medoid_str_host.restype = c.c_int
-    lib.kc_medoid_str.argtypes = [vp, vp, vp, i64, i32, vp, vp, vp]
-    lib.kc_medoid_str.restype = c.c_int
-    lib.kc_medoid_str_method.argtypes = [vp, vp, vp, i64, i32, i32, vp, vp, vp]
-    lib.kc_medoid_str_method.restype = c.c_int
-    lib.kc_levenshtein.argtypes = [c.c_char_p, i32, c.c_char_p, i32]
-    lib.kc_levenshtein.restype = i32
-    lib.kc_free_strings.argtypes = [vp, i64]
-    lib.kc_free_strings.restype = None
-    lib.kc_consolidate_json_packed.argtypes = [vp, vp, i64, i32, f64, f64, c.c_int, i32, c.c_uint32, c.POINTER(vp)]
-    lib.kc_json_result_view.argtypes = [vp] + [c.POINTER(vp)] * 7 + [vp]
-    lib.kc_json_result_free.argtypes = [vp]
-    lib.kc_json_result_free.restype = None
-    lib.kc_debug_jsongpu_plan.argtypes = [vp, vp, i64, i32, c.POINTER(vp)]
-    lib.kc_debug_jsongpu_inputs.argtypes = [vp] + [vp] * 5
-    lib.kc_debug_jsongpu_emit.argtypes = [vp, vp, vp, vp] + [c.POINTER(vp)] * 4
-    lib.kc_debug_jsongpu_medoid_inputs.argtypes = [vp] + [c.POINTER(vp)] * 3 + [c.POINTER(i64)]
-    lib.kc_debug_jsongpu_set_medoid.argtypes = [vp, vp, vp]
-    lib.kc_debug_jsongpu_medoid_inputs.restype = lib.kc_debug_jsongpu_set_medoid.restype = c.c_int
-    lib.kc_debug_jsongpu_free.argtypes = [vp]
-    lib.kc_debug_jsongpu_free.restype = None
-    lib.kc_debug_parse_doubles.argtypes = [vp, vp, i64, vp, vp]
-    lib.kc_debug_float_reprs.argtypes = [vp, i64, vp, vp]
-    lib.kc_debug_round5.argtypes = [vp, i64, vp]
-    lib.kc_debug_s32_texts.argtypes = [c.c_uint64, i64, i32, i32, vp, i64, vp]
-    lib.kc_debug_s32_texts.restype = c.c_int
-    lib.kc_push_results.argtypes = [vp, vp, i64, vp, vp, i64, vp, vp, vp, i32, i32, vp, vp, i32, vp]
-    lib.kc_push_results.restype = c.c_int
-    lib.kc_vote_i32_wire.argtypes = [vp, i64, i32, vp, i32, vp, vp, vp, i32, i32, vp, vp, vp]
-    lib.kc_vote_i32_wire.restype = c.c_int
-    for name in ("kc_consolidate_json_packed", "kc_json_result_view", "kc_debug_jsongpu_plan", "kc_debug_jsongpu_inputs",
-                 "kc_debug_jsongpu_emit", "kc_debug_parse_doubles", "kc_debug_float_reprs", "kc_debug_round5"):
-        getattr(lib, name).restype = c.c_int
-    lib.kc_host_alloc.argtypes = [c.c_uint64]
-    lib.kc_host_alloc.restype = vp
-    lib.kc_host_free.argtypes = [vp]
-    lib.kc_host_free.restype = None
-    for name in ("kc_sm_count", "kc_set_device", "kc_vote_i32", "kc_numeric_f64", "kc_confidence_f64", "kc_logprob_sum_f32",
-                 "kc_weighted_vote_i32", "kc_vote_i32_ex", "kc_numeric_f64_ex", "kc_vote_i8", "kc_consensus_host_i8", "kc_vote_i8", "kc_consensus_host_i8", "kc_consolidate_json", "kc_free_strings", "kc_levenshtein", "kc_medoid_str", "kc_medoid_str_host", "kc_align_json", "kc_debug_similarity_json", "kc_debug_lsap", "kc_json_plan", "kc_json_inputs", "kc_json_emit", "kc_json_free", "kc_vote_i32_peers", "kc_numeric_f64_peers", "kc_vote_i32_peers_packed",
-                 "kc_consensus_host"):
-        getattr(lib, name).restype = c.c_int
+    for name, (restype, argtypes) in _SIGNATURES.items():
+        fn = getattr(lib, name)
+        fn.argtypes = argtypes
+        if restype is not ctypes.c_int:  # c_int is ctypes' default
+            fn.restype = restype
     _lib = lib
     return lib
 

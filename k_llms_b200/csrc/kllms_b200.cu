@@ -13,6 +13,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
+#include <type_traits>
 #include <vector>
 
 #include <nvtx3/nvToolsExt.h>
@@ -27,17 +28,7 @@
 #include "kc_vote.cuh"
 
 namespace {
-
 thread_local char g_err[512] = "";
-
-int fail(int code, const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
-
 }  // namespace
 
 int kc_fail(int code, const char *fmt, ...) {
@@ -50,12 +41,6 @@ int kc_fail(int code, const char *fmt, ...) {
 
 namespace {
 
-#define KC_CUDA(call)                                                                                         \
-    do {                                                                                                      \
-        cudaError_t e_ = (call);                                                                              \
-        if (e_ != cudaSuccess) return fail(KC_ECUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
-    } while (0)
-
 struct DeviceInfo {
     int sm_count = 0;
     int cc_major = 0;
@@ -63,19 +48,53 @@ struct DeviceInfo {
 
 int device_info(DeviceInfo &info) {
     int dev = 0;
-    KC_CUDA(cudaGetDevice(&dev));
+    KC_CUDA_I(cudaGetDevice(&dev));
     static std::mutex mu;
     static std::vector<DeviceInfo> cache;
     std::lock_guard<std::mutex> lock(mu);
     if ((int)cache.size() <= dev) cache.resize(dev + 1);
     if (cache[dev].sm_count == 0) {
-        KC_CUDA(cudaDeviceGetAttribute(&cache[dev].sm_count, cudaDevAttrMultiProcessorCount, dev));
-        KC_CUDA(cudaDeviceGetAttribute(&cache[dev].cc_major, cudaDevAttrComputeCapabilityMajor, dev));
+        KC_CUDA_I(cudaDeviceGetAttribute(&cache[dev].sm_count, cudaDevAttrMultiProcessorCount, dev));
+        KC_CUDA_I(cudaDeviceGetAttribute(&cache[dev].cc_major, cudaDevAttrComputeCapabilityMajor, dev));
     }
     info = cache[dev];
-    if (info.cc_major != 9) return fail(KC_ENODEV, "device %d has compute capability %d.x; this library is sm_90a only", dev, info.cc_major);
+    if (info.cc_major != 9) return kc_fail(KC_ENODEV, "device %d has compute capability %d.x; this library is sm_90a only", dev, info.cc_major);
     return KC_OK;
 }
+
+// grid of a grid-stride kernel: one CTA per block of work, at most 8 per SM
+int stride_grid(int64_t blocks, int &grid) {
+    DeviceInfo info;
+    int rc = device_info(info);
+    if (rc) return rc;
+    grid = (int)std::min<int64_t>(blocks, (int64_t)info.sm_count * 8);
+    return KC_OK;
+}
+
+// grid of a kernel sized by its occupancy: one CTA per block of work, at most one wave of resident CTAs
+template <typename Kernel>
+int persistent_grid(Kernel kernel, int threads, size_t smem, int64_t blocks, int &grid) {
+    DeviceInfo info;
+    int rc = device_info(info);
+    if (rc) return rc;
+    KC_CUDA_I(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int per_sm = 0;
+    KC_CUDA_I(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
+    if (per_sm < 1) return kc_fail(KC_ECUDA, "kernel does not fit on an SM (%d threads, smem %zu)", threads, smem);
+    grid = (int)std::min<int64_t>(blocks, (int64_t)info.sm_count * per_sm);
+    return KC_OK;
+}
+
+// f(std::integral_constant<int, NP>{}) for NP = n rounded up to a power of two, at least NP0 and at most KC_MAX_CANDIDATES
+template <int NP0, typename F>
+int with_pow2(int n, F &&f) {
+    if constexpr (NP0 < KC_MAX_CANDIDATES) {
+        if (n > NP0) return with_pow2<NP0 * 2>(n, f);
+    }
+    return f(std::integral_constant<int, NP0>{});
+}
+
+bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 
 // ---------------------------------------------------------------- TMA descriptor
 
@@ -90,8 +109,8 @@ int get_encode_fn(EncodeTiledFn &fn) {
     if (!cached) {
         void *p = nullptr;
         cudaDriverEntryPointQueryResult q;
-        KC_CUDA(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q));
-        if (q != cudaDriverEntryPointSuccess || !p) return fail(KC_ECUDA, "cuTensorMapEncodeTiled entry point unavailable");
+        KC_CUDA_I(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q));
+        if (q != cudaDriverEntryPointSuccess || !p) return kc_fail(KC_ECUDA, "cuTensorMapEncodeTiled entry point unavailable");
         cached = reinterpret_cast<EncodeTiledFn>(p);
     }
     fn = cached;
@@ -116,25 +135,33 @@ int make_row_tensor_map(CUtensorMap &map, const void *base, int64_t n_groups, in
     CUresult r = encode(&map, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<void *>(base), dims, strides, box, elem_strides,
                         CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r != CUDA_SUCCESS) return fail(KC_ECUDA, "cuTensorMapEncodeTiled failed: CUresult %d", (int)r);
-    return KC_OK;
-}
-
-template <typename Kernel>
-int persistent_grid(Kernel kernel, int threads, size_t smem, int64_t n_tiles, int &grid) {
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
-    KC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 0;
-    KC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
-    if (per_sm < 1) return fail(KC_ECUDA, "kernel does not fit on an SM (smem %zu)", smem);
-    grid = (int)std::min<int64_t>(n_tiles, (int64_t)info.sm_count * per_sm);  // one wave of resident CTAs
+    if (r != CUDA_SUCCESS) return kc_fail(KC_ECUDA, "cuTensorMapEncodeTiled failed: CUresult %d", (int)r);
     return KC_OK;
 }
 
 // A TMA tile coordinate is int32: launch in slabs of at most this many groups.
 constexpr int64_t kMaxGroupsPerLaunch = (int64_t)1 << 28;
+
+// A TMA front-end over G rows of `row_bytes`: tiles of 32 rows, one warp per tile, one wave of resident CTAs, in slabs of
+// at most kMaxGroupsPerLaunch rows.  A slab is a whole number of `rows_per_record` rows, so that
+// (g - g0) % n_fields == g % n_fields.  launch(grid, map, g0, gs) launches `kernel` on rows [g0, g0 + gs).
+template <typename Kernel, typename Launch>
+int launch_tma_slabs(Kernel kernel, int warps, size_t smem, const void *rows, int64_t G, int row_bytes, int64_t rows_per_record,
+                     Launch &&launch) {
+    const int64_t slab = std::max<int64_t>(rows_per_record, kMaxGroupsPerLaunch / rows_per_record * rows_per_record);
+    for (int64_t g0 = 0; g0 < G; g0 += slab) {
+        const int64_t gs = std::min(slab, G - g0);
+        CUtensorMap map;
+        int rc = make_row_tensor_map(map, static_cast<const char *>(rows) + g0 * row_bytes, gs, row_bytes, 32);
+        if (rc) return rc;
+        int grid = 0;
+        rc = persistent_grid(kernel, warps * 32, smem, ((gs + 31) / 32 + warps - 1) / warps, grid);
+        if (rc) return rc;
+        launch(grid, map, g0, gs);
+        KC_CUDA_I(cudaGetLastError());
+    }
+    return KC_OK;
+}
 
 // ---------------------------------------------------------------- K1 launchers
 
@@ -146,74 +173,50 @@ kc::FieldMap make_field_map(const int32_t *none_code, int n_fields) {
     return fm;
 }
 
-template <int N, int WARPS, int STAGES, bool HAS_NC>
-int launch_vote_tma_nc(const int32_t *codes, int64_t G, const int32_t *none_code, int n_fields, int32_t *win, uint32_t *meta,
-                       cudaStream_t st, kc::OutRoute mc) {
-    auto kernel = kc::vote_tma_kernel<N, WARPS, STAGES, HAS_NC>;
-    const size_t smem = (size_t)WARPS * STAGES * 32 * N * 4 + 1024;
-    // a slab starts on a record boundary so that (g - g0) % n_fields == g % n_fields
-    const int64_t slab = std::max<int64_t>(n_fields, kMaxGroupsPerLaunch / n_fields * n_fields);
-    for (int64_t g0 = 0; g0 < G; g0 += slab) {
-        const int64_t gs = std::min(slab, G - g0);
-        CUtensorMap map;
-        int rc = make_row_tensor_map(map, codes + g0 * N, gs, N * 4, 32);
-        if (rc) return rc;
-        int grid = 0;
-        rc = persistent_grid(kernel, WARPS * 32, smem, ((gs + 31) / 32 + WARPS - 1) / WARPS, grid);
-        if (rc) return rc;
-        kernel<<<grid, WARPS * 32, smem, st>>>(map, (uint32_t)gs, make_field_map(none_code, n_fields), win + g0, meta + g0, mc);
-        KC_CUDA(cudaGetLastError());
-    }
-    return KC_OK;
-}
-
 template <int N, int WARPS, int STAGES>
 int launch_vote_tma(const int32_t *codes, int64_t G, const int32_t *none_code, int n_fields, int32_t *win, uint32_t *meta,
                     cudaStream_t st, kc::OutRoute mc) {
-    if (none_code && n_fields < 60000)
-        return launch_vote_tma_nc<N, WARPS, STAGES, true>(codes, G, none_code, n_fields, win, meta, st, mc);
-    if (none_code) return fail(KC_EINVAL, "kc_vote_i32: more than 60000 fields with none_code is not supported");
-    return launch_vote_tma_nc<N, WARPS, STAGES, false>(codes, G, nullptr, 1, win, meta, st, mc);
+    if (none_code && n_fields >= 60000) return kc_fail(KC_EINVAL, "kc_vote_i32: more than 60000 fields with none_code is not supported");
+    const size_t smem = (size_t)WARPS * STAGES * 32 * N * 4 + 1024;
+    const kc::FieldMap fm = make_field_map(none_code, n_fields);
+    auto go = [&](auto kernel) {
+        return launch_tma_slabs(kernel, WARPS, smem, codes, G, N * 4, n_fields, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
+            kernel<<<grid, WARPS * 32, smem, st>>>(map, (uint32_t)gs, fm, win + g0, meta + g0, mc);
+        });
+    };
+    return none_code ? go(kc::vote_tma_kernel<N, WARPS, STAGES, true>) : go(kc::vote_tma_kernel<N, WARPS, STAGES, false>);
 }
 
+// VEC: n == NP, whole 16-byte rows; those up to NP = 16 request the next row before working on this one
 template <int NP, bool VEC>
 int launch_vote_direct(const int32_t *codes, int64_t G, int n, const int32_t *none_code, int n_fields, int32_t *win,
                        uint32_t *meta, cudaStream_t st, kc::OutRoute mc) {
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
+    constexpr bool kPrefetch = VEC && NP >= 4 && NP <= 16;
     const int threads = 256;
-    const int64_t blocks = (G + threads - 1) / threads;
-    const int grid = (int)std::min<int64_t>(blocks, (int64_t)info.sm_count * 8);
-    const kc::FieldMap fm = make_field_map(none_code, n_fields);
-    static const bool prefetch = [] { const char *e = getenv("KC_VOTE_PREFETCH"); return !e || e[0] != '0'; }();
-    constexpr bool kCanPrefetch = VEC && NP >= 4 && NP <= 16;
-    auto go = [&](auto kernel) -> int {
-        kernel<<<grid, threads, 0, st>>>(codes, G, n, fm, win, meta, mc);
-        KC_CUDA(cudaGetLastError());
-        return KC_OK;
-    };
-    if (kCanPrefetch && prefetch) return none_code ? go(kc::vote_direct_kernel<NP, VEC, true, kCanPrefetch>) : go(kc::vote_direct_kernel<NP, VEC, false, kCanPrefetch>);
-    return none_code ? go(kc::vote_direct_kernel<NP, VEC, true, false>) : go(kc::vote_direct_kernel<NP, VEC, false, false>);
+    int grid = 0;
+    int rc = stride_grid((G + threads - 1) / threads, grid);
+    if (rc) return rc;
+    auto kernel = none_code ? kc::vote_direct_kernel<NP, VEC, true, kPrefetch> : kc::vote_direct_kernel<NP, VEC, false, kPrefetch>;
+    kernel<<<grid, threads, 0, st>>>(codes, G, n, make_field_map(none_code, n_fields), win, meta, mc);
+    KC_CUDA_I(cudaGetLastError());
+    return KC_OK;
 }
 
-// small rows, local results: GPT consecutive groups per thread (kc::vote_multi_kernel); the remainder (< GPT groups) and every
-// routed mode go through the one-group-per-thread kernel
+// small rows, local results: GPT consecutive groups per thread (kc::vote_multi_kernel); the remainder (< GPT groups) goes
+// through the one-group-per-thread kernel
 template <int NP>
 int launch_vote_multi(const int32_t *codes, int64_t G, const int32_t *none_code, int n_fields, int32_t *win, uint32_t *meta,
                       cudaStream_t st) {
     constexpr int GPT = 16 / NP;
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
     const int64_t units = G / GPT;
     if (units > 0) {
         const int threads = 256;
-        const int grid = (int)std::min<int64_t>((units + threads - 1) / threads, (int64_t)info.sm_count * 8);
-        const kc::FieldMap fm = make_field_map(none_code, n_fields);
-        if (none_code) kc::vote_multi_kernel<NP, GPT, true><<<grid, threads, 0, st>>>(codes, units, fm, win, meta);
-        else kc::vote_multi_kernel<NP, GPT, false><<<grid, threads, 0, st>>>(codes, units, fm, win, meta);
-        KC_CUDA(cudaGetLastError());
+        int grid = 0;
+        int rc = stride_grid((units + threads - 1) / threads, grid);
+        if (rc) return rc;
+        auto kernel = none_code ? kc::vote_multi_kernel<NP, GPT, true> : kc::vote_multi_kernel<NP, GPT, false>;
+        kernel<<<grid, threads, 0, st>>>(codes, units, make_field_map(none_code, n_fields), win, meta);
+        KC_CUDA_I(cudaGetLastError());
     }
     const int64_t done = units * GPT;
     if (done < G) {  // the last few groups: their field phase continues where the units stopped
@@ -222,7 +225,7 @@ int launch_vote_multi(const int32_t *codes, int64_t G, const int32_t *none_code,
         // rotate the field table so that group `done` sees its own field first: simplest is one group per launch (< GPT of them)
         for (int64_t g = done; g < G; ++g) {
             const int f = (int)(g % n_fields);
-            rc = launch_vote_direct<NP, true>(codes + g * NP, 1, NP, none_code + f, 1, win + g, meta + g, st, local);
+            int rc = launch_vote_direct<NP, true>(codes + g * NP, 1, NP, none_code + f, 1, win + g, meta + g, st, local);
             if (rc) return rc;
         }
     }
@@ -232,128 +235,93 @@ int launch_vote_multi(const int32_t *codes, int64_t G, const int32_t *none_code,
 template <int NP, bool VEC>
 int launch_vote_i8(const int8_t *codes, int64_t G, int n, const int32_t *none_code, int n_fields, int32_t *win, uint32_t *meta,
                    cudaStream_t st) {
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
     const int threads = 256;
-    const int grid = (int)std::min<int64_t>((G + threads - 1) / threads, (int64_t)info.sm_count * 8);
-    const kc::FieldMap fm = make_field_map(none_code, n_fields);
-    if (none_code)
-        kc::vote_i8_kernel<NP, VEC, true><<<grid, threads, 0, st>>>(codes, G, n, fm, win, meta, kc::OutRoute{});
-    else
-        kc::vote_i8_kernel<NP, VEC, false><<<grid, threads, 0, st>>>(codes, G, n, fm, win, meta, kc::OutRoute{});
-    KC_CUDA(cudaGetLastError());
-    return KC_OK;
-}
-
-// ---------------------------------------------------------------- K3 launcher
-
-template <int T, int CAP>
-static int launch_logprob_tile(const float *d_logprobs, const int64_t *d_offsets, int64_t n_seq, float *d_sum, const DeviceInfo &info,
-                               void *stream) {
-    // T sequences per tile, their contiguous tokens staged in shared memory (up to CAP floats; longer tiles fall back to
-    // the warp-per-sequence loop inside the kernel)
-    auto kernel = kc::logprob_sum_tile_kernel<T, CAP>;
-    const size_t smem = (size_t)(CAP + 4) * sizeof(float);
-    KC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 1;
-    KC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, T, smem));
-    const int64_t tiles = (n_seq + T - 1) / T;
-    const int grid = (int)std::min<int64_t>(tiles, (int64_t)info.sm_count * std::max(per_sm, 1));
-    kernel<<<grid, T, smem, static_cast<cudaStream_t>(stream)>>>(d_logprobs, d_offsets, n_seq, d_sum);
-    KC_CUDA(cudaGetLastError());
+    int grid = 0;
+    int rc = stride_grid((G + threads - 1) / threads, grid);
+    if (rc) return rc;
+    auto kernel = none_code ? kc::vote_i8_kernel<NP, VEC, true> : kc::vote_i8_kernel<NP, VEC, false>;
+    kernel<<<grid, threads, 0, st>>>(codes, G, n, make_field_map(none_code, n_fields), win, meta, kc::OutRoute{});
+    KC_CUDA_I(cudaGetLastError());
     return KC_OK;
 }
 
 // ---------------------------------------------------------------- K2 launchers
 
-template <int N, int WARPS, int STAGES, int MIN_CTAS = 1>
+template <int N, int WARPS, int STAGES, int MIN_CTAS>
 int launch_numeric_tma(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
                        cudaStream_t st, kc::OutRoute mc) {
     auto kernel = kc::numeric_tma_kernel<N, WARPS, STAGES, MIN_CTAS>;
     const size_t smem = (size_t)WARPS * STAGES * 32 * N * 8 + (size_t)WARPS * 32 * N * 8 + 1024;
-    for (int64_t g0 = 0; g0 < G; g0 += kMaxGroupsPerLaunch) {
-        const int64_t gs = std::min(kMaxGroupsPerLaunch, G - g0);
-        CUtensorMap map;
-        int rc = make_row_tensor_map(map, vals + g0 * N, gs, N * 8, 32);
-        if (rc) return rc;
-        int grid = 0;
-        rc = persistent_grid(kernel, WARPS * 32, smem, ((gs + 31) / 32 + WARPS - 1) / WARPS, grid);
-        if (rc) return rc;
+    return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
         kernel<<<grid, WARPS * 32, smem, st>>>(map, gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
-        KC_CUDA(cudaGetLastError());
-    }
-    return KC_OK;
+    });
 }
 
-// fast path in front (kc::numeric_fast), general path for the groups it leaves open; KC_NUM_FAST=0 disables it
+// fast path in front (kc::numeric_fast), general path for the groups it leaves open
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
 int launch_numeric_tma_fast(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
                             cudaStream_t st, kc::OutRoute mc) {
     auto kernel = kc::numeric_tma_fast_kernel<N, WARPS, STAGES, MIN_CTAS>;
     const size_t smem = (size_t)WARPS * STAGES * 32 * N * 8 + (size_t)WARPS * 32 * N * 8 + 1024;
-    for (int64_t g0 = 0; g0 < G; g0 += kMaxGroupsPerLaunch) {
-        const int64_t gs = std::min(kMaxGroupsPerLaunch, G - g0);
-        CUtensorMap map;
-        int rc = make_row_tensor_map(map, vals + g0 * N, gs, N * 8, 32);
-        if (rc) return rc;
-        int grid = 0;
-        rc = persistent_grid(kernel, WARPS * 32, smem, ((gs + 31) / 32 + WARPS - 1) / WARPS, grid);
-        if (rc) return rc;
+    return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
         kernel<<<grid, WARPS * 32, smem, st>>>(map, vals + g0 * N, gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
-        KC_CUDA(cudaGetLastError());
-    }
-    return KC_OK;
+    });
 }
 
-static bool numeric_fast_env() {
-    static const bool on = [] { const char *e = getenv("KC_NUM_FAST"); return !(e && e[0] == '0'); }();
-    return on;
-}
-
+// PREFETCH (n == NP, NP in [4, 16]): the next row is requested before this one is worked on
 template <int NP, int T>
 int launch_numeric_direct(const double *vals, int64_t G, int n, double rel_eps, double abs_eps, double *value,
                           uint32_t *meta, cudaStream_t st, kc::OutRoute mc) {
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
-    static const bool prefetch_env = [] { const char *e = getenv("KC_NUM_PREFETCH"); return !e || e[0] != '0'; }();
-    const bool prefetch = prefetch_env && n == NP && NP >= 4 && NP <= 16;
     const size_t smem = (size_t)NP * T * 8;
     auto launch = [&](auto kernel) -> int {
-        KC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        int per_sm = 0;
-        KC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, T, smem));
-        if (per_sm < 1) return fail(KC_ECUDA, "numeric_direct_kernel<%d> does not fit", NP);
-        const int64_t blocks = (G + T - 1) / T;
-        const int grid = (int)std::min<int64_t>(blocks, (int64_t)info.sm_count * per_sm);
+        int grid = 0;
+        int rc = persistent_grid(kernel, T, smem, (G + T - 1) / T, grid);
+        if (rc) return rc;
         kernel<<<grid, T, smem, st>>>(vals, G, n, rel_eps, abs_eps, value, meta, mc);
-        KC_CUDA(cudaGetLastError());
+        KC_CUDA_I(cudaGetLastError());
         return KC_OK;
     };
     if constexpr (NP >= 4 && NP <= 16) {
-        if (prefetch) return launch(kc::numeric_direct_kernel<NP, T, true>);
+        if (n == NP) return launch(kc::numeric_direct_kernel<NP, T, true>);
     }
     return launch(kc::numeric_direct_kernel<NP, T, false>);
 }
 
-bool aligned16(const void *p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
+// the n = 2 and n = 4 case analyses (kc::numeric_pairs_kernel, kc::numeric_quads_kernel): GPT groups per thread; the last
+// < GPT groups go through the direct kernel
+template <int NP, int GPT, typename Kernel>
+int launch_numeric_units(Kernel kernel, const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
+                         cudaStream_t st, kc::OutRoute mc) {
+    const int64_t units = G / GPT;
+    if (units > 0) {
+        int grid = 0;
+        int rc = stride_grid((units + 255) / 256, grid);
+        if (rc) return rc;
+        kernel<<<grid, 256, 0, st>>>(vals, units, rel_eps, abs_eps, value, meta);
+        KC_CUDA_I(cudaGetLastError());
+    }
+    const int64_t done = units * GPT;
+    if (done == G) return KC_OK;
+    return launch_numeric_direct<NP, 128>(vals + done * NP, G - done, NP, rel_eps, abs_eps, value + done, meta + done, st, mc);
+}
 
-// A-B knobs: KC_FORCE_DIRECT=1 / KC_FORCE_TMA=1 route every n through one family of front-ends.
-bool force_tma() {
-    static const bool v = [] {
-        const char *e = getenv("KC_FORCE_TMA");
-        return e && e[0] == '1';
-    }();
-    return v;
+template <int NP>
+int launch_numeric_direct_fast(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
+                               cudaStream_t st, kc::OutRoute mc) {
+    constexpr int T = 128;
+    auto kernel = kc::numeric_direct_fast_kernel<NP, T>;
+    const size_t smem = (size_t)T * NP * 8;
+    int grid = 0;
+    int rc = persistent_grid(kernel, T, smem, (G + T - 1) / T, grid);
+    if (rc) return rc;
+    kernel<<<grid, T, smem, st>>>(vals, G, rel_eps, abs_eps, value, meta, mc);
+    KC_CUDA_I(cudaGetLastError());
+    return KC_OK;
 }
-bool force_direct() {
-    static const bool v = [] {
-        const char *e = getenv("KC_FORCE_DIRECT");
-        return e && e[0] == '1';
-    }();
-    return v;
-}
+
+// Never launched (n = 4 and 8 take other K2 kernels).  Without these two instantiations, 13 other K2 kernels, which share
+// __noinline__ helpers with them, compile to different SASS; they stay so that the K2 kernels are the ones that were timed.
+[[maybe_unused]] void *const kPinNumericSass[] = {(void *)kc::numeric_tma_kernel<4, 8, 2, 3>, (void *)kc::numeric_tma_kernel<8, 8, 2, 3>};
 
 }  // namespace
 
@@ -370,7 +338,7 @@ struct DevBuf {
         cap = 0;
         if (cudaMalloc(&p, need) != cudaSuccess) {
             cudaGetLastError();
-            return fail(KC_ENOMEM, "cudaMalloc(%zu) failed", need);
+            return kc_fail(KC_ENOMEM, "cudaMalloc(%zu) failed", need);
         }
         cap = need;
         return KC_OK;
@@ -413,12 +381,12 @@ int kc_device_count(void) {
 
 int kc_sm_count(int device) {
     int sm = 0;
-    KC_CUDA(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device));
+    KC_CUDA_I(cudaDeviceGetAttribute(&sm, cudaDevAttrMultiProcessorCount, device));
     return sm;
 }
 
 int kc_set_device(int device) {
-    KC_CUDA(cudaSetDevice(device));
+    KC_CUDA_I(cudaSetDevice(device));
     return KC_OK;
 }
 
@@ -428,13 +396,13 @@ int kc_vote_i32(const int32_t *d_codes, int64_t n_groups, int32_t n, const int32
 }
 
 static int make_peer_route(const char *who, int32_t n_peers, const int64_t *peer_delta_bytes, kc::OutRoute &r) {
-    if (n_peers < 0 || n_peers > 7) return fail(KC_EINVAL, "%s: n_peers=%d outside [0,7]", who, n_peers);
-    if (n_peers > 0 && !peer_delta_bytes) return fail(KC_EINVAL, "%s: NULL peer_delta_bytes", who);
+    if (n_peers < 0 || n_peers > 7) return kc_fail(KC_EINVAL, "%s: n_peers=%d outside [0,7]", who, n_peers);
+    if (n_peers > 0 && !peer_delta_bytes) return kc_fail(KC_EINVAL, "%s: NULL peer_delta_bytes", who);
     r = kc::OutRoute{};
     r.mode = KC_OUT_PEERS;
     r.n_peers = n_peers;
     for (int k = 0; k < n_peers; ++k) {
-        if (peer_delta_bytes[k] % 8 != 0) return fail(KC_EINVAL, "%s: peer_delta_bytes[%d] is not a multiple of 8", who, k);
+        if (peer_delta_bytes[k] % 8 != 0) return kc_fail(KC_EINVAL, "%s: peer_delta_bytes[%d] is not a multiple of 8", who, k);
         r.delta[k] = (long long)peer_delta_bytes[k];
     }
     return KC_OK;
@@ -445,7 +413,7 @@ static int vote_i32_routed(const int32_t *d_codes, int64_t n_groups, int32_t n, 
 
 int kc_vote_i32_ex(const int32_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t n_fields,
                    int32_t *d_win_code, uint32_t *d_meta, uint32_t out_mode, void *stream) {
-    if (out_mode > KC_OUT_MULTIMEM) return fail(KC_EINVAL, "kc_vote_i32_ex: unknown out_mode %u (peers: kc_vote_i32_peers)", out_mode);
+    if (out_mode > KC_OUT_MULTIMEM) return kc_fail(KC_EINVAL, "kc_vote_i32_ex: unknown out_mode %u (peers: kc_vote_i32_peers)", out_mode);
     kc::OutRoute mc{};
     mc.mode = out_mode;
     return vote_i32_routed(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, mc, stream);
@@ -462,7 +430,7 @@ int kc_vote_i32_peers(const int32_t *d_codes, int64_t n_groups, int32_t n, const
 int kc_vote_i32_peers_packed(const int32_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t n_fields,
                              int32_t *d_win_code, uint32_t *d_meta, uint32_t *d_packed, int32_t n_peers,
                              const int64_t *peer_delta_bytes, uint32_t *d_overflow, void *stream) {
-    if (!d_packed || !d_overflow) return fail(KC_EINVAL, "kc_vote_i32_peers_packed: NULL d_packed / d_overflow");
+    if (!d_packed || !d_overflow) return kc_fail(KC_EINVAL, "kc_vote_i32_peers_packed: NULL d_packed / d_overflow");
     kc::OutRoute mc;
     int rc = make_peer_route("kc_vote_i32_peers_packed", n_peers, peer_delta_bytes, mc);
     if (rc) return rc;
@@ -474,55 +442,43 @@ int kc_vote_i32_peers_packed(const int32_t *d_codes, int64_t n_groups, int32_t n
 
 static int vote_i32_routed(const int32_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t n_fields,
                            int32_t *d_win_code, uint32_t *d_meta, kc::OutRoute mc, void *stream) {
-    if (n < 1 || n > KC_MAX_CANDIDATES) return fail(KC_EINVAL, "kc_vote_i32: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
-    if (n_groups < 0) return fail(KC_EINVAL, "kc_vote_i32: negative n_groups");
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_vote_i32: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
+    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_vote_i32: negative n_groups");
     if (n_groups == 0) return KC_OK;
-    if (!d_codes || !d_win_code || !d_meta) return fail(KC_EINVAL, "kc_vote_i32: NULL buffer");
-    if (d_none_code && n_fields < 1) return fail(KC_EINVAL, "kc_vote_i32: none_code given but n_fields=%d", n_fields);
+    if (!d_codes || !d_win_code || !d_meta) return kc_fail(KC_EINVAL, "kc_vote_i32: NULL buffer");
+    if (d_none_code && n_fields < 1) return kc_fail(KC_EINVAL, "kc_vote_i32: none_code given but n_fields=%d", n_fields);
     if (!d_none_code) n_fields = 1;
-    if (!aligned16(d_codes)) return fail(KC_EINVAL, "kc_vote_i32: d_codes must be 16-byte aligned");
+    if (!aligned16(d_codes)) return kc_fail(KC_EINVAL, "kc_vote_i32: d_codes must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // measured on H100 SXM (400 W, 1M x 24 fields): the direct front-end wins up to n = 16 (0.59 vs 0.63 ms at n = 16), the
     // TMA pipeline from n = 32 (1.12 vs 1.30 ms at n = 32)
-    static const bool multi = [] { const char *e = getenv("KC_VOTE_MULTI"); return !e || e[0] != '0'; }();
-    if (multi && mc.local() && !force_tma() && (n == 2 || n == 4 || n == 8)) {
-        if (n == 2) return launch_vote_multi<2>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st);
-        if (n == 4) return launch_vote_multi<4>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st);
-        return launch_vote_multi<8>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st);
-    }
-    if (force_direct() || (!force_tma() && n <= 16)) {
+    if (mc.local()) {  // the multi-group kernel only has local stores
         switch (n) {
-            case 1: return launch_vote_direct<1, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-            case 2: return launch_vote_direct<2, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-            case 4: return launch_vote_direct<4, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-            case 8: return launch_vote_direct<8, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-            case 16: return launch_vote_direct<16, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-            case 32: return launch_vote_direct<32, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-            case 64: return launch_vote_direct<64, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
+            case 2: return launch_vote_multi<2>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st);
+            case 4: return launch_vote_multi<4>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st);
+            case 8: return launch_vote_multi<8>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st);
             default: break;
         }
-    } else
+    }
     switch (n) {
         case 1: return launch_vote_direct<1, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
         case 2: return launch_vote_direct<2, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
         case 4: return launch_vote_direct<4, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-        case 8: return launch_vote_tma<8, 8, 4>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-        case 16: return launch_vote_tma<16, 8, 4>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st, mc);  // KC_FORCE_TMA only
+        case 8: return launch_vote_direct<8, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
+        case 16: return launch_vote_direct<16, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
         case 32: return launch_vote_tma<32, 8, 2>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st, mc);
         case 64: return launch_vote_tma<64, 4, 2>(d_codes, n_groups, d_none_code, n_fields, d_win_code, d_meta, st, mc);
         default: break;
     }
-    if (n < 4) return launch_vote_direct<4, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-    if (n < 8) return launch_vote_direct<8, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-    if (n < 16) return launch_vote_direct<16, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-    if (n < 32) return launch_vote_direct<32, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
-    return launch_vote_direct<64, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
+    return with_pow2<4>(n, [&](auto np) {
+        return launch_vote_direct<decltype(np)::value, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, mc);
+    });
 }
 
 int kc_vote_i32_wire(const int32_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t n_fields,
                      int32_t *d_win_code, uint32_t *d_meta, void *d_wire_words, int32_t wide, int32_t n_peers,
                      const int64_t *peer_delta_bytes, uint32_t *d_overflow, void *stream) {
-    if (!d_wire_words || !d_overflow) return fail(KC_EINVAL, "kc_vote_i32_wire: NULL d_wire_words / d_overflow");
+    if (!d_wire_words || !d_overflow) return kc_fail(KC_EINVAL, "kc_vote_i32_wire: NULL d_wire_words / d_overflow");
     kc::OutRoute mc{};
     if (n_peers) {
         int rc = make_peer_route("kc_vote_i32_wire", n_peers, peer_delta_bytes, mc);
@@ -538,14 +494,14 @@ int kc_vote_i32_wire(const int32_t *d_codes, int64_t n_groups, int32_t n, const 
 static int fill_push_args(kc::PushArgs &a, const int32_t *d_win_code, const uint32_t *d_vote_meta, int64_t n_vote_groups, const double *d_value,
                           const uint32_t *d_num_meta, int64_t n_num_groups, void *d_wire_votes, void *d_wire_value, void *d_wire_num_meta,
                           int32_t wide, int32_t n_peers, const int64_t *peer_delta_bytes, uint32_t *d_overflow) {
-    if (n_vote_groups < 0 || n_num_groups < 0) return fail(KC_EINVAL, "kc_push_results: negative size");
-    if (n_vote_groups % 8 || n_num_groups % 8) return fail(KC_EINVAL, "kc_push_results: group counts must be multiples of 8 (whole 16-byte vectors)");
-    if (n_peers < 0 || n_peers > 7 || (n_peers && !peer_delta_bytes)) return fail(KC_EINVAL, "kc_push_results: n_peers=%d outside [0,7] or NULL deltas", n_peers);
+    if (n_vote_groups < 0 || n_num_groups < 0) return kc_fail(KC_EINVAL, "kc_push_results: negative size");
+    if (n_vote_groups % 8 || n_num_groups % 8) return kc_fail(KC_EINVAL, "kc_push_results: group counts must be multiples of 8 (whole 16-byte vectors)");
+    if (n_peers < 0 || n_peers > 7 || (n_peers && !peer_delta_bytes)) return kc_fail(KC_EINVAL, "kc_push_results: n_peers=%d outside [0,7] or NULL deltas", n_peers);
     if ((n_vote_groups && (((!d_win_code) != (!d_vote_meta)) || !d_wire_votes)) || (n_num_groups && (!d_value || !d_num_meta || !d_wire_value || !d_wire_num_meta)))
-        return fail(KC_EINVAL, "kc_push_results: NULL buffer");
+        return kc_fail(KC_EINVAL, "kc_push_results: NULL buffer");
     for (const void *p : {(const void *)d_win_code, (const void *)d_vote_meta, (const void *)d_value, (const void *)d_num_meta,
                           (const void *)d_wire_votes, (const void *)d_wire_value, (const void *)d_wire_num_meta})
-        if (!aligned16(p)) return fail(KC_EINVAL, "kc_push_results: buffers must be 16-byte aligned");
+        if (!aligned16(p)) return kc_fail(KC_EINVAL, "kc_push_results: buffers must be 16-byte aligned");
     a = kc::PushArgs{};
     a.win = d_win_code;
     a.vmeta = d_vote_meta;
@@ -558,7 +514,7 @@ static int fill_push_args(kc::PushArgs &a, const int32_t *d_win_code, const uint
     a.wire_nmeta = static_cast<uint8_t *>(d_wire_num_meta);
     a.n_peers = n_peers;
     for (int k = 0; k < n_peers; ++k) {
-        if (peer_delta_bytes[k] % 16 != 0) return fail(KC_EINVAL, "kc_push_results: peer_delta_bytes[%d] is not a multiple of 16", k);
+        if (peer_delta_bytes[k] % 16 != 0) return kc_fail(KC_EINVAL, "kc_push_results: peer_delta_bytes[%d] is not a multiple of 16", k);
         a.delta[k] = (long long)peer_delta_bytes[k];
     }
     a.wide = wide ? 1 : 0;
@@ -581,33 +537,26 @@ int kc_push_results(const int32_t *d_win_code, const uint32_t *d_vote_meta, int6
     int64_t grid = (units + 255) / 256;
     grid = std::min<int64_t>(grid, max_ctas > 0 ? max_ctas : info.sm_count * 2);
     kc::push_kernel<<<(int)std::max<int64_t>(grid, 1), 256, 0, static_cast<cudaStream_t>(stream)>>>(a);
-    KC_CUDA(cudaGetLastError());
+    KC_CUDA_I(cudaGetLastError());
     return KC_OK;
 }
 
 int kc_vote_i8(const int8_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t n_fields,
                int32_t *d_win_code, uint32_t *d_meta, void *stream) {
-    if (n < 1 || n > KC_MAX_CANDIDATES) return fail(KC_EINVAL, "kc_vote_i8: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
-    if (n_groups < 0) return fail(KC_EINVAL, "kc_vote_i8: negative n_groups");
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_vote_i8: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
+    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_vote_i8: negative n_groups");
     if (n_groups == 0) return KC_OK;
-    if (!d_codes || !d_win_code || !d_meta) return fail(KC_EINVAL, "kc_vote_i8: NULL buffer");
-    if (d_none_code && n_fields < 1) return fail(KC_EINVAL, "kc_vote_i8: none_code given but n_fields=%d", n_fields);
+    if (!d_codes || !d_win_code || !d_meta) return kc_fail(KC_EINVAL, "kc_vote_i8: NULL buffer");
+    if (d_none_code && n_fields < 1) return kc_fail(KC_EINVAL, "kc_vote_i8: none_code given but n_fields=%d", n_fields);
     if (!d_none_code) n_fields = 1;
-    if (!aligned16(d_codes)) return fail(KC_EINVAL, "kc_vote_i8: d_codes must be 16-byte aligned");
+    if (!aligned16(d_codes)) return kc_fail(KC_EINVAL, "kc_vote_i8: d_codes must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    switch (n) {
-        case 4: return launch_vote_i8<4, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-        case 8: return launch_vote_i8<8, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-        case 16: return launch_vote_i8<16, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-        case 32: return launch_vote_i8<32, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-        case 64: return launch_vote_i8<64, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-        default: break;
-    }
-    if (n < 4) return launch_vote_i8<4, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-    if (n < 8) return launch_vote_i8<8, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-    if (n < 16) return launch_vote_i8<16, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-    if (n < 32) return launch_vote_i8<32, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-    return launch_vote_i8<64, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
+    // n a power of two from 4 on: whole 16-byte rows; any other n: the next power of two, cells beyond n absent
+    return with_pow2<4>(n, [&](auto np) {
+        constexpr int NP = decltype(np)::value;
+        if (n == NP) return launch_vote_i8<NP, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
+        return launch_vote_i8<NP, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
+    });
 }
 
 int kc_numeric_f64(const double *d_vals, int64_t n_groups, int32_t n, double rel_eps, double abs_eps, double *d_value,
@@ -620,7 +569,7 @@ static int numeric_f64_routed(const double *d_vals, int64_t n_groups, int32_t n,
 
 int kc_numeric_f64_ex(const double *d_vals, int64_t n_groups, int32_t n, double rel_eps, double abs_eps, double *d_value,
                       uint32_t *d_meta, uint32_t out_mode, void *stream) {
-    if (out_mode > KC_OUT_MULTIMEM) return fail(KC_EINVAL, "kc_numeric_f64_ex: unknown out_mode %u (peers: kc_numeric_f64_peers)", out_mode);
+    if (out_mode > KC_OUT_MULTIMEM) return kc_fail(KC_EINVAL, "kc_numeric_f64_ex: unknown out_mode %u (peers: kc_numeric_f64_peers)", out_mode);
     kc::OutRoute mc{};
     mc.mode = out_mode;
     return numeric_f64_routed(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, mc, stream);
@@ -636,223 +585,146 @@ int kc_numeric_f64_peers(const double *d_vals, int64_t n_groups, int32_t n, doub
 
 static int numeric_f64_routed(const double *d_vals, int64_t n_groups, int32_t n, double rel_eps, double abs_eps, double *d_value,
                               uint32_t *d_meta, kc::OutRoute mc, void *stream) {
-    if (n < 1 || n > KC_MAX_CANDIDATES) return fail(KC_EINVAL, "kc_numeric_f64: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
-    if (n_groups < 0) return fail(KC_EINVAL, "kc_numeric_f64: negative n_groups");
-    if (!(rel_eps >= 0.0) || !(abs_eps >= 0.0)) return fail(KC_EINVAL, "kc_numeric_f64: rel_eps/abs_eps must be >= 0");
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_numeric_f64: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
+    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_numeric_f64: negative n_groups");
+    if (!(rel_eps >= 0.0) || !(abs_eps >= 0.0)) return kc_fail(KC_EINVAL, "kc_numeric_f64: rel_eps/abs_eps must be >= 0");
     if (n_groups == 0) return KC_OK;
-    if (!d_vals || !d_value || !d_meta) return fail(KC_EINVAL, "kc_numeric_f64: NULL buffer");
-    if (!aligned16(d_vals)) return fail(KC_EINVAL, "kc_numeric_f64: d_vals must be 16-byte aligned");
+    if (!d_vals || !d_value || !d_meta) return kc_fail(KC_EINVAL, "kc_numeric_f64: NULL buffer");
+    if (!aligned16(d_vals)) return kc_fail(KC_EINVAL, "kc_numeric_f64: d_vals must be 16-byte aligned");
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // The fast kernels store a group's result when it is decided — most lanes at once, the deferred ones later and
-    // scattered.  Local stores do not care; multicast stores do (the general kernel's whole-warp
-    // stores use the link better than the fast kernel's), and a fused step is NVLink-bound anyway.
-    const bool numeric_fast = numeric_fast_env() && mc.local();  // the fast kernels only have local stores
     // measured on H100 SXM (400 W, 1M x 8 fields): the TMA pipeline wins from n = 16 (0.43 vs 0.46 ms at n = 16, 0.83 vs
     // 1.03 at n = 32, 2.55 vs 2.78 at n = 64); direct at n <= 8 (tiles too small to prefetch far enough)
-    if (!force_direct() && (force_tma() || n == 16 || n == 32 || n == 64))
+    if (mc.local()) {
+        // The fast and small-n kernels only have local stores.  The fast kernels store a group's result when it is decided —
+        // most lanes at once, the deferred ones later and scattered.  Local stores do not care; multicast stores do (the
+        // general kernel's whole-warp stores use the link better than the fast kernel's), and a fused step is NVLink-bound anyway.
         switch (n) {
-            case 4: return launch_numeric_tma<4, 8, 2, 3>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 8: return launch_numeric_tma<8, 8, 2, 3>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 16:
-                if (numeric_fast) return launch_numeric_tma_fast<16, 4, 1, 6>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-                return launch_numeric_tma<16, 4, 1, 7>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 32:
-                if (numeric_fast) return launch_numeric_tma_fast<32, 4, 1, 4>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-                return launch_numeric_tma<32, 4, 1, 4>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 64: return launch_numeric_tma<64, 2, 1, 3>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 2: return launch_numeric_units<2, 4>(kc::numeric_pairs_kernel, d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 4: return launch_numeric_units<4, 2>(kc::numeric_quads_kernel, d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 8: return launch_numeric_direct_fast<8>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 16: return launch_numeric_tma_fast<16, 4, 1, 6>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 32: return launch_numeric_tma_fast<32, 4, 1, 4>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
             default: break;
         }
-    static const bool quads = [] { const char *e = getenv("KC_NUM_QUADS"); return !e || e[0] != '0'; }();
-    if (n == 4 && quads && mc.local() && !force_direct() && !force_tma()) {  // the n = 4 pattern analysis, two groups per thread
-        DeviceInfo info;
-        int rc = device_info(info);
-        if (rc) return rc;
-        const int64_t units = n_groups / 2;
-        if (units > 0) {
-            const int grid = (int)std::min<int64_t>((units + 255) / 256, (int64_t)info.sm_count * 8);
-            kc::numeric_quads_kernel<<<grid, 256, 0, st>>>(d_vals, units, rel_eps, abs_eps, d_value, d_meta);
-            KC_CUDA(cudaGetLastError());
-        }
-        const int64_t done = units * 2;
-        if (done == n_groups) return KC_OK;
-        return launch_numeric_direct<4, 128>(d_vals + done * 4, n_groups - done, n, rel_eps, abs_eps, d_value + done, d_meta + done, st, mc);
     }
-    if (numeric_fast && !force_direct() && (n == 8 || n == 4)) {
-        auto launch_fast = [&](auto kernel, int NP) -> int {
-            DeviceInfo info;
-            int rc = device_info(info);
-            if (rc) return rc;
-            const int T = 128;
-            const size_t smem = (size_t)T * NP * 8;
-            int per_sm = 0;
-            KC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, T, smem));
-            if (per_sm < 1) return fail(KC_ECUDA, "numeric_direct_fast_kernel<%d> does not fit", NP);
-            const int64_t want = (n_groups + T - 1) / T;
-            const int grid = (int)std::min<int64_t>(want, (int64_t)info.sm_count * per_sm);
-            kernel<<<grid, T, smem, st>>>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, mc);
-            KC_CUDA(cudaGetLastError());
-            return KC_OK;
-        };
-        if (n == 8) return launch_fast(kc::numeric_direct_fast_kernel<8, 128>, 8);
-        return launch_fast(kc::numeric_direct_fast_kernel<4, 128>, 4);
+    switch (n) {
+        case 16: return launch_numeric_tma<16, 4, 1, 7>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+        case 32: return launch_numeric_tma<32, 4, 1, 4>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+        case 64: return launch_numeric_tma<64, 2, 1, 3>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+        default: break;
     }
-    static const bool pairs = [] { const char *e = getenv("KC_NUM_PAIRS"); return !e || e[0] != '0'; }();
-    if (n == 2 && pairs && mc.local() && !force_direct()) {  // the n = 2 case analysis, four groups per thread; the last < 4 groups below
-        DeviceInfo info;
-        int rc = device_info(info);
-        if (rc) return rc;
-        const int64_t units = n_groups / 4;
-        if (units > 0) {
-            const int grid = (int)std::min<int64_t>((units + 255) / 256, (int64_t)info.sm_count * 8);
-            kc::numeric_pairs_kernel<<<grid, 256, 0, st>>>(d_vals, units, rel_eps, abs_eps, d_value, d_meta);
-            KC_CUDA(cudaGetLastError());
-        }
-        const int64_t done = units * 4;
-        if (done == n_groups) return KC_OK;
-        return launch_numeric_direct<2, 128>(d_vals + done * 2, n_groups - done, n, rel_eps, abs_eps, d_value + done, d_meta + done, st, mc);
-    }
-    if (n <= 2) return launch_numeric_direct<2, 128>(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, st, mc);
-    if (n <= 4) return launch_numeric_direct<4, 128>(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, st, mc);
-    if (n <= 8) return launch_numeric_direct<8, 128>(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, st, mc);
-    if (n <= 16) return launch_numeric_direct<16, 128>(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, st, mc);
-    if (n <= 32) return launch_numeric_direct<32, 128>(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, st, mc);
-    return launch_numeric_direct<64, 64>(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, st, mc);
+    return with_pow2<2>(n, [&](auto np) {
+        constexpr int NP = decltype(np)::value;
+        return launch_numeric_direct<NP, NP == 64 ? 64 : 128>(d_vals, n_groups, n, rel_eps, abs_eps, d_value, d_meta, st, mc);
+    });
 }
 
 int kc_confidence_f64(const uint32_t *d_meta, int64_t n_groups, int32_t numeric, const double *d_pvf, double *d_conf,
                       void *stream) {
-    if (n_groups < 0) return fail(KC_EINVAL, "kc_confidence_f64: negative n_groups");
+    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_confidence_f64: negative n_groups");
     if (n_groups == 0) return KC_OK;
-    if (!d_meta || !d_conf) return fail(KC_EINVAL, "kc_confidence_f64: NULL buffer");
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
+    if (!d_meta || !d_conf) return kc_fail(KC_EINVAL, "kc_confidence_f64: NULL buffer");
     const int threads = 256;
-    const int grid = (int)std::min<int64_t>((n_groups + threads - 1) / threads, (int64_t)info.sm_count * 8);
+    int grid = 0;
+    int rc = stride_grid((n_groups + threads - 1) / threads, grid);
+    if (rc) return rc;
     kc::confidence_kernel<<<grid, threads, 0, static_cast<cudaStream_t>(stream)>>>(d_meta, n_groups, numeric != 0, d_pvf, d_conf);
-    KC_CUDA(cudaGetLastError());
+    KC_CUDA_I(cudaGetLastError());
     return KC_OK;
 }
 
 int kc_logprob_sum_f32(const float *d_logprobs, const int64_t *d_offsets, int64_t n_seq, float *d_sum, void *stream) {
-    if (n_seq < 0) return fail(KC_EINVAL, "kc_logprob_sum_f32: negative n_seq");
+    if (n_seq < 0) return kc_fail(KC_EINVAL, "kc_logprob_sum_f32: negative n_seq");
     if (n_seq == 0) return KC_OK;
-    if (!d_offsets || !d_sum) return fail(KC_EINVAL, "kc_logprob_sum_f32: NULL buffer");
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
-    static const bool staged = [] { const char *e = getenv("KC_K3_STAGED"); return !e || e[0] != '0'; }();
-    if (staged && n_seq >= 4096 && aligned16(d_logprobs)) {
-        // 64 sequences per tile, 24 KB of staged tokens (chosen from {128/48 KB, 64/24 KB, 64/16 KB, 32/12 KB}; 32/12 KB falls
-        // back from 96 tokens per sequence on; not re-timed on H100)
-        return launch_logprob_tile<64, 6 * 1024>(d_logprobs, d_offsets, n_seq, d_sum, info, stream);
+    if (!d_offsets || !d_sum) return kc_fail(KC_EINVAL, "kc_logprob_sum_f32: NULL buffer");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    int grid = 0;
+    if (n_seq >= 4096 && aligned16(d_logprobs)) {
+        // T sequences per tile, their contiguous tokens staged in shared memory (up to CAP floats; longer tiles fall back to
+        // the warp-per-sequence loop inside the kernel).  64 sequences per tile, 24 KB of staged tokens (chosen from
+        // {128/48 KB, 64/24 KB, 64/16 KB, 32/12 KB}; 32/12 KB falls back from 96 tokens per sequence on; not re-timed on H100)
+        constexpr int T = 64, CAP = 6 * 1024;
+        auto kernel = kc::logprob_sum_tile_kernel<T, CAP>;
+        const size_t smem = (size_t)(CAP + 4) * sizeof(float);
+        int rc = persistent_grid(kernel, T, smem, (n_seq + T - 1) / T, grid);
+        if (rc) return rc;
+        kernel<<<grid, T, smem, st>>>(d_logprobs, d_offsets, n_seq, d_sum);
+    } else {
+        int rc = stride_grid((n_seq + 7) / 8, grid);  // 8 warps, one sequence per warp per iteration
+        if (rc) return rc;
+        kc::logprob_sum_kernel<<<grid, 256, 0, st>>>(d_logprobs, d_offsets, n_seq, d_sum);
     }
-    const int threads = 256;  // 8 warps, one sequence per warp per iteration
-    const int64_t warps = n_seq;
-    const int grid = (int)std::min<int64_t>((warps + 7) / 8, (int64_t)info.sm_count * 8);
-    kc::logprob_sum_kernel<<<grid, threads, 0, static_cast<cudaStream_t>(stream)>>>(d_logprobs, d_offsets, n_seq, d_sum);
-    KC_CUDA(cudaGetLastError());
+    KC_CUDA_I(cudaGetLastError());
     return KC_OK;
 }
 
 int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int64_t n_records, int32_t n_fields,
                          int32_t n, const int32_t *d_none_code, int32_t *d_win_code, uint32_t *d_meta, float *d_weight,
                          void *stream) {
-    if (n < 1 || n > KC_MAX_CANDIDATES) return fail(KC_EINVAL, "kc_weighted_vote_i32: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
-    if (n_records < 0 || n_fields < 1) return fail(KC_EINVAL, "kc_weighted_vote_i32: bad sizes");
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_weighted_vote_i32: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
+    if (n_records < 0 || n_fields < 1) return kc_fail(KC_EINVAL, "kc_weighted_vote_i32: bad sizes");
     if (n_records == 0) return KC_OK;
-    if (!d_codes || !d_seq_logprob || !d_win_code || !d_meta || !d_weight) return fail(KC_EINVAL, "kc_weighted_vote_i32: NULL buffer");
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
+    if (!d_codes || !d_seq_logprob || !d_win_code || !d_meta || !d_weight) return kc_fail(KC_EINVAL, "kc_weighted_vote_i32: NULL buffer");
     const int64_t G = n_records * n_fields;
-    const int threads = 128;
-    const int grid = (int)std::min<int64_t>((G + threads - 1) / threads, (int64_t)info.sm_count * 8);
     const kc::FieldMap fm = make_field_map(d_none_code, n_fields);
+    const bool has_nc = d_none_code != nullptr;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    static const bool per_record = [] { const char *e = getenv("KC_K3B_REC"); return !e || e[0] != '0'; }();
-    static const bool use_tma = [] { const char *e = getenv("KC_K3B_TMA"); return !e || e[0] != '0'; }();
-    if (per_record && use_tma && (n == 32 || n == 64) && n_fields < 60000) {  // rows through K1's warp-private TMA pipelines
-        auto launch_tma = [&](auto kernel, int N, int WARPS, int STAGES) -> int {
-            const int rec_cap = std::min(32, 31 / n_fields + 2);  // records a tile of 32 groups can span
-            const size_t smem = (size_t)WARPS * STAGES * 32 * N * 4 + 1024 + (size_t)WARPS * rec_cap * (N + 1) * 4;
-            const int64_t slab = std::max<int64_t>(n_fields, kMaxGroupsPerLaunch / n_fields * n_fields);  // slabs start on record boundaries
-            for (int64_t g0 = 0; g0 < G; g0 += slab) {
-                const int64_t gs = std::min(slab, G - g0);
-                CUtensorMap map;
-                int rc2 = make_row_tensor_map(map, d_codes + g0 * N, gs, N * 4, 32);
-                if (rc2) return rc2;
-                int grid2 = 0;
-                rc2 = persistent_grid(kernel, WARPS * 32, smem, ((gs + 31) / 32 + WARPS - 1) / WARPS, grid2);
-                if (rc2) return rc2;
-                const uint64_t inv_fields = n_fields > 1 ? ~uint64_t(0) / (uint64_t)n_fields + 1 : 0;
-                kernel<<<grid2, WARPS * 32, smem, st>>>(map, d_seq_logprob + (g0 / n_fields) * N, (uint32_t)gs, fm, d_none_code != nullptr, rec_cap,
-                                                        inv_fields, d_win_code + g0, d_meta + g0, d_weight + g0);
-                KC_CUDA(cudaGetLastError());
-            }
-            return KC_OK;
+    if ((n == 32 || n == 64) && n_fields < 60000) {  // rows through K1's warp-private TMA pipelines
+        const int rec_cap = std::min(32, 31 / n_fields + 2);  // records a tile of 32 groups can span
+        const uint64_t inv_fields = n_fields > 1 ? ~uint64_t(0) / (uint64_t)n_fields + 1 : 0;
+        // weights: `wrow` floats per record, from `wts`
+        auto launch_tma = [&](auto kernel, int N, int warps, size_t smem, const float *wts, int wrow) {
+            return launch_tma_slabs(kernel, warps, smem, d_codes, G, N * 4, n_fields, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
+                kernel<<<grid, warps * 32, smem, st>>>(map, wts + (g0 / n_fields) * wrow, (uint32_t)gs, fm, has_nc, rec_cap, inv_fields,
+                                                       d_win_code + g0, d_meta + g0, d_weight + g0);
+            });
         };
-        static const bool rows = [] { const char *e = getenv("KC_K3B_ROWS"); return !e || e[0] != '0'; }();
-        const int rec_cap0 = std::min(32, 31 / n_fields + 2);
-        if (rows && n == 32 && rec_cap0 <= 8) {  // weights by a pre-pass, fetched per tile by a bulk copy (n_fields >= 6; n = 32 only)
-            auto launch_rows = [&](auto pre_kernel, auto kernel, int N, int WARPS, int STAGES) -> int {
-                const int WROW = N + 4;
-                float *d_rows = nullptr;
-                KC_CUDA(cudaMallocAsync(reinterpret_cast<void **>(&d_rows), (size_t)n_records * WROW * 4, st));
-                const int pre_grid = (int)std::min<int64_t>((n_records + 7) / 8, (int64_t)info.sm_count * 8);
-                pre_kernel<<<pre_grid, 256, 0, st>>>(d_seq_logprob, n_records, d_rows);
-                int rc2 = cudaGetLastError() == cudaSuccess ? KC_OK : fail(KC_ECUDA, "kc_weighted_vote_i32: weight_rows_kernel launch failed");
-                const size_t smem = (size_t)WARPS * STAGES * 32 * N * 4 + 1024 + (size_t)WARPS * (STAGES + 1) * rec_cap0 * WROW * 4;
-                const int64_t slab = std::max<int64_t>(n_fields, kMaxGroupsPerLaunch / n_fields * n_fields);
-                for (int64_t g0 = 0; g0 < G && !rc2; g0 += slab) {
-                    const int64_t gs = std::min(slab, G - g0);
-                    CUtensorMap map;
-                    rc2 = make_row_tensor_map(map, d_codes + g0 * N, gs, N * 4, 32);
-                    int grid2 = 0;
-                    if (!rc2) rc2 = persistent_grid(kernel, WARPS * 32, smem, ((gs + 31) / 32 + WARPS - 1) / WARPS, grid2);
-                    if (rc2) break;
-                    const uint64_t inv_fields = n_fields > 1 ? ~uint64_t(0) / (uint64_t)n_fields + 1 : 0;
-                    kernel<<<grid2, WARPS * 32, smem, st>>>(map, d_rows + (g0 / n_fields) * WROW, (uint32_t)gs, fm, d_none_code != nullptr, rec_cap0,
-                                                            inv_fields, d_win_code + g0, d_meta + g0, d_weight + g0);
-                    if (cudaGetLastError() != cudaSuccess) rc2 = fail(KC_ECUDA, "kc_weighted_vote_i32: launch failed");
-                }
-                cudaFreeAsync(d_rows, st);
-                return rc2;
-            };
-            return launch_rows(kc::weight_rows_kernel<32>, kc::weighted_vote_rows_kernel<32, 8, 2, 3>, 32, 8, 2);
+        if (n == 32 && rec_cap <= 8) {  // weights by a pre-pass, fetched per tile by a bulk copy (n_fields >= 6; n = 32 only)
+            constexpr int N = 32, WARPS = 8, STAGES = 2, WROW = N + 4;
+            int pre_grid = 0;
+            int rc = stride_grid((n_records + 7) / 8, pre_grid);
+            if (rc) return rc;
+            float *d_rows = nullptr;
+            KC_CUDA_I(cudaMallocAsync(reinterpret_cast<void **>(&d_rows), (size_t)n_records * WROW * 4, st));
+            kc::weight_rows_kernel<N><<<pre_grid, 256, 0, st>>>(d_seq_logprob, n_records, d_rows);
+            rc = cudaGetLastError() == cudaSuccess ? KC_OK : kc_fail(KC_ECUDA, "kc_weighted_vote_i32: weight_rows_kernel launch failed");
+            const size_t smem = (size_t)WARPS * STAGES * 32 * N * 4 + 1024 + (size_t)WARPS * (STAGES + 1) * rec_cap * WROW * 4;
+            if (!rc) rc = launch_tma(kc::weighted_vote_rows_kernel<N, WARPS, STAGES, 3>, N, WARPS, smem, d_rows, WROW);
+            cudaFreeAsync(d_rows, st);
+            return rc;
         }
         // n = 32 with 3 CTAs / SM (80 registers) and the logprobs requested a tile ahead; n = 64 (2 x the registers per row)
         // without the prefetch (not re-timed on H100)
-        if (n == 32) return launch_tma(kc::weighted_vote_tma_kernel<32, 8, 2, 3, true>, 32, 8, 2);
-        return launch_tma(kc::weighted_vote_tma_kernel<64, 4, 2, 3, false>, 64, 4, 2);
+        auto tma_smem = [&](int N, int warps, int stages) { return (size_t)warps * stages * 32 * N * 4 + 1024 + (size_t)warps * rec_cap * (N + 1) * 4; };
+        if (n == 32) return launch_tma(kc::weighted_vote_tma_kernel<32, 8, 2, 3, true>, 32, 8, tma_smem(32, 8, 2), d_seq_logprob, 32);
+        return launch_tma(kc::weighted_vote_tma_kernel<64, 4, 2, 3, false>, 64, 4, tma_smem(64, 4, 2), d_seq_logprob, 64);
     }
-    if (per_record && n >= 8) {  // weights once per record, one row per thread straight from global memory
-        const int max_recs = threads / n_fields + 2;
-        auto launch = [&](auto kernel, int NP) -> int {
-            const size_t smem = (size_t)max_recs * NP * 4;  // the candidate weights of the tile's records
-            KC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            int per_sm = 1;
-            KC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, threads, smem));
-            const int g2 = (int)std::min<int64_t>((G + threads - 1) / threads, (int64_t)info.sm_count * std::max(per_sm, 1));
-            kernel<<<g2, threads, smem, st>>>(d_codes, d_seq_logprob, G, n, fm, d_none_code != nullptr, d_win_code, d_meta, d_weight);
-            KC_CUDA(cudaGetLastError());
-            return KC_OK;
-        };
-        if (n <= 8) return launch(kc::weighted_vote_rec_kernel<8, 128>, 8);
-        if (n <= 16) return launch(kc::weighted_vote_rec_kernel<16, 128>, 16);
-        if (n <= 32) return launch(kc::weighted_vote_rec_kernel<32, 128>, 32);
-        return launch(kc::weighted_vote_rec_kernel<64, 128>, 64);
+    // n < 8: one group per thread, weights computed per group; faster there than the per-record kernel below (H100 SXM,
+    // 700 W, 256 K records x 24 fields: 0.07 against 0.16 ms at n = 2, 0.11 against 0.16 ms at n = 4)
+    if (n < 8) {
+        const int threads = 128;
+        int grid = 0;
+        int rc = stride_grid((G + threads - 1) / threads, grid);
+        if (rc) return rc;
+        auto kernel = n <= 2 ? kc::weighted_vote_kernel<2> : n <= 4 ? kc::weighted_vote_kernel<4> : kc::weighted_vote_kernel<8>;
+        kernel<<<grid, threads, 0, st>>>(d_codes, d_seq_logprob, G, n, fm, has_nc, d_win_code, d_meta, d_weight);
+        KC_CUDA_I(cudaGetLastError());
+        return KC_OK;
     }
-#define KC_WV(NP) kc::weighted_vote_kernel<NP><<<grid, threads, 0, st>>>(d_codes, d_seq_logprob, G, n, fm, d_none_code != nullptr, d_win_code, d_meta, d_weight)
-    if (n <= 2) KC_WV(2);
-    else if (n <= 4) KC_WV(4);
-    else if (n <= 8) KC_WV(8);
-    else if (n <= 16) KC_WV(16);
-    else if (n <= 32) KC_WV(32);
-    else KC_WV(64);
-#undef KC_WV
-    KC_CUDA(cudaGetLastError());
-    return KC_OK;
+    // weights once per record, one row per thread straight from global memory
+    constexpr int T = 128;
+    const int max_recs = T / n_fields + 2;
+    return with_pow2<8>(n, [&](auto np) {
+        constexpr int NP = decltype(np)::value;
+        auto kernel = kc::weighted_vote_rec_kernel<NP, T>;
+        const size_t smem = (size_t)max_recs * NP * 4;  // the candidate weights of the tile's records
+        int grid = 0;
+        int rc = persistent_grid(kernel, T, smem, (G + T - 1) / T, grid);
+        if (rc) return rc;
+        kernel<<<grid, T, smem, st>>>(d_codes, d_seq_logprob, G, n, fm, has_nc, d_win_code, d_meta, d_weight);
+        KC_CUDA_I(cudaGetLastError());
+        return KC_OK;
+    });
 }
 
 int kc_medoid_str(const uint8_t *d_chars, const int32_t *d_str_off, const int32_t *d_grp_off, int64_t n_groups,
@@ -862,47 +734,43 @@ int kc_medoid_str(const uint8_t *d_chars, const int32_t *d_str_off, const int32_
 
 int kc_medoid_str_method(const uint8_t *d_chars, const int32_t *d_str_off, const int32_t *d_grp_off, int64_t n_groups,
                          int32_t max_group, int32_t method, int32_t *d_best_idx, double *d_best_avg, void *stream) {
-    if (method < KC_SIM_LEVENSHTEIN || method > KC_SIM_HAMMING) return fail(KC_EINVAL, "kc_medoid_str: unknown similarity method %d", method);
-    if (n_groups < 0) return fail(KC_EINVAL, "kc_medoid_str: negative n_groups");
+    if (method < KC_SIM_LEVENSHTEIN || method > KC_SIM_HAMMING) return kc_fail(KC_EINVAL, "kc_medoid_str: unknown similarity method %d", method);
+    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_medoid_str: negative n_groups");
     if (max_group < 2 || max_group > kc::kMedoidMaxN)
-        return fail(KC_EINVAL, "kc_medoid_str: max_group=%d outside [2,%d]", max_group, kc::kMedoidMaxN);
+        return kc_fail(KC_EINVAL, "kc_medoid_str: max_group=%d outside [2,%d]", max_group, kc::kMedoidMaxN);
     if (n_groups == 0) return KC_OK;
-    if (!d_chars || !d_str_off || !d_grp_off || !d_best_idx || !d_best_avg) return fail(KC_EINVAL, "kc_medoid_str: NULL buffer");
-    DeviceInfo info;
-    int rc = device_info(info);
-    if (rc) return rc;
+    if (!d_chars || !d_str_off || !d_grp_off || !d_best_idx || !d_best_avg) return kc_fail(KC_EINVAL, "kc_medoid_str: NULL buffer");
     constexpr int WARPS = 4;
     auto kernel = kc::medoid_kernel<WARPS>;
     const size_t per_warp = (kc::MedoidSmem::bytes(max_group) + 15) & ~size_t(15);  // match tables + distances, sized by max_group
     const size_t smem = WARPS * per_warp;
-    KC_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 1;
-    KC_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, WARPS * 32, smem));
-    const int grid = (int)std::min<int64_t>((n_groups + WARPS - 1) / WARPS, (int64_t)info.sm_count * std::max(per_sm, 1));
+    int grid = 0;
+    int rc = persistent_grid(kernel, WARPS * 32, smem, (n_groups + WARPS - 1) / WARPS, grid);
+    if (rc) return rc;
     kernel<<<grid, WARPS * 32, smem, static_cast<cudaStream_t>(stream)>>>(d_chars, d_str_off, d_grp_off, n_groups, max_group,
                                                                          d_best_idx, d_best_avg, method);
-    KC_CUDA(cudaGetLastError());
+    KC_CUDA_I(cudaGetLastError());
     return KC_OK;
 }
 
 int kc_medoid_str_host(const uint8_t *h_chars, int64_t n_chars, const int32_t *h_str_off, const int32_t *h_grp_off, int64_t n_groups,
                        int32_t max_group, int32_t *h_best_idx, double *h_best_avg, int device) {
-    if (n_groups < 0 || n_chars < 0) return fail(KC_EINVAL, "kc_medoid_str_host: negative size");
+    if (n_groups < 0 || n_chars < 0) return kc_fail(KC_EINVAL, "kc_medoid_str_host: negative size");
     if (n_groups == 0) return KC_OK;
-    if (!h_str_off || !h_grp_off || !h_best_idx || !h_best_avg || (n_chars && !h_chars)) return fail(KC_EINVAL, "kc_medoid_str_host: NULL buffer");
-    KC_CUDA(cudaSetDevice(device));
+    if (!h_str_off || !h_grp_off || !h_best_idx || !h_best_avg || (n_chars && !h_chars)) return kc_fail(KC_EINVAL, "kc_medoid_str_host: NULL buffer");
+    KC_CUDA_I(cudaSetDevice(device));
     const int64_t n_str = h_grp_off[n_groups];
-    if (n_str < 0 || h_str_off[n_str] != n_chars) return fail(KC_EINVAL, "kc_medoid_str_host: offsets do not add up to n_chars");
+    if (n_str < 0 || h_str_off[n_str] != n_chars) return kc_fail(KC_EINVAL, "kc_medoid_str_host: offsets do not add up to n_chars");
     const size_t b_chars = ((size_t)n_chars + 255) & ~size_t(255), b_str = (((size_t)n_str + 1) * 4 + 255) & ~size_t(255),
                  b_grp = (((size_t)n_groups + 1) * 4 + 255) & ~size_t(255), b_idx = ((size_t)n_groups * 4 + 255) & ~size_t(255),
                  b_avg = (size_t)n_groups * 8;
     uint8_t *d = nullptr;
-    KC_CUDA(cudaMalloc(&d, b_chars + b_str + b_grp + b_idx + b_avg + 256));
+    KC_CUDA_I(cudaMalloc(&d, b_chars + b_str + b_grp + b_idx + b_avg + 256));
     uint8_t *d_chars = d, *d_str = d + b_chars + 256, *d_grp = d_str + b_str, *d_idx = d_grp + b_grp, *d_avg = d_idx + b_idx;
     int rc = KC_OK;
     cudaStream_t st = nullptr;
     auto guard = [&](cudaError_t e, const char *what) {
-        if (e != cudaSuccess && rc == KC_OK) rc = fail(KC_ECUDA, "kc_medoid_str_host: %s: %s", what, cudaGetErrorString(e));
+        if (e != cudaSuccess && rc == KC_OK) rc = kc_fail(KC_ECUDA, "kc_medoid_str_host: %s: %s", what, cudaGetErrorString(e));
     };
     guard(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking), "stream");
     if (n_chars) guard(cudaMemcpyAsync(d_chars, h_chars, (size_t)n_chars, cudaMemcpyHostToDevice, st), "H2D chars");
@@ -963,17 +831,17 @@ static int consensus_host_impl(const void *h_codes_v, int code_bytes, int32_t n_
                                uint32_t *h_num_meta, int device, float *device_ms) {
     const uint8_t *h_codes = static_cast<const uint8_t *>(h_codes_v);
     if (device_ms) *device_ms = 0.0f;
-    if (n < 1 || n > KC_MAX_CANDIDATES) return fail(KC_EINVAL, "kc_consensus_host: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
-    if (n_records < 0 || n_vote_fields < 0 || n_num_fields < 0) return fail(KC_EINVAL, "kc_consensus_host: negative size");
-    if (device < 0 || device >= 16) return fail(KC_EINVAL, "kc_consensus_host: device %d out of range", device);
-    if (n_vote_fields > 0 && (!h_codes || !h_win_code || !h_vote_meta)) return fail(KC_EINVAL, "kc_consensus_host: NULL vote buffer");
-    if (n_num_fields > 0 && (!h_vals || !h_value || !h_num_meta)) return fail(KC_EINVAL, "kc_consensus_host: NULL numeric buffer");
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_consensus_host: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
+    if (n_records < 0 || n_vote_fields < 0 || n_num_fields < 0) return kc_fail(KC_EINVAL, "kc_consensus_host: negative size");
+    if (device < 0 || device >= 16) return kc_fail(KC_EINVAL, "kc_consensus_host: device %d out of range", device);
+    if (n_vote_fields > 0 && (!h_codes || !h_win_code || !h_vote_meta)) return kc_fail(KC_EINVAL, "kc_consensus_host: NULL vote buffer");
+    if (n_num_fields > 0 && (!h_vals || !h_value || !h_num_meta)) return kc_fail(KC_EINVAL, "kc_consensus_host: NULL numeric buffer");
     if (n_records == 0 || (n_vote_fields == 0 && n_num_fields == 0)) return KC_OK;
 
     std::lock_guard<std::mutex> lock(g_host_mu);
     int prev = 0;
-    KC_CUDA(cudaGetDevice(&prev));
-    KC_CUDA(cudaSetDevice(device));
+    KC_CUDA_I(cudaGetDevice(&prev));
+    KC_CUDA_I(cudaSetDevice(device));
     HostCtx &cx = g_host[device];
     int rc = KC_OK;
     auto finish = [&](int code) {
@@ -982,7 +850,7 @@ static int consensus_host_impl(const void *h_codes_v, int code_bytes, int32_t n_
     };
     if (cx.device != device) {
         for (auto &s : cx.streams)
-            if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return finish(fail(KC_ECUDA, "cudaStreamCreate failed"));
+            if (cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) != cudaSuccess) return finish(kc_fail(KC_ECUDA, "cudaStreamCreate failed"));
         cx.device = device;
     }
     // chunk: ~48 MiB of input per stream buffer keeps H2D, kernels and D2H of neighbouring chunks overlapped
@@ -1009,7 +877,7 @@ static int consensus_host_impl(const void *h_codes_v, int code_bytes, int32_t n_
         if (rc) return finish(rc);
         if (cudaMemcpyAsync(cx.none.p, h_none_code, (size_t)n_vote_fields * 4, cudaMemcpyHostToDevice, cx.streams[0]) != cudaSuccess ||
             cudaStreamSynchronize(cx.streams[0]) != cudaSuccess)
-            return finish(fail(KC_ECUDA, "none_code upload failed: %s", cudaGetErrorString(cudaGetLastError())));
+            return finish(kc_fail(KC_ECUDA, "none_code upload failed: %s", cudaGetErrorString(cudaGetLastError())));
         d_none = cx.none.as<int32_t>();
     }
     // device-side timing of the whole call: start on stream 0 before the first copy; stop on stream 0 after it has
@@ -1055,7 +923,7 @@ static int consensus_host_impl(const void *h_codes_v, int code_bytes, int32_t n_
                 e = cudaMemcpyAsync(h_num_meta + r0 * n_num_fields, cx.nmeta[s].as<uint32_t>(), (size_t)G * 4, cudaMemcpyDeviceToHost, st);
         }
         nvtxRangePop();
-        if (e != cudaSuccess) rc = fail(KC_ECUDA, "kc_consensus_host: %s", cudaGetErrorString(e));
+        if (e != cudaSuccess) rc = kc_fail(KC_ECUDA, "kc_consensus_host: %s", cudaGetErrorString(e));
     }
     if (device_ms) {
         for (int s = 1; s < HostCtx::kStreams; ++s) {
@@ -1066,7 +934,7 @@ static int consensus_host_impl(const void *h_codes_v, int code_bytes, int32_t n_
     }
     for (auto &s : cx.streams) {
         cudaError_t e = cudaStreamSynchronize(s);
-        if (e != cudaSuccess && !rc) rc = fail(KC_ECUDA, "kc_consensus_host sync: %s", cudaGetErrorString(e));
+        if (e != cudaSuccess && !rc) rc = kc_fail(KC_ECUDA, "kc_consensus_host sync: %s", cudaGetErrorString(e));
     }
     if (device_ms) {
         if (!rc) cudaEventElapsedTime(device_ms, ev_start, ev_stop);

@@ -306,7 +306,7 @@ def test_s32_full_size_properties():
     assert np.array_equal(nmeta.view(N, 8)[sel].cpu().numpy().reshape(-1).view(np.uint32), enm)
 
 
-@pytest.mark.parametrize("n", [2, 3, 8, 16, 32, 64])
+@pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 8, 16, 32, 64])
 def test_weighted_vote_matches_oracle(n):
     """K3b (self-defined spec, DESIGN.md §5): bit-exact against the C oracle, incl. the class weights."""
     torch = _torch()

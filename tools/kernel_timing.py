@@ -63,8 +63,7 @@ def main():
             tn = sorted(e[1].elapsed_time(e[2]) for e in evs)[len(evs) // 2]
             print(json.dumps({"interleaved": args.other, "vote_ms": round(tv, 4), "numeric_ms": round(tn, 4), "vote_frac": round(bv / tv / 1e6 / peak, 3),
                               "numeric_frac": round(bn / tn / 1e6 / peak, 3)}), flush=True)
-        out = {"n": n, "records": N, "p_agree": args.p_agree, "force_direct": os.environ.get("KC_FORCE_DIRECT", "0"),
-               "vote_ms": round(t_v, 4), "vote_GBps": round(bv / t_v / 1e6, 1), "vote_frac": round(bv / t_v / 1e6 / peak, 3),
+        out = {"n": n, "records": N, "p_agree": args.p_agree, "vote_ms": round(t_v, 4), "vote_GBps": round(bv / t_v / 1e6, 1), "vote_frac": round(bv / t_v / 1e6 / peak, 3),
                "numeric_ms": round(t_n, 4), "numeric_GBps": round(bn / t_n / 1e6, 1),
                "numeric_frac": round(bn / t_n / 1e6 / peak, 3),
                "records_per_s": round(N / ((t_v + t_n) / 1e3)), "both_frac": round((bv + bn) / (t_v + t_n) / 1e6 / peak, 3)}
