@@ -26,6 +26,82 @@ def same(a, b) -> bool:
     return a == b
 
 
+def random_codes(rng, G, n, vocab, p_none=0.08, p_absent=0.03, p_agree=0.6):
+    """K1 input: int32 [G, n] codes around a per-group truth, with None (-1) and absent (-2) cells."""
+    truth = rng.integers(0, vocab, (G, 1))
+    draw = rng.integers(0, vocab, (G, n))
+    codes = np.where(rng.random((G, n)) < p_agree, truth, draw).astype(np.int32)
+    codes[rng.random((G, n)) < p_none] = -1
+    codes[rng.random((G, n)) < p_absent] = -2
+    return codes
+
+
+def random_vals(rng, G, n, style):
+    """K2 input: float64 [G, n] in one of five styles, with None / absent / NaN / inf cells."""
+    from oracle.columnar import F64_ABSENT, F64_NONE
+    if style == "ints":
+        t = np.floor(rng.random((G, 1)) * 1e6) + 1
+        d = np.floor(rng.random((G, n)) * 1e6) + 1
+    elif style == "near":  # straddle the 3% tolerance, both signs, zeros, tiny values
+        base = rng.choice([1.0, -1.0, 100.0, 1e-7, 0.0, 12.5, -3000.0], (G, 1))
+        t = base
+        d = base * (1.0 + rng.choice([-0.05, -0.031, -0.029, 0.0, 0.015, 0.0299, 0.0301, 0.06], (G, n)))
+    elif style == "pow10":  # decimal-shift and sign mistakes -> tie-resolution paths
+        base = rng.choice([12.5, 7.0, 0.125, 3.3], (G, 1))
+        t = base
+        d = base * rng.choice([1.0, 10.0, 0.1, -1.0, 100.0, 1.0, 1.0], (G, n))
+    elif style == "lowbits":  # values that differ only in low mantissa bits (32-bit sort keys tie; repair path)
+        base = rng.choice([1.0, -1.0, 3.141592653589793, 1e-300, -7e5, 123456.0], (G, 1))
+        t = base
+        d = base * (1.0 + rng.integers(-40, 40, (G, n)) * 2.0 ** rng.choice([-52, -50, -45, -40, -33, -30, -20], (G, 1)))
+    else:
+        t = rng.uniform(1, 1e4, (G, 1))
+        d = rng.uniform(1, 1e4, (G, n))
+    p_agree = rng.choice([0.2, 0.5, 0.8], (G, 1))
+    vals = np.where(rng.random((G, n)) < p_agree, t, d).astype(np.float64)
+    vals[rng.random((G, n)) < 0.08] = F64_NONE
+    vals[rng.random((G, n)) < 0.03] = F64_ABSENT
+    vals[rng.random((G, n)) < 0.02] = np.nan
+    vals[rng.random((G, n)) < 0.01] = np.inf
+    return np.ascontiguousarray(vals)
+
+
+VAL_STYLES = ("ints", "near", "pow10", "floats", "lowbits")
+
+# (rel_eps, abs_eps) settings that put K2's tolerance tests on their edges: the default, exact equality, very loose, and
+# a relative tolerance below one ulp with a denormal absolute one
+EDGE_EPS = ((0.03, 1e-6), (0.0, 0.0), (0.9, 10.0), (1e-12, 1e-300))
+
+
+def numeric_edge_vals(rng, G, n):
+    """K2 input where the majority shortcut has to give up or sits on a boundary, and the general kernels' tie and low-bit
+    repair paths run: neighbours right at the tolerance, cells sharing v's high word, signed zeros, -inf / negative NaN /
+    odd NaN payloads, absent cells, overflow of the sum, every majority size."""
+    from oracle.columnar import F64_ABSENT, F64_NONE
+    pool = np.array([0.0, -0.0, 1.0, 5e-324, 1e-310, 2.0 ** -1022, 1.7e308, 9e307, 123456.0, 0.1, 1e15 + 0.5, 3.0, 2.0 ** 52,
+                     1048576.0, 1048577.0, 0.999999, 33.333333333333336], dtype=np.float64)
+    v = pool[rng.integers(0, len(pool), G)]
+    odd = np.array([F64_NONE, F64_ABSENT, np.nan, -np.nan, np.inf, -np.inf], dtype=np.float64)
+    odd = np.concatenate([odd, np.array([0x7FFFFFFFFFFFFFFF, 0xFFF8000000000001, 0x7FF8C0DE00000001, 0x7FF8C0E000000000],
+                                        dtype=np.uint64).view(np.float64)])
+    factor = np.array([0.97, 0.9700000001, 0.9699999999, 1.03, 1.0300000001, 1.0299999999, 1 + 1e-9, 1 - 2.0 ** -20, 1 + 2.0 ** -21,
+                       1 + 2.0 ** -33, 0.5, 2.0, -1.0, 1.0309278350515465, 0.9708737864077669], dtype=np.float64)
+    vals = np.repeat(v[:, None], n, axis=1)
+    c = rng.integers(1, n + 1, G)                                  # copies of v kept
+    for g in range(G):
+        k = n - c[g]
+        if k == 0:
+            continue
+        pos = rng.choice(n, k, replace=False)
+        kind = rng.integers(0, 5, k)
+        repl = np.where(kind == 0, odd[rng.integers(0, len(odd), k)],
+                np.where(kind == 1, v[g] * factor[rng.integers(0, len(factor), k)],
+                np.where(kind == 2, np.nextafter(v[g], np.inf * rng.choice([-1.0, 1.0], k)),
+                np.where(kind == 3, F64_NONE, rng.uniform(-10, 2e6, k)))))
+        vals[g, pos] = repl
+    return np.ascontiguousarray(vals)
+
+
 def raising_embeddings(texts):
     raise RuntimeError("no network in tests")
 

@@ -3,6 +3,7 @@ import numpy as np
 import pytest
 
 from oracle import columnar as OC
+from tests.helpers import EDGE_EPS, numeric_edge_vals, random_codes, random_vals
 
 pytestmark = pytest.mark.gpu
 
@@ -12,43 +13,6 @@ NONE, ABSENT = OC.F64_NONE, OC.F64_ABSENT
 def _torch():
     import torch
     return torch
-
-
-def random_codes(rng, G, n, vocab, p_none=0.08, p_absent=0.03, p_agree=0.6):
-    truth = rng.integers(0, vocab, (G, 1))
-    draw = rng.integers(0, vocab, (G, n))
-    codes = np.where(rng.random((G, n)) < p_agree, truth, draw).astype(np.int32)
-    codes[rng.random((G, n)) < p_none] = -1
-    codes[rng.random((G, n)) < p_absent] = -2
-    return codes
-
-
-def random_vals(rng, G, n, style):
-    if style == "ints":
-        t = np.floor(rng.random((G, 1)) * 1e6) + 1
-        d = np.floor(rng.random((G, n)) * 1e6) + 1
-    elif style == "near":  # straddle the 3% tolerance, both signs, zeros, tiny values
-        base = rng.choice([1.0, -1.0, 100.0, 1e-7, 0.0, 12.5, -3000.0], (G, 1))
-        t = base
-        d = base * (1.0 + rng.choice([-0.05, -0.031, -0.029, 0.0, 0.015, 0.0299, 0.0301, 0.06], (G, n)))
-    elif style == "pow10":  # decimal-shift and sign mistakes -> tie-resolution paths
-        base = rng.choice([12.5, 7.0, 0.125, 3.3], (G, 1))
-        t = base
-        d = base * rng.choice([1.0, 10.0, 0.1, -1.0, 100.0, 1.0, 1.0], (G, n))
-    elif style == "lowbits":  # values that differ only in low mantissa bits (32-bit sort keys tie; repair path)
-        base = rng.choice([1.0, -1.0, 3.141592653589793, 1e-300, -7e5, 123456.0], (G, 1))
-        t = base
-        d = base * (1.0 + rng.integers(-40, 40, (G, n)) * 2.0 ** rng.choice([-52, -50, -45, -40, -33, -30, -20], (G, 1)))
-    else:
-        t = rng.uniform(1, 1e4, (G, 1))
-        d = rng.uniform(1, 1e4, (G, n))
-    p_agree = rng.choice([0.2, 0.5, 0.8], (G, 1))
-    vals = np.where(rng.random((G, n)) < p_agree, t, d).astype(np.float64)
-    vals[rng.random((G, n)) < 0.08] = NONE
-    vals[rng.random((G, n)) < 0.03] = ABSENT
-    vals[rng.random((G, n)) < 0.02] = np.nan
-    vals[rng.random((G, n)) < 0.01] = np.inf
-    return np.ascontiguousarray(vals)
 
 
 def same_bits(a: np.ndarray, b: np.ndarray) -> bool:
@@ -85,6 +49,29 @@ def test_vote_single_field_with_none_code(n):
         exp_win, exp_meta = OC.vote(codes, nc)
         win, meta = K.vote(torch.from_numpy(codes).cuda(), torch.from_numpy(nc).cuda())
         assert np.array_equal(win.cpu().numpy(), exp_win) and np.array_equal(meta.cpu().numpy().view(np.uint32), exp_meta)
+
+
+@pytest.mark.parametrize("n", [2, 4, 8, 16, 32, 64])
+@pytest.mark.parametrize("n_fields", [1, 2, 3, 5, 7, 9, 17, 33, 1000, 59999])
+def test_vote_field_maps(n, n_fields):
+    """Voting Nones with a different none_code per field, from fewer fields than vote_multi_kernel's groups per thread (the
+    field wraps inside a thread's unit) up to the largest count the TMA kernels' field map takes.  The group count is odd and
+    ends inside a record, so the one-group launches after vote_multi_kernel run and must pick up the field where it stopped."""
+    torch = _torch()
+    from k_llms_b200 import _native as K
+    rng = np.random.default_rng(1000 * n + n_fields)
+    G = max(20000, 2 * n_fields + n_fields // 2) | 1
+    codes = random_codes(rng, G, n, 4, p_none=0.3, p_absent=0.02)
+    none_code = rng.integers(-1, 7, n_fields).astype(np.int32)
+    none_code[: min(n_fields, 2)] = (5, -1)[: min(n_fields, 2)]
+    exp_win, exp_meta = OC.vote(codes, none_code)
+    d_codes, d_nc = torch.from_numpy(codes).cuda(), torch.from_numpy(none_code).cuda()
+    win = torch.empty(G, dtype=torch.int32, device="cuda")
+    meta = torch.empty(G, dtype=torch.int32, device="cuda")
+    K.check(K.load().kc_vote_i32(d_codes.data_ptr(), G, n, d_nc.data_ptr(), n_fields, win.data_ptr(), meta.data_ptr(),
+                                 torch.cuda.current_stream().cuda_stream))
+    bad = np.nonzero((win.cpu().numpy() != exp_win) | (meta.cpu().numpy().view(np.uint32) != exp_meta))[0]
+    assert bad.size == 0, (bad.size, bad[:5], bad[:5] % n_fields)
 
 
 @pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 8, 11, 16, 24, 32, 48, 64])
@@ -153,31 +140,9 @@ def test_numeric_fast_path_edges(n):
     torch = _torch()
     from k_llms_b200 import _native as K
     rng = np.random.default_rng(900 + n)
-    G = 20000
-    pool = np.array([0.0, -0.0, 1.0, 5e-324, 1e-310, 2.0 ** -1022, 1.7e308, 9e307, 123456.0, 0.1, 1e15 + 0.5, 3.0, 2.0 ** 52,
-                     1048576.0, 1048577.0, 0.999999, 33.333333333333336], dtype=np.float64)
-    v = pool[rng.integers(0, len(pool), G)]
-    odd = np.array([NONE, ABSENT, np.nan, -np.nan, np.inf, -np.inf], dtype=np.float64)
-    odd = np.concatenate([odd, np.array([0x7FFFFFFFFFFFFFFF, 0xFFF8000000000001, 0x7FF8C0DE00000001, 0x7FF8C0E000000000],
-                                        dtype=np.uint64).view(np.float64)])
-    factor = np.array([0.97, 0.9700000001, 0.9699999999, 1.03, 1.0300000001, 1.0299999999, 1 + 1e-9, 1 - 2.0 ** -20, 1 + 2.0 ** -21,
-                       1 + 2.0 ** -33, 0.5, 2.0, -1.0, 1.0309278350515465, 0.9708737864077669], dtype=np.float64)
-    vals = np.repeat(v[:, None], n, axis=1)
-    c = rng.integers(1, n + 1, G)                                  # copies of v kept
-    for g in range(G):
-        k = n - c[g]
-        if k == 0:
-            continue
-        pos = rng.choice(n, k, replace=False)
-        kind = rng.integers(0, 5, k)
-        repl = np.where(kind == 0, odd[rng.integers(0, len(odd), k)],
-                np.where(kind == 1, v[g] * factor[rng.integers(0, len(factor), k)],
-                np.where(kind == 2, np.nextafter(v[g], np.inf * rng.choice([-1.0, 1.0], k)),
-                np.where(kind == 3, NONE, rng.uniform(-10, 2e6, k)))))
-        vals[g, pos] = repl
-    vals = np.ascontiguousarray(vals)
+    vals = numeric_edge_vals(rng, 20000, n)
     d_vals = torch.from_numpy(vals).cuda()
-    for rel, ab in ((0.03, 1e-6), (0.0, 0.0), (0.9, 10.0), (1e-12, 1e-300)):
+    for rel, ab in EDGE_EPS:
         with np.errstate(all="ignore"):
             exp_val, exp_meta = OC.numeric(vals, rel, ab)
         val, meta = K.numeric(d_vals, rel, ab)
@@ -306,7 +271,7 @@ def test_s32_full_size_properties():
     assert np.array_equal(nmeta.view(N, 8)[sel].cpu().numpy().reshape(-1).view(np.uint32), enm)
 
 
-@pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 8, 16, 32, 64])
+@pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 6, 7, 8, 12, 16, 24, 32, 48, 64])
 def test_weighted_vote_matches_oracle(n):
     """K3b (self-defined spec, DESIGN.md §5): bit-exact against the C oracle, incl. the class weights."""
     torch = _torch()
@@ -411,7 +376,7 @@ def test_logprob_sum_staged_tiles_and_fallback():
 
 
 @pytest.mark.parametrize("n", [8, 16, 32, 64])
-@pytest.mark.parametrize("fields", [1, 5, 24, 200])
+@pytest.mark.parametrize("fields", [1, 4, 5, 24, 200])
 def test_weighted_vote_per_record_kernel(n, fields):
     """K3b's weights-once-per-record kernel over several fields-per-record shapes (tiles spanning 1 .. 128 records)."""
     torch = _torch()
@@ -432,7 +397,25 @@ def test_weighted_vote_per_record_kernel(n, fields):
             assert np.array_equal(wt.cpu().numpy().view(np.uint32), ewt.view(np.uint32))
 
 
-@pytest.mark.parametrize("n", [3, 4, 8, 16, 32, 64])
+@pytest.mark.parametrize("n", [32, 64])
+def test_weighted_vote_many_fields_per_record_fallback(n):
+    """At n = 32 and 64, 60000 fields or more per record leave the TMA kernels (their field map stops below 60000) for the
+    per-record kernel."""
+    torch = _torch()
+    from k_llms_b200 import _native as K
+    rng = np.random.default_rng(60000 + n)
+    R, F = 3, 60000
+    codes = random_codes(rng, R * F, n, 5, p_none=0.2, p_absent=0.05).reshape(R, F, n)
+    seq = (-rng.exponential(4.0, (R, n))).astype(np.float32)
+    none_code = rng.integers(-1, 6, F).astype(np.int32)
+    for nc in (None, none_code):
+        win, meta, wt = K.weighted_vote(torch.from_numpy(codes).cuda(), torch.from_numpy(seq).cuda(),
+                                        torch.from_numpy(nc).cuda() if nc is not None else None)
+        ew, em, ewt = OC.weighted_vote(codes, seq, nc)
+        assert np.array_equal(win.cpu().numpy(), ew) and np.array_equal(meta.cpu().numpy().view(np.uint32), em)
+        assert np.array_equal(wt.cpu().numpy().view(np.uint32), ewt.view(np.uint32))
+
+@pytest.mark.parametrize("n", [1, 2, 3, 4, 5, 8, 16, 17, 32, 33, 64])
 def test_vote_i8_equals_i32(n):
     """Compact int8 cells are a lossless input format: same outputs as the int32 path and as the oracle."""
     torch = _torch()
