@@ -728,17 +728,21 @@ __global__ void __launch_bounds__(T) numeric_direct_kernel(const double *__restr
 // Candidates of one field mostly agree bit for bit.  If one value v fills a strict majority of the m finite cells, its
 // cluster is the unique largest one whatever the rest looks like (cu:1145-1187), and if no other finite cell is close
 // to v the cluster is exactly the c copies of v: value = np.mean([v]*c), support = c — no sort, no closeness chain.
+// With one or two cells chained to v the cluster is still known: those extras, then the copies, in sorted order.
 //   1. guess v as the bitwise "at least half" vote over the cells (carry-save adder tree, kc_csa.cuh);
 //   2. verify exactly: c = cells bit-identical to v, 2c > m;
 //   3. the nearest finite cells below and above v are found on the HIGH words only (two unsigned min/max scans; only
 //      groups without negative cells are taken, so raw high words are ordered like the values); each stands for every
 //      double sharing that high word.  They are certified far from v with
 //      fl() monotonicity alone: |v - x| >= fl(v - x_nearest_possible) and tol(x, v) <= max(abs, fl(rel * max(|x|_max,
-//      |v|, 1))) for rel >= 0 (the launcher rejects rel < 0);
+//      |v|, 1))) for rel >= 0 (the launcher rejects rel < 0).  A neighbour that cannot be certified so is completed from
+//      the one cell with its high word, tested exactly (far_bit, as numeric_core's chain) and, if close, taken as an
+//      extra; the walk goes on from it, for at most two extras in all;
 //   4. the cell census comes from the same adder tree (bit 31 of x = hi + 2^20 counts the non-finite cells) plus one
 //      min scan that proves every non-finite cell is a None / absent tag;
-//   5. anything else — no majority, a neighbour within reach, a cell sharing v's high word, a negative cell, an inf or
-//      an untagged NaN, a single non-None cell — is NOT decided here: the caller parks the group for numeric_core
+//   5. anything else — no majority, a third extra, a neighbour sharing its high word with another cell, a cell sharing
+//      v's high word, a negative cell, an inf or an untagged NaN, a single non-None cell — is NOT decided here: the caller
+//      parks the group for numeric_core
 //      (exact, general).
 // numeric_fast_decide() returns true when the group is decided; numeric_fast_finish() then produces (value, meta).
 // n += (x == key), as a predicated add (the compiler prefers select + add)
@@ -764,11 +768,29 @@ __device__ __forceinline__ void match_cell(uint32_t h, uint32_t l, uint32_t hv, 
 constexpr uint32_t kFastBias = 0x00100000u;
 
 struct FastDecision {
-    double v;                    // the majority value
-    uint32_t c, tagged, absent;  // its copies; None + absent cells; absent cells
+    double v;       // the majority value
+    double e0, e1;  // the extras chained to v, the last found first (the walk goes down from v, then up)
+    // the result word with v's copies as the support, and in the first-seen index bits (0 in the result) the number of
+    // extras below v (bits 0-1) and above it (bits 2-3): one register while the cells are still live
+    uint32_t word;
 };
 
-// Phase 1: decide.  True <=> the group's result is np.mean([v] * c); the cells are not needed afterwards.
+// The walk to extras pays off from n = 16 (the share of groups with a close neighbour grows with n); at n = 8 it measured
+// slower on H100 than deferring those groups, so there every group with a close neighbour is deferred, and the finish
+// sums the copies of v alone.
+template <int N>
+constexpr bool kWalkExtras = N >= 16;
+
+// Every double with the high word h lies beyond reach of f: h below f's high word (below) or above it.  fl(rel * .) is
+// monotone, so it is enough that the least possible distance exceeds thr = max(abs, rel) and rel * the largest magnitude.
+__device__ __forceinline__ bool certainly_far(double f, uint32_t h, bool below, double rel_eps, double thr) {
+    const double d = below ? __dadd_rn(f, -__hiloint2double((int)h, -1)) : __dadd_rn(__hiloint2double((int)h, 0), -f);
+    const double mag = below ? f : __hiloint2double((int)h, -1);
+    return d > thr && d > __dmul_rn(rel_eps, mag);
+}
+
+// Phase 1: decide.  True <=> the group's result is the mean of v's copies and the extras in `out`; the cells are not needed
+// afterwards.
 template <int N>
 __device__ __forceinline__ bool numeric_fast_decide(const uint32_t (&x)[N], const uint32_t (&lo)[N], uint32_t top, double rel_eps,
                                                     double thr, FastDecision &out) {
@@ -815,16 +837,63 @@ __device__ __forceinline__ bool numeric_fast_decide(const uint32_t (&x)[N], cons
     // close(a, b) <=> |a-b| <= max(abs, rel*max(|a|,|b|,1)) = max(thr, fl(rel*max(|a|,|b|))) with thr = max(abs, rel),
     // because fl(rel * .) is monotone; so "certainly far" <=> d > thr and d > fl(rel * upper bound of the magnitudes).
     const uint32_t hb = hv + below, ha = hv + above + 1u;
-    const double db = __dadd_rn(v, -__hiloint2double((int)hb, -1));
-    const double da = __dadd_rn(__hiloint2double((int)ha, 0), -v);
-    const bool far_b = db > thr && db > __dmul_rn(rel_eps, v);
-    const bool far_a = da > thr && da > __dmul_rn(rel_eps, __hiloint2double((int)ha, -1));
     const bool has_b = below >= 0x80000000u, has_a = above < 0x7FFFFFFFu && ha < 0x7FF00000u;
-    if ((has_b && !far_b) || (has_a && !far_a)) return false;
+    const bool need_b = has_b && !certainly_far(v, hb, true, rel_eps, thr);
+    const bool need_a = has_a && !certainly_far(v, ha, false, rel_eps, thr);
     out.v = v;
-    out.c = c;
-    out.tagged = tagged;
-    out.absent = absent;
+    out.word = (c << 6) + (((uint32_t)N - tagged) << 13) + (((uint32_t)N - absent) << 20) + ((uint32_t)KC_FLAG_HAS_VALUE << 27);
+    out.e0 = out.e1 = v;
+    // A neighbour within possible reach: walk outwards from v, one cell per step, below v first.  A step needs the
+    // neighbour's high word to be unique among the cells (that cell's low word completes it), tests it exactly as
+    // numeric_core's chain does, and if it is close takes it as an extra and certifies the next cell beyond it far.  At
+    // most two extras; anything else is left to the general path.
+    // xn: the neighbour under test (biased high word, below xv while walking down), xa: where the upward walk starts
+    // (0: nowhere, and xn = 0 ends the walk)
+    if constexpr (!kWalkExtras<N>) {
+        if (need_b || need_a) return false;
+    }
+    uint32_t xn = need_b ? hb + kFastBias : 0u, xa = need_a ? ha + kFastBias : 0u;
+    if (xn == 0u) {
+        xn = xa;
+        xa = 0u;
+    }
+    while (xn != 0u) {
+        const uint32_t nb = out.word & 3u, na = (out.word >> 2) & 3u;
+        if (nb + na == 2u) return false;
+        const bool down = xn < xv;
+        // beyond: as `below` / `above` from xn, mirrored for the upward walk (>= 2^31 <=> a cell lies beyond xn)
+        const uint32_t sm = down ? 0u : 0xFFFFFFFFu, neg = 0u - (xn ^ sm);
+        uint32_t cnt = 0, ln = 0, beyond = 0;
+#pragma unroll
+        for (int i = 0; i < N; ++i) {
+            beyond = max(beyond, (x[i] ^ sm) + neg);
+            asm("{\n\t.reg .pred p;\n\t"
+                "setp.eq.u32 p, %2, %4;\n\t"
+                "@p add.u32 %0, %0, 1;\n\t"
+                "@p mov.b32 %1, %3;\n\t}"
+                : "+r"(cnt), "+r"(ln)
+                : "r"(x[i]), "r"(lo[i]), "r"(xn));
+        }
+        if (cnt != 1u) return false;
+        const double e = __hiloint2double((int)(xn - kFastBias), (int)ln);
+        const double f = (down ? nb : na) ? out.e0 : v;  // the cluster's outermost value on this side so far
+        const double a = down ? e : f, b = down ? f : e;
+        const bool close = far_bit(__dadd_rn(b, -a), __dmul_rn(rel_eps, b), -__dmul_rn(rel_eps, a), thr, 1u) == 0u;
+        bool side_done = !close;
+        if (close) {
+            out.e1 = out.e0;
+            out.e0 = e;
+            out.word += down ? 1u : 4u;
+            const uint32_t hn = (down ? xn + beyond : xn - beyond) - kFastBias;
+            const bool exists = beyond >= 0x80000000u && (down || hn < 0x7FF00000u);
+            side_done = !exists || certainly_far(e, hn, down, rel_eps, thr);
+            xn = hn + kFastBias;
+        }
+        if (side_done) {
+            xn = xa;
+            xa = 0u;
+        }
+    }
     return true;
 }
 
@@ -832,23 +901,57 @@ __device__ __forceinline__ bool numeric_fast_decide(const uint32_t (&x)[N], cons
 template <int N>
 __device__ __forceinline__ void numeric_fast_finish(const FastDecision &d, double &value, uint32_t &meta) {
     const double v = d.v;
-    const uint32_t c = d.c, tagged = d.tagged, absent = d.absent;
-    // np.mean of c copies of v in numpy's summation order: for c >= 8 the eight accumulators are identical (r = the
-    // sequential sum of c/8 copies) and their pairwise sum is 8r exactly; then the c%8 stragglers one by one.
-    double res = -0.0;  // -0.0 + v == v
-    if (c >= 8) {
-        double r = v;
+    const uint32_t c = (d.word >> 6) & 127u;
+    if constexpr (!kWalkExtras<N>) {
+        // c copies of v alone: for c >= 8 the eight accumulators are identical (r = the sequential sum of c/8 copies) and
+        // their pairwise sum is 8r exactly; then the c%8 stragglers one by one.
+        double res = -0.0;  // -0.0 + v == v
+        if (c >= 8) {
+            double r = v;
 #pragma unroll
-        for (int k = 2; k <= N / 8; ++k)
-            if ((int)(c >> 3) >= k) r = __dadd_rn(r, v);
-        res = __dmul_rn(r, 8.0);
+            for (int k = 2; k <= N / 8; ++k)
+                if ((int)(c >> 3) >= k) r = __dadd_rn(r, v);
+            res = __dmul_rn(r, 8.0);
+        }
+#pragma unroll
+        for (int k = 1; k <= 7; ++k)
+            if ((int)(c & 7u) >= k) res = __dadd_rn(res, v);
+        value = __ddiv_rn(__dadd_rn(0.0, res), (double)c);
+        meta = d.word;
+        return;
     }
-    const uint32_t tail = c & 7u;
+    const uint32_t nb = d.word & 3u, na = (d.word >> 2) & 3u;
+    const uint32_t z = c + nb + na, q = z >> 3, t = z & 7u;
+    const double f0 = nb == 0u ? v : (na == 0u ? d.e0 : d.e1), f1 = nb == 2u ? d.e1 : v;  // first two in sorted order
+    const double l2 = na == 2u ? d.e1 : v, l1 = na == 0u ? v : d.e0;                       // last two
+    // np.mean of the sorted cluster [f0 f1 | v ... v | l2 l1] (nb extras first, na last) in numpy's summation order.
+    // z >= 8: accumulator j sums the positions = j (mod 8) below z - t.  Extras below v can only open accumulators 0 and
+    // 1; extras above v can only close accumulators 6 and 7 (t = 0: both, t = 1: the one before the last) or sit in the
+    // tail.  So r2..r5 are the plain sum of q copies, and each other accumulator is one sequential sum with its extra.
+    double r0 = f0, r1 = f1, rp = -0.0;  // rp: q - 1 copies (-0.0 + x == x)
+#pragma unroll
+    for (int k = 2; k <= N / 8; ++k)
+        if ((int)q >= k) {
+            r0 = __dadd_rn(r0, v);
+            r1 = __dadd_rn(r1, v);
+            rp = __dadd_rn(rp, v);
+        }
+    const double r6 = __dadd_rn(rp, t == 0u ? l2 : v), r7 = __dadd_rn(rp, t == 0u ? l1 : (t == 1u ? l2 : v));
+    const double r2 = __dadd_rn(rp, v), s23 = __dadd_rn(r2, r2);
+    const double tree = __dadd_rn(__dadd_rn(__dadd_rn(r0, r1), s23), __dadd_rn(s23, __dadd_rn(r6, r7)));
+    // then left to right: z < 8 the whole cluster from -0.0, otherwise the tail (copies of v, then the extras above in it)
+    const bool small = z < 8u;
+    const uint32_t sb = small ? nb : 0u, sa = small ? na : min(na, t), sv = small ? c : t - sa;
+    double res = small ? -0.0 : tree;
+    if (sb >= 1u) res = __dadd_rn(res, f0);
+    if (sb >= 2u) res = __dadd_rn(res, f1);
 #pragma unroll
     for (int k = 1; k <= 7; ++k)
-        if ((int)tail >= k) res = __dadd_rn(res, v);
-    value = __ddiv_rn(__dadd_rn(0.0, res), (double)c);
-    meta = (c << 6) + (((uint32_t)N - tagged) << 13) + (((uint32_t)N - absent) << 20) + ((uint32_t)KC_FLAG_HAS_VALUE << 27);
+        if ((int)sv >= k) res = __dadd_rn(res, v);
+    if (sa >= 2u) res = __dadd_rn(res, l2);
+    if (sa >= 1u) res = __dadd_rn(res, l1);
+    value = __ddiv_rn(__dadd_rn(0.0, res), (double)z);
+    meta = (d.word & ~15u) + ((nb + na) << 6);
 }
 
 // Register-prefetch front-end (n == NP, small rows) with the fast path: same deferral queue as the TMA variant below.
