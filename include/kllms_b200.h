@@ -287,8 +287,19 @@ void kc_json_free(kc_json_batch *h);
  * to an ulp, alignments are pinned on the reference's goldens (tests/test_align_native.py).
  */
 int kc_align_json(const char *const *texts, const int64_t *lens, int32_t n, double min_support_ratio, char **out_texts);
-/* test hooks of H2: generic_similarity (consensus_utils.py:892-917) of two JSON values; scipy.optimize.linear_sum_assignment */
+/* kc_align_json for n_records records of n candidate texts each (texts / lens record-major; lens may be NULL): the element
+ * similarities of every list node reached through dicts only (at most 512 elements) are computed in one pass on `device`
+ * (kc_alignsim.cuh; device < 0 runs the same phase on the host), the rest of the alignment on `threads` host threads
+ * (<= 0: default).  Per record: out_texts[r*n + c] and out_status[r] exactly as kc_align_json gives them (0, 1 or KC_EINVAL;
+ * texts only for status 0).  out_counts (optional, 2 entries): element pairs the similarity pass decided, element pairs the
+ * host computed while aligning.  Returns KC_OK or a negative code for the call. */
+int kc_align_json_batch(const char *const *texts, const int64_t *lens, int64_t n_records, int32_t n, double min_support_ratio, int device,
+                        int32_t threads, char **out_texts, int32_t *out_status, int64_t *out_counts);
+/* test hooks of H2: generic_similarity (consensus_utils.py:892-917) of two JSON values; scipy.optimize.linear_sum_assignment;
+ * the similarity pass of kc_align_json_batch on the host for one list of T JSON elements (out: T x T, NaN = left to the host;
+ * returns the pairs i < j it decided) */
 int kc_debug_similarity_json(const char *a, const char *b, double *out);
+int kc_debug_alignsim(const char *const *texts, int32_t T, double *out);
 int kc_debug_lsap(int32_t nr, int32_t nc, const double *cost, int32_t *row_ind, int32_t *col_ind);
 
 /*

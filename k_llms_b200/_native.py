@@ -58,6 +58,7 @@ _SIGNATURES = {
     "kc_consolidate_json": (_int, [_vp, _vp, _i64, _i32, _f64, _f64, _int, _i32, _vp, _vp, _vp]),
     "kc_free_strings": (None, [_vp, _i64]),
     "kc_align_json": (_int, [ctypes.POINTER(_str), _vp, _i32, _f64, ctypes.POINTER(_str)]),
+    "kc_align_json_batch": (_int, [_vp, _vp, _i64, _i32, _f64, _int, _i32, _vp, _vp, _vp]),
     "kc_json_plan": (_int, [_vp, _vp, _i64, _i32, _i32, _pp]),
     "kc_json_inputs": (_int, [_vp] * 10),
     "kc_json_emit": (_int, [_vp] * 9),
@@ -67,6 +68,7 @@ _SIGNATURES = {
     "kc_json_result_free": (None, [_vp]),
     "kc_debug_similarity_json": (_int, [_str, _str, ctypes.POINTER(_f64)]),
     "kc_debug_lsap": (_int, [_i32, _i32, _vp, _vp, _vp]),
+    "kc_debug_alignsim": (_int, [_vp, _i32, _vp]),
     "kc_debug_jsongpu_plan": (_int, [_vp, _vp, _i64, _i32, _pp]),
     "kc_debug_jsongpu_inputs": (_int, [_vp] * 6),
     "kc_debug_jsongpu_emit": (_int, [_vp, _vp, _vp, _vp] + [_pp] * 4),
@@ -273,14 +275,10 @@ def medoid_str(chars, str_off, grp_off, max_group=MAX_CANDIDATES, stream=None, m
     return idx, avg
 
 
-def align_json(values, min_support_ratio: float):
-    """H2: the alignment pre-pass (recursive_list_alignments, default similarity method) of ONE record in native code.
-    values: n JSON-serialisable candidate values.  Returns the aligned values, or None when the record needs the Python
-    pre-pass (long string pairs that go to the embeddings service, non-ASCII text, values json cannot carry)."""
+def _align_texts(values):
+    """The candidate values of one record as ASCII JSON texts for kc_align_json(_batch), or None when the record needs the
+    Python pre-pass."""
     import json
-    n = len(values)
-    if n == 0:
-        return None
     # Precondition: the values look like json.loads output as far as OBJECT IDENTITY goes.  The reference's majority ordering
     # finds an aligned cell's source position by id() (majority_sorting.py:14-17), and the native code restates CPython's
     # behaviour for freshly parsed values (True / False / ints in [-5, 256] / one-character strings are shared objects,
@@ -301,9 +299,23 @@ def align_json(values, min_support_ratio: float):
     if any(shared_identity(v) for v in values):
         return None
     try:
-        texts = (ctypes.c_char_p * n)(*[json.dumps(v).encode("ascii") for v in values])
+        return [json.dumps(v).encode("ascii") for v in values]
     except (TypeError, ValueError):
         return None
+
+
+def align_json(values, min_support_ratio: float):
+    """H2: the alignment pre-pass (recursive_list_alignments, default similarity method) of ONE record in native code.
+    values: n JSON-serialisable candidate values.  Returns the aligned values, or None when the record needs the Python
+    pre-pass (long string pairs that go to the embeddings service, non-ASCII text, values json cannot carry)."""
+    import json
+    n = len(values)
+    if n == 0:
+        return None
+    enc = _align_texts(values)
+    if enc is None:
+        return None
+    texts = (ctypes.c_char_p * n)(*enc)
     out = (ctypes.c_char_p * n)()
     rc = load().kc_align_json(texts, None, n, float(min_support_ratio), out)
     if rc != 0:
@@ -312,6 +324,45 @@ def align_json(values, min_support_ratio: float):
         return [json.loads(out[i]) for i in range(n)]
     finally:
         load().kc_free_strings(out, n)
+
+
+def align_json_batch(records, min_support_ratio: float = 0.51, device: int = 0, threads: int = 0, counts=None):
+    """align_json for many records at once: the element similarities of their list fields are computed in one pass on
+    `device` (kc_align_json_batch; device < 0 runs that pass on the host), the rest of the alignment on host threads.
+    records: list of lists of candidate values.  Returns [align_json(r, min_support_ratio) for r in records] (None where a
+    record needs the Python pre-pass).  counts (optional dict) receives "device_pairs" (element pairs the similarity pass
+    decided) and "host_pairs" (pairs computed on the host while aligning)."""
+    import json
+    lib = load()
+    res = [None] * len(records)
+    by_n = {}  # one call per candidate count
+    for i, values in enumerate(records):
+        enc = _align_texts(values) if len(values) else None
+        if enc is not None:
+            by_n.setdefault(len(values), []).append((i, enc))
+    total = [0, 0]
+    for n, items in by_n.items():
+        R = len(items)
+        blobs = [b for _, enc in items for b in enc]
+        texts = (ctypes.c_char_p * (R * n))(*blobs)
+        lens = (ctypes.c_int64 * (R * n))(*[len(b) for b in blobs])
+        out = (ctypes.c_void_p * (R * n))()
+        status = (ctypes.c_int32 * R)()
+        cnt = (ctypes.c_int64 * 2)()
+        check(lib.kc_align_json_batch(ctypes.cast(texts, ctypes.c_void_p), ctypes.cast(lens, ctypes.c_void_p), R, n, float(min_support_ratio),
+                                      int(device), int(threads), ctypes.cast(out, ctypes.c_void_p), ctypes.cast(status, ctypes.c_void_p),
+                                      ctypes.cast(cnt, ctypes.c_void_p)))
+        try:
+            for k, (i, _) in enumerate(items):
+                if status[k] == 0:
+                    res[i] = [json.loads(ctypes.string_at(out[k * n + c])) for c in range(n)]
+        finally:
+            lib.kc_free_strings(ctypes.cast(out, ctypes.c_void_p), R * n)
+        total[0] += cnt[0]
+        total[1] += cnt[1]
+    if counts is not None:
+        counts["device_pairs"], counts["host_pairs"] = total
+    return res
 
 
 def levenshtein(a: str, b: str) -> int:

@@ -35,6 +35,7 @@
 #include <vector>
 
 #include "../../include/kllms_b200.h"
+#include "kc_internal.h"    // kc_alignsim: element similarities of the alignment pre-pass (kc_alignsim.cuh)
 #include "kc_jsoncore.cuh"  // to_double: exact decimal -> float64 without strtod (host-callable)
 
 namespace {
@@ -656,7 +657,8 @@ void plan_dict(Record &rec, int32_t node, const std::vector<Item> *const *items,
 
 void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Record &rec);
 
-void plan_record(const char *const *texts, const int64_t *lens, int n, Record &rec) {
+// defer_lists: a record with list fields keeps status 2 for the caller, which aligns it (plan_batch); else it is aligned here
+void plan_record(const char *const *texts, const int64_t *lens, int n, Record &rec, bool defer_lists) {
     thread_local std::vector<std::vector<Item>> cands;
     if ((int)cands.size() < n) cands.resize((size_t)n);
     static const char kTextKey[] = "text";
@@ -699,7 +701,7 @@ void plan_record(const char *const *texts, const int64_t *lens, int n, Record &r
     top.assign((size_t)n, nullptr);
     for (int c = 0; c < n; ++c) top[(size_t)c] = &cands[(size_t)c];
     plan_dict(rec, 0, top.data(), n, 0);
-    if (rec.status == 2) plan_record_tree(texts, lens, n, rec);  // list fields: align first (H2), then plan on the aligned tree
+    if (rec.status == 2 && !defer_lists) plan_record_tree(texts, lens, n, rec);  // list fields: align first (H2), then plan on the aligned tree
 }
 
 void encode_vote(GroupKind kind, const Tok *toks, int n, int8_t *cells) {
@@ -996,16 +998,15 @@ void plan_tree_value(Record &rec, AlignCtx &cx, int32_t node, const std::vector<
     rec.groups.push_back(g);
 }
 
-void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Record &rec) {
+// The candidate texts of a record with list fields as a value tree; false: the record takes the Python path (status 1).
+bool parse_record_tree(const char *const *texts, const int64_t *lens, int n, Record &rec, AlignCtx &cx, std::vector<int32_t> &values) {
     rec.status = 0;
     rec.groups.clear();
     rec.cells.clear();
     rec.mchars.clear();
     rec.mlen.clear();
     rec.nodes.clear();
-    auto cxp = std::make_shared<AlignCtx>();
-    AlignCtx &cx = *cxp;
-    std::vector<int32_t> values((size_t)n);
+    values.assign((size_t)n, -1);
     {
         size_t bytes = 0;
         for (int c = 0; c < n; ++c) bytes += lens ? (size_t)lens[c] : strlen(texts[c]);
@@ -1022,7 +1023,7 @@ void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Reco
         }
         if (ok && cx.tr.v[(size_t)values[(size_t)c]].t != A_DICT) {  // valid JSON but not an object: Python path (as the flat planner does)
             rec.status = 1;
-            return;
+            return false;
         }
         if (!ok) {  // {"text": content}
             cx.tr.v.resize(mark);
@@ -1033,6 +1034,12 @@ void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Reco
             values[(size_t)c] = d;
         }
     }
+    return true;
+}
+
+// The alignment pre-pass, then the plan on the aligned tree
+void finish_record_tree(Record &rec, const std::shared_ptr<AlignCtx> &cxp, std::vector<int32_t> &values, int n) {
+    AlignCtx &cx = *cxp;
     align_values(cx, values, /*min_support_ratio=*/0.51, 0);  // ConsensusSettings default (cu:41); other settings: Python path
     if (cx.decline) {
         rec.status = 1;
@@ -1042,6 +1049,12 @@ void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Reco
     rec.nodes.emplace_back();
     plan_tree_value(rec, cx, 0, values, n, 0, tmp);
     if (rec.status == 0) rec.tree = cxp;  // from here on nothing is added to the tree: cells and keys point into it
+}
+
+void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Record &rec) {
+    auto cxp = std::make_shared<AlignCtx>();
+    std::vector<int32_t> values;
+    if (parse_record_tree(texts, lens, n, rec, *cxp, values)) finish_record_tree(rec, cxp, values, n);
 }
 
 // ---------------------------------------------------------------- a batch of records: plan, encode, emit
@@ -1057,10 +1070,36 @@ struct Batch {
 
 int default_threads() { return (int)std::min(32u, std::max(1u, std::thread::hardware_concurrency())); }  // parsing saturates memory / malloc beyond ~32
 
-void plan_batch(Batch &b, const char *const *texts, const int64_t *lens, int64_t n_records, int n, int threads) {
+// sim_device >= 0: the element similarities of the records with list fields come from one kc_alignsim pass on that device
+// (the records are aligned after it); < 0: every similarity is computed on the host while aligning.
+int plan_batch(Batch &b, const char *const *texts, const int64_t *lens, int64_t n_records, int n, int threads, int sim_device) {
     b.n = n;
     b.recs.assign((size_t)n_records, Record());
-    parallel_for(n_records, threads, [&](int64_t r) { plan_record(texts + r * n, lens ? lens + r * n : nullptr, n, b.recs[(size_t)r]); });
+    const bool defer = sim_device >= 0;
+    parallel_for(n_records, threads, [&](int64_t r) { plan_record(texts + r * n, lens ? lens + r * n : nullptr, n, b.recs[(size_t)r], defer); });
+    if (defer) {
+        std::vector<int64_t> idx;  // the records with list fields
+        for (int64_t r = 0; r < n_records; ++r)
+            if (b.recs[(size_t)r].status == 2) idx.push_back(r);
+        std::vector<std::shared_ptr<AlignCtx>> cxs(idx.size());
+        std::vector<std::vector<int32_t>> values(idx.size());
+        std::vector<AlignCtx *> tabs(idx.size(), nullptr);
+        parallel_for((int64_t)idx.size(), threads, [&](int64_t i) {
+            const int64_t r = idx[(size_t)i];
+            cxs[(size_t)i] = std::make_shared<AlignCtx>();
+            if (!parse_record_tree(texts + r * n, lens ? lens + r * n : nullptr, n, b.recs[(size_t)r], *cxs[(size_t)i], values[(size_t)i])) {
+                cxs[(size_t)i].reset();
+                return;
+            }
+            sim_collect(*cxs[(size_t)i], values[(size_t)i], 0);
+            tabs[(size_t)i] = cxs[(size_t)i].get();
+        });
+        const int rc = sim_batch(tabs, sim_device, threads, nullptr, [&](int64_t i) {
+            if (cxs[(size_t)i]) finish_record_tree(b.recs[(size_t)idx[(size_t)i]], cxs[(size_t)i], values[(size_t)i], n);
+            cxs[(size_t)i].reset();  // a planned record keeps its tree through Record::tree
+        });
+        if (rc) return rc;
+    }
     for (auto &rec : b.recs) {
         if (rec.status) continue;
         for (auto &g : rec.groups) {
@@ -1075,6 +1114,7 @@ void plan_batch(Batch &b, const char *const *texts, const int64_t *lens, int64_t
         }
         if (!rec.mchars.empty()) b.m_chars.insert(b.m_chars.end(), rec.mchars.begin(), rec.mchars.end());
     }
+    return KC_OK;
 }
 
 void encode_batch(const Batch &b, int8_t *codes, double *vals, int threads) {
@@ -1121,7 +1161,7 @@ int kc_consolidate_json(const char *const *texts, const int64_t *lens, int64_t n
     auto ms = [](auto a, auto b) { return std::chrono::duration<double, std::milli>(b - a).count(); };
     const auto t0 = now();
     Batch batch;
-    plan_batch(batch, texts, lens, n_records, n, threads);
+    if (const int rc = plan_batch(batch, texts, lens, n_records, n, threads, device)) return rc;
     const auto t1 = now();
     const int64_t gv = batch.gv, gx = batch.gx, gm = batch.gm;
     std::vector<int32_t> m_idx((size_t)gm);
@@ -1186,7 +1226,10 @@ int kc_json_plan(const char *const *texts, const int64_t *lens, int64_t n_record
     kc_json_batch *h = new (std::nothrow) kc_json_batch;
     if (!h) return KC_ENOMEM;
     h->threads = threads;
-    plan_batch(h->batch, texts, lens, n_records, n, threads);
+    if (const int rc = plan_batch(h->batch, texts, lens, n_records, n, threads, -1)) {
+        delete h;
+        return rc;
+    }
     h->codes.resize((size_t)h->batch.gv * n);
     h->vals.resize((size_t)h->batch.gx * n);
     encode_batch(h->batch, h->codes.data(), h->vals.data(), threads);
@@ -1248,6 +1291,97 @@ int kc_align_json(const char *const *texts, const int64_t *lens, int32_t n, doub
         out_texts[c] = dup_string(out);
     }
     return 0;
+}
+
+// kc_align_json for a batch of records (n candidate texts each, record-major), with the element similarities of their list
+// nodes computed in one kc_alignsim pass on `device` (< 0: the same phase on the host) before the records are aligned.
+int kc_align_json_batch(const char *const *texts, const int64_t *lens, int64_t n_records, int32_t n, double min_support_ratio, int device,
+                        int32_t threads, char **out_texts, int32_t *out_status, int64_t *out_counts) {
+    if (!texts || !out_texts || !out_status || n < 1 || n_records < 0) return kc_fail(KC_EINVAL, "kc_align_json_batch: bad arguments");
+    if (threads <= 0) threads = default_threads();
+    std::vector<std::unique_ptr<AlignCtx>> cxs((size_t)n_records);
+    std::vector<std::vector<int32_t>> values((size_t)n_records);
+    std::vector<AlignCtx *> tabs((size_t)n_records, nullptr);
+    parallel_for(n_records, threads, [&](int64_t r) {  // parse as kc_align_json does, then flatten the list nodes
+        for (int32_t c = 0; c < n; ++c) out_texts[r * n + c] = nullptr;
+        auto cx = std::make_unique<AlignCtx>();
+        std::vector<int32_t> &vals = values[(size_t)r];
+        vals.assign((size_t)n, -1);
+        out_status[r] = 0;
+        for (int32_t c = 0; c < n && !out_status[r]; ++c) {
+            const char *t = texts[r * n + c];
+            const size_t len = lens ? (size_t)lens[r * n + c] : strlen(t);
+            Scanner sc{t, t + len};
+            if (!aparse(sc, cx->tr, vals[(size_t)c], 0)) {
+                out_status[r] = KC_EINVAL;
+                break;
+            }
+            sc.ws();
+            if (sc.p != sc.end) out_status[r] = KC_EINVAL;
+            else if (sc.non_ascii) out_status[r] = 1;
+            for (size_t i = 0; i < len && !out_status[r]; ++i)
+                if ((unsigned char)t[i] >= 0x80) out_status[r] = 1;
+        }
+        if (out_status[r]) return;
+        sim_collect(*cx, vals, 0);
+        tabs[(size_t)r] = cx.get();
+        cxs[(size_t)r] = std::move(cx);
+    });
+    int64_t device_pairs = 0;
+    std::atomic<int64_t> host_pairs{0};
+    const int rc = sim_batch(tabs, device, threads, &device_pairs, [&](int64_t r) {
+        if (!cxs[(size_t)r]) return;
+        AlignCtx &cx = *cxs[(size_t)r];
+        std::vector<int32_t> &vals = values[(size_t)r];
+        align_values(cx, vals, min_support_ratio, 0);
+        host_pairs += cx.host_pairs;
+        if (cx.decline) {
+            out_status[r] = 1;
+        } else {
+            std::string out;
+            for (int32_t c = 0; c < n; ++c) {
+                out.clear();
+                adump(cx.tr, vals[(size_t)c], out);
+                out_texts[r * n + c] = dup_string(out);
+            }
+        }
+        cxs[(size_t)r].reset();
+    });
+    if (rc) {
+        for (int64_t i = 0; i < n_records * n; ++i) {
+            free(out_texts[i]);
+            out_texts[i] = nullptr;
+        }
+        return rc;
+    }
+    if (out_counts) {
+        out_counts[0] = device_pairs;
+        out_counts[1] = host_pairs.load();
+    }
+    return KC_OK;
+}
+
+// The similarity phase of kc_align_json_batch instantiated on the host for one node whose T elements are given as JSON
+// texts: out[i * T + j] as kc_alignsim computes it (NaN where it leaves the pair to the host).  Test hook.  Returns the
+// number of pairs i < j it decided, KC_EINVAL on invalid / non-ASCII JSON or T outside [2, 512].
+int kc_debug_alignsim(const char *const *texts, int32_t T, double *out) {
+    if (!texts || !out || T < 2 || T > 512) return KC_EINVAL;
+    AlignCtx cx;
+    const int32_t list = cx.tr.add(A_LIST);
+    for (int32_t k = 0; k < T; ++k) {
+        Scanner sc{texts[k], texts[k] + strlen(texts[k])};
+        int32_t id;
+        if (!aparse(sc, cx.tr, id, 0) || sc.non_ascii) return KC_EINVAL;
+        sc.ws();
+        if (sc.p != sc.end) return KC_EINVAL;
+        cx.tr.v[(size_t)list].items.push_back(id);
+    }
+    sim_add_node(cx, std::vector<int32_t>{list}, cx.sims);
+    int64_t pairs = 0;
+    const SimTable &t = cx.sims;
+    const int rc = kc_alignsim(t.nodes.data(), (int64_t)t.nodes.size(), t.vals.data(), (int64_t)t.vals.size(),
+                               reinterpret_cast<const uint8_t *>(t.chars.data()), (int64_t)t.chars.size(), out, t.out_len, -1, &pairs);
+    return rc ? rc : (int)pairs;
 }
 
 // generic_similarity (consensus_utils.py:892-917, default string method) of two JSON values; test hook of the native alignment.

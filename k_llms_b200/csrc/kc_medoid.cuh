@@ -26,16 +26,34 @@ constexpr int kMedoidMaxPattern = 64;  // the shorter string of every pair must 
 constexpr int kAlphabet = 36;
 constexpr int kPeqStride = 37;  // u64 per table: odd, so that lanes building different tables spread over the banks
 
-__device__ __forceinline__ int alnum_index(uint32_t c) { return (int)c - (c > 64u ? 'a' - 10 : '0'); }
+__host__ __device__ __forceinline__ int alnum_index(uint32_t c) { return (int)c - (c > 64u ? 'a' - 10 : '0'); }
+
+// read-only byte load: through the non-coherent cache on the device, a plain load in the host instantiation
+__host__ __device__ __forceinline__ uint8_t ld_ro(const uint8_t *p) {
+#ifdef __CUDA_ARCH__
+    return __ldg(p);
+#else
+    return *p;
+#endif
+}
+
+// Match table of a pattern of l <= 64 normalised characters: bit q of tab[c] is set where pattern[q] is symbol c.
+__host__ __device__ __forceinline__ void myers_table(uint64_t *tab, const uint8_t *__restrict__ s, int l) {
+#ifdef __CUDA_ARCH__
+#pragma unroll 4
+#endif
+    for (int c = 0; c < kAlphabet; ++c) tab[c] = 0;
+    for (int q = 0; q < l; ++q) tab[alnum_index(ld_ro(s + q))] |= 1ull << q;
+}
 
 // Edit distance of a pattern of m characters (match table peq) against text t.  Myers 1999 in Hyyro's formulation.
 template <typename W>
-__device__ __forceinline__ int myers(const uint64_t *peq, int m, const uint8_t *__restrict__ t, int tn) {
+__host__ __device__ __forceinline__ int myers(const uint64_t *peq, int m, const uint8_t *__restrict__ t, int tn) {
     W pv = ~W(0), mv = 0;
     int score = m;
     const int sh = m - 1;
     for (int k = 0; k < tn; ++k) {
-        const W eq = (W)peq[alnum_index(__ldg(t + k))];
+        const W eq = (W)peq[alnum_index(ld_ro(t + k))];
         const W xv = eq | mv;
         const W xh = (((eq & pv) + pv) ^ pv) | eq;
         W ph = mv | ~(xh | pv);
@@ -153,9 +171,7 @@ __global__ void __launch_bounds__(WARPS * 32) medoid_kernel(const uint8_t *__res
                 for (int q = 0; q < l; ++q) set |= 1ull << alnum_index(__ldg(chars + o + q));
                 tab[0] = set;
             } else if (method == 0 && l <= kMedoidMaxPattern) {
-#pragma unroll 4
-                for (int c = 0; c < kAlphabet; ++c) tab[c] = 0;
-                for (int q = 0; q < l; ++q) tab[alnum_index(__ldg(chars + o + q))] |= 1ull << q;
+                myers_table(tab, chars + o, l);
             }
             sim[a * kmax + a] = 1.0;  // identical strings: 1 - 0/max_len, or the empty-pair rule cu:756-757
         }

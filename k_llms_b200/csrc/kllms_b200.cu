@@ -20,6 +20,7 @@
 
 #include "../../include/kllms_b200.h"
 #include "kc_internal.h"
+#include "kc_alignsim.cuh"
 #include "kc_common.cuh"
 #include "kc_extra.cuh"
 #include "kc_medoid.cuh"
@@ -786,6 +787,60 @@ int kc_medoid_str_host(const uint8_t *h_chars, int64_t n_chars, const int32_t *h
         cudaStreamDestroy(st);
     }
     cudaFree(d);
+    return rc;
+}
+
+// Element similarities of the list-alignment pre-pass (kc_alignsim.cuh): H2D of the value table, one launch, D2H of the
+// matrices (synchronous); device < 0 runs the same phase on the calling host thread.
+int kc_alignsim(const KcAsNode *nodes, int64_t n_nodes, const KcAsVal *vals, int64_t n_vals, const uint8_t *chars, int64_t n_chars,
+                double *h_out, int64_t n_out, int device, int64_t *pairs) {
+    if (pairs) *pairs = 0;
+    if (n_nodes < 0 || n_vals < 0 || n_chars < 0 || n_out < 0) return kc_fail(KC_EINVAL, "kc_alignsim: negative size");
+    if (n_nodes == 0) return KC_OK;
+    if (!nodes || !vals || !h_out || (n_chars && !chars)) return kc_fail(KC_EINVAL, "kc_alignsim: NULL buffer");
+    if (device < 0) {
+        uint64_t tab[kc::kPeqStride];
+        int64_t decided = 0;
+        for (int64_t g = 0; g < n_nodes; ++g) decided += kc::alignsim_node(nodes[g], vals, chars, h_out, 0, 1, tab);
+        if (pairs) *pairs = decided;
+        return KC_OK;
+    }
+    KC_CUDA_I(cudaSetDevice(device));
+    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
+    const size_t b_nodes = up((size_t)n_nodes * sizeof(KcAsNode)), b_vals = up((size_t)n_vals * sizeof(KcAsVal)), b_chars = up((size_t)n_chars),
+                 b_out = (size_t)n_out * 8;
+    uint8_t *d = nullptr;
+    KC_CUDA_I(cudaMalloc(&d, 256 + b_nodes + b_vals + b_chars + b_out));
+    unsigned long long *d_pairs = reinterpret_cast<unsigned long long *>(d);
+    uint8_t *d_nodes = d + 256, *d_vals = d_nodes + b_nodes, *d_chars = d_vals + b_vals, *d_out = d_chars + b_chars;
+    int rc = KC_OK;
+    cudaStream_t st = nullptr;
+    auto guard = [&](cudaError_t e, const char *what) {
+        if (e != cudaSuccess && rc == KC_OK) rc = kc_fail(KC_ECUDA, "kc_alignsim: %s: %s", what, cudaGetErrorString(e));
+    };
+    guard(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking), "stream");
+    guard(cudaMemsetAsync(d_pairs, 0, 8, st), "memset");
+    guard(cudaMemcpyAsync(d_nodes, nodes, (size_t)n_nodes * sizeof(KcAsNode), cudaMemcpyHostToDevice, st), "H2D nodes");
+    if (n_vals) guard(cudaMemcpyAsync(d_vals, vals, (size_t)n_vals * sizeof(KcAsVal), cudaMemcpyHostToDevice, st), "H2D values");
+    if (n_chars) guard(cudaMemcpyAsync(d_chars, chars, (size_t)n_chars, cudaMemcpyHostToDevice, st), "H2D chars");
+    constexpr int WARPS = 4;
+    auto kernel = kc::alignsim_kernel<WARPS>;
+    int grid = 0;
+    if (rc == KC_OK) rc = persistent_grid(kernel, WARPS * 32, 0, (n_nodes + WARPS - 1) / WARPS, grid);
+    if (rc == KC_OK) {
+        kernel<<<grid, WARPS * 32, 0, st>>>(reinterpret_cast<const KcAsNode *>(d_nodes), n_nodes, reinterpret_cast<const KcAsVal *>(d_vals),
+                                            d_chars, reinterpret_cast<double *>(d_out), d_pairs);
+        guard(cudaGetLastError(), "launch");
+    }
+    unsigned long long decided = 0;
+    if (n_out) guard(cudaMemcpyAsync(h_out, d_out, b_out, cudaMemcpyDeviceToHost, st), "D2H matrices");
+    guard(cudaMemcpyAsync(&decided, d_pairs, 8, cudaMemcpyDeviceToHost, st), "D2H pairs");
+    if (st) {
+        guard(cudaStreamSynchronize(st), "sync");
+        cudaStreamDestroy(st);
+    }
+    cudaFree(d);
+    if (pairs) *pairs = (int64_t)decided;
     return rc;
 }
 
