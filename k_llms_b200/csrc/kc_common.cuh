@@ -1,5 +1,5 @@
-// kc_common.cuh — sm_90a PTX helpers shared by the consensus kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// streaming stores, the packed result word.  No libraries; inline PTX only.
+// kc_common.cuh — sm_90a PTX helpers shared by the consensus kernels: mbarrier, TMA (cp.async.bulk.tensor) and the
+// warp-private tile pipeline built on them, streaming stores, the packed result word.  No libraries; inline PTX only.
 #pragma once
 
 #include <cuda.h>
@@ -18,22 +18,22 @@ __host__ __device__ __forceinline__ uint32_t pack_meta(uint32_t idx, uint32_t su
            ((flags & 0x1Fu) << 27);
 }
 
-// ---------------------------------------------------------------- shared-memory addresses, mbarrier
+// ---------------------------------------------------------------- shared-memory addresses, mbarrier (32-bit shared-space addresses)
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 
-__device__ __forceinline__ void mbar_init(uint64_t *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
 }
 
 // make mbarrier.init visible to the async (TMA) proxy
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
 }
 
-__device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
     asm volatile(
         "{\n\t"
         ".reg .pred p;\n\t"
@@ -42,27 +42,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t *bar, uint32_t parity) {
         "@p bra KC_DONE_%=;\n\t"
         "bra KC_WAIT_%=;\n\t"
         "KC_DONE_%=:\n\t"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-
-// Variants taking 32-bit shared-space addresses (no generic->shared conversion in the loop).
-__device__ __forceinline__ void mbar_init_a(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx_a(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "KC_WAITA_%=:\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-        "@p bra KC_DONEA_%=;\n\t"
-        "bra KC_WAITA_%=;\n\t"
-        "KC_DONEA_%=:\n\t"
         "}\n" ::"r"(bar),
         "r"(parity)
         : "memory");
@@ -90,28 +69,145 @@ __device__ __forceinline__ uint64_t policy_evict_normal() {
     return pol;
 }
 
-__device__ __forceinline__ void tma_load_2d(void *smem_dst, const CUtensorMap *map, int32_t c0, int32_t c1, uint64_t *bar,
+__device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap *map, int32_t c0, int32_t c1, uint32_t bar,
                                             uint64_t policy) {
     asm volatile(
         "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], "
-        "[%4], %5;" ::"r"(smem_u32(smem_dst)),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(smem_u32(bar)), "l"(policy)
+        "[%4], %5;" ::"r"(smem_dst),
+        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar), "l"(policy)
         : "memory");
 }
 
-// 32-bit shared-space addresses + dependency register.
-__device__ __forceinline__ void tma_load_2d_a(uint32_t smem_dst, const CUtensorMap *map, int32_t c0, int32_t c1, uint32_t bar,
-                                              uint64_t policy, uint32_t dep) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 kc_dep;\n\t"
-        "mov.b32 kc_dep, %6;\n\t"
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%2, %3}], "
-        "[%4], %5;\n\t"
-        "}\n" ::"r"(smem_dst),
-        "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar), "l"(policy), "r"(dep)
-        : "memory");
+// contiguous bytes, global -> smem (16-byte aligned, a multiple of 16 bytes)
+__device__ __forceinline__ void bulk_load_1d(uint32_t smem_dst, const void *src, uint32_t bytes, uint32_t bar) {
+    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_dst),
+                 "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar)
+                 : "memory");
 }
+
+// ---------------------------------------------------------------- the warp-private tile pipeline of the TMA front-ends
+
+template <int ROW_BYTES>
+struct Swizzle {  // TMA swizzle mode for a row of ROW_BYTES (rows wider than 128 B are split into 128 B box rows)
+    static constexpr uint32_t kMask = ROW_BYTES >= 128 ? 7u : (ROW_BYTES == 64 ? 3u : 1u);
+    __device__ static __forceinline__ uint32_t apply(uint32_t off) { return off ^ (((off >> 7) & kMask) << 4); }
+};
+
+// A further copy that lands on a tile's barrier next to the tile: `bytes` from `src` to the shared-space address `dst`;
+// none if `src` is null.
+struct ExtraCopy {
+    const void *src;
+    uint32_t dst, bytes;
+};
+struct NoExtraCopy {
+    __device__ ExtraCopy operator()(uint32_t, uint32_t) const { return {nullptr, 0u, 0u}; }
+};
+
+enum class L2Policy { evict_first, evict_normal };
+
+// Persistent kernels, warp-private pipelines.  Global warp w owns warp-tiles w, w + W, ... (W = warps in the grid); a
+// warp-tile is 32 consecutive rows of ROW_BYTES (one group each) and lane l owns row l.  Each warp keeps STAGES tiles in
+// flight in its own ring of swizzled shared-memory tiles: lane 0 arms the stage's mbarrier with the tile's byte count and
+// issues one cp.async.bulk.tensor.2d; all lanes wait on the barrier and pull their row with swizzled (bank-conflict-free)
+// LDS; release() hands the stage back for the tile STAGES ahead before the warp computes.  Out-of-range rows of the last
+// tile are zero-filled by TMA and never stored.  There is no __syncthreads(): warps never wait for each other.  All indices
+// are 32-bit: the launchers cut the input into slabs of < 2^28 groups.
+//
+//     WarpTiles<ROW_BYTES, WARPS, STAGES> tiles(&tmap, n_groups);
+//     tiles.start(L2Policy::evict_first);
+//     for (; tiles.t < tiles.n_tiles; tiles.next()) {
+//         const uint32_t tile = tiles.wait();   // LDS at tile + tiles.at(byte of the row)
+//         tiles.release(dep);                   // dep: computed from every load of the tile
+//         ...                                   // group tiles.t * 32 + lane, from registers
+//     }
+//
+// The dynamic shared memory holds the WARPS rings from its first 1024-byte boundary on; a kernel keeps its own data
+// from end() on.
+template <int ROW_BYTES, int WARPS, int STAGES>
+struct WarpTiles {
+    static constexpr uint32_t BOX_ROWS_PER_GROUP = ROW_BYTES > 128 ? ROW_BYTES / 128 : 1;
+    static constexpr uint32_t TILE_BYTES = 32 * ROW_BYTES;
+    static_assert(TILE_BYTES % 1024 == 0, "warp tile must keep the swizzle atom alignment");
+    static_assert((STAGES & (STAGES - 1)) == 0, "STAGES must be a power of two");
+
+    const CUtensorMap *map;
+    uint32_t lane, warp;
+    uint32_t base, ring, bar;  // shared-space addresses: all rings, this warp's ring, this warp's STAGES barriers
+    uint32_t t, step, n_tiles;  // the current tile; the walk
+    uint32_t it = 0;            // tiles done: stage it % STAGES, barrier phase (it / STAGES) & 1
+    uint64_t policy = 0;        // lane 0's
+
+    __device__ __forceinline__ WarpTiles(const CUtensorMap *tmap, uint32_t n_groups) : map(tmap) {
+        extern __shared__ __align__(1024) uint8_t smem_raw[];
+        __shared__ __align__(8) uint64_t full_bar[WARPS * STAGES];
+        lane = threadIdx.x & 31;
+        warp = __shfl_sync(0xFFFFFFFFu, threadIdx.x >> 5, 0);  // warp-uniform by construction
+        base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+        ring = base + warp * (STAGES * TILE_BYTES);
+        bar = smem_u32(full_bar) + warp * (STAGES * 8);
+        n_tiles = (n_groups + 31u) >> 5;
+        t = blockIdx.x * WARPS + warp;
+        step = gridDim.x * WARPS;
+    }
+
+    // lane 0 sets up the barriers and requests the first STAGES tiles
+    template <class Extra = NoExtraCopy>
+    __device__ __forceinline__ void start(L2Policy l2, const Extra &extra = {}) {
+        if (lane == 0) {
+            tma_prefetch_desc(map);
+#pragma unroll
+            for (int s = 0; s < STAGES; ++s) mbar_init(bar + s * 8, 1);
+            fence_barrier_init();
+            policy = l2 == L2Policy::evict_first ? policy_evict_first() : policy_evict_normal();
+#pragma unroll
+            for (int s = 0; s < STAGES; ++s) {
+                const uint32_t ts = t + (uint32_t)s * step;
+                if (ts < n_tiles) arm(ts, (uint32_t)s, 0u, extra);
+            }
+        }
+        __syncwarp();
+    }
+
+    // waits for the current tile; its shared-space address
+    __device__ __forceinline__ uint32_t wait() const {
+        const uint32_t s = it & (STAGES - 1), tile = ring + s * TILE_BYTES;  // before the wait: LDS can issue right after it
+        mbar_wait(bar + s * 8, (it / STAGES) & 1);
+        return tile;
+    }
+
+    // swizzled offset of byte `byte` of this lane's row inside a tile
+    __device__ __forceinline__ uint32_t at(uint32_t byte) const { return Swizzle<ROW_BYTES>::apply(lane * ROW_BYTES + byte); }
+
+    // Hands the current stage back: lane 0 requests the tile STAGES ahead into it.  Every row must be in registers first.
+    // `dep` depends on every load the lane made from the tile, a warp instruction issues only when its operands are ready
+    // in every lane, and the shuffle is one: `order` is 0 on lane 0 but only the hardware knows it (a shuffle result), so
+    // folding it into the TMA coordinate gives the copy a true register dependency on the loaded data, which neither nvvm
+    // nor ptxas can schedule away.
+    template <class Extra = NoExtraCopy>
+    __device__ __forceinline__ void release(uint32_t dep, const Extra &extra = {}) const {
+        const uint32_t order = __shfl_sync(0xFFFFFFFFu, dep, 0) ^ dep;
+        const uint32_t tn = t + STAGES * step;
+        if (lane == 0 && tn < n_tiles) arm(tn, it + STAGES, order, extra);
+    }
+
+    __device__ __forceinline__ void next() {
+        t += step;
+        ++it;
+    }
+
+    // first shared-space address past the rings of all warps
+    __device__ __forceinline__ uint32_t end() const { return base + WARPS * STAGES * TILE_BYTES; }
+
+    // tile `tt`, the warp's tile number `j` (stage j % STAGES), plus what `extra(tt, j)` asks for, on the stage's barrier
+    template <class Extra>
+    __device__ __forceinline__ void arm(uint32_t tt, uint32_t j, uint32_t dep, const Extra &extra) const {
+        const uint32_t s = j & (STAGES - 1), b = bar + s * 8;
+        const ExtraCopy x = extra(tt, j);
+        mbar_arrive_expect_tx(b, TILE_BYTES + x.bytes);
+        tma_load_2d(ring + s * TILE_BYTES, map, 0, (int32_t)(tt * 32 * BOX_ROWS_PER_GROUP + dep), b, policy);
+        if (x.src) bulk_load_1d(x.dst, x.src, x.bytes, b);
+    }
+};
 
 // ---------------------------------------------------------------- global memory: streaming loads / stores
 

@@ -527,10 +527,9 @@ __device__ __forceinline__ void wv_warp_walk(uint32_t lane, uint32_t owner, cons
     }
 }
 
-// K3b with K1's TMA front-end (n in {32, 64} cells per group = 128 / 256 byte rows): every WARP runs its own pipeline of STAGES
-// tiles of 32 consecutive groups (one cp.async.bulk.tensor.2d per tile, hardware swizzle, the warp's own mbarrier, conflict-free
-// LDS.128; see vote_tma_kernel) instead of one 128-byte row per thread straight from global memory (latency-bound at 0.39 of the
-// HBM peak: a warp's 32 rows are 32 separate lines per load instruction).  The weights of the tile's records (32 groups span
+// K3b with K1's TMA front-end (n in {32, 64} cells per group = 128 / 256 byte rows; WarpTiles, kc_common.cuh) instead of one
+// 128-byte row per thread straight from global memory (latency-bound at 0.39 of the HBM peak: a warp's 32 rows are 32 separate
+// lines per load instruction).  The weights of the tile's records (32 groups span
 // 32 / n_fields + 2 records at most) are computed by the warp itself into its own shared-memory rows (lane = candidate, warp
 // max by shuffles), padded by one float so that lanes of different records read different banks; the pad slot carries the index of
 // the record's heaviest candidate, whose class weighted_core sums in its first pass (one pass decides most groups).  No block-wide
@@ -540,49 +539,15 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
                                                                        uint32_t n_groups, FieldMap fm, bool has_nc, int rec_cap, uint64_t inv_fields,
                                                                        int32_t *__restrict__ win, uint32_t *__restrict__ meta,
                                                                        float *__restrict__ weight) {
-    constexpr int ROW_BYTES = N * 4;
-    constexpr int BOX_ROWS_PER_GROUP = ROW_BYTES > 128 ? ROW_BYTES / 128 : 1;
-    constexpr uint32_t TILE_BYTES = 32 * ROW_BYTES;
     constexpr int WROW = N + 1;
     // x / n_fields for any 32-bit x without a division: inv_fields = floor(2^64 / n_fields) + 1 (exact for n_fields >= 2)
     auto record_of = [&](uint32_t x) -> uint32_t { return fm.n_fields == 1u ? x : (uint32_t)__umul64hi((uint64_t)x, inv_fields); };
-    static_assert(TILE_BYTES % 1024 == 0, "warp tile must keep the swizzle atom alignment");
-    static_assert((STAGES & (STAGES - 1)) == 0, "STAGES must be a power of two");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[WARPS * STAGES];
-
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warp = __shfl_sync(0xFFFFFFFFu, threadIdx.x >> 5, 0);
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t my_smem = smem_base + warp * (STAGES * TILE_BYTES);
-    const uint32_t my_bar = smem_u32(full_bar) + warp * (STAGES * 8);
+    WarpTiles<N * 4, WARPS, STAGES> tiles(&tmap, n_groups);
+    const uint32_t lane = tiles.lane;
     // the weight rows live behind the tiles of all warps
-    float *wts = reinterpret_cast<float *>(smem_raw + (smem_base - smem_u32(smem_raw)) + (size_t)WARPS * STAGES * TILE_BYTES) +
-                 (size_t)warp * rec_cap * WROW;
-
-    const uint32_t n_tiles = (n_groups + 31u) >> 5;
-    const uint32_t first = blockIdx.x * WARPS + warp;
-    const uint32_t step = gridDim.x * WARPS;
-    uint64_t policy = 0;
-    if (lane == 0) {
-        tma_prefetch_desc(&tmap);
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) mbar_init_a(my_bar + s * 8, 1);
-        fence_barrier_init();
-        policy = policy_evict_first();
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) {
-            const uint32_t t = first + (uint32_t)s * step;
-            if (t < n_tiles) {
-                mbar_arrive_expect_tx_a(my_bar + s * 8, TILE_BYTES);
-                tma_load_2d_a(my_smem + s * TILE_BYTES, &tmap, 0, (int32_t)(t * 32 * BOX_ROWS_PER_GROUP), my_bar + s * 8, policy, 0);
-            }
-        }
-    }
-    __syncwarp();
-    uint32_t piece[N / 4];
-#pragma unroll
-    for (int q = 0; q < N / 4; ++q) piece[q] = Swizzle<ROW_BYTES>::apply(lane * ROW_BYTES + q * 16);
+    float *wts = reinterpret_cast<float *>(smem_raw + (tiles.end() - smem_u32(smem_raw))) + (size_t)tiles.warp * rec_cap * WROW;
+    tiles.start(L2Policy::evict_first);
 
     // The sequence logprobs of a tile's records are requested one tile AHEAD (a warp works through its tiles one after the other:
     // a global-memory round trip per tile in front of the weights would be exposed every time).  Up to PF records per tile are
@@ -603,15 +568,11 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
             }
         }
     };
-    if (prefetch && first < n_tiles) fetch(first, cur_lo, cur_hi);
+    if (prefetch && tiles.t < tiles.n_tiles) fetch(tiles.t, cur_lo, cur_hi);
 
-    uint32_t it = 0;
-    for (uint32_t t = first; t < n_tiles; t += step, ++it) {
-        const uint32_t stage = it & (STAGES - 1);
-        const uint32_t parity = (it / STAGES) & 1;
-        const uint32_t bar = my_bar + stage * 8;
-        const uint32_t tile = my_smem + stage * TILE_BYTES;
-        if (prefetch && t + step < n_tiles) fetch(t + step, nxt_lo, nxt_hi);
+    for (; tiles.t < tiles.n_tiles; tiles.next()) {
+        const uint32_t t = tiles.t;
+        if (prefetch && t + tiles.step < tiles.n_tiles) fetch(t + tiles.step, nxt_lo, nxt_hi);
         // the weights of this tile's records, while the tile is still on its way
         const uint32_t g0 = t * 32, g_last = min(g0 + 31u, n_groups - 1u);
         const uint32_t r0 = record_of(g0), r_last = record_of(g_last);
@@ -638,11 +599,11 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
             if (lane == 0) w[N] = __int_as_float(imax);
         }
         __syncwarp();
-        mbar_wait_a(bar, parity);
+        const uint32_t tile = tiles.wait();
         int32_t raw[N];
 #pragma unroll
         for (int q = 0; q < N / 4; ++q) {
-            const int4 v4 = lds_v4(tile + piece[q]);
+            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
             raw[4 * q + 0] = v4.x;
             raw[4 * q + 1] = v4.y;
             raw[4 * q + 2] = v4.z;
@@ -656,16 +617,10 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
         const int imax = __float_as_int(wrow[N]);
         int32_t graw = KC_CODE_NONE - 1;
         if (imax < N) {
-            asm volatile("ld.shared.s32 %0, [%1];" : "=r"(graw) : "r"(tile + Swizzle<ROW_BYTES>::apply(lane * ROW_BYTES + (uint32_t)imax * 4u)));
+            asm volatile("ld.shared.s32 %0, [%1];" : "=r"(graw) : "r"(tile + tiles.at((uint32_t)imax * 4u)));
         }
-        // hand the stage back to the TMA unit only after every lane's row is in registers (see vote_tma_kernel)
         const int32_t lo = min(row_min<N>(raw), graw);
-        const uint32_t order = __shfl_sync(0xFFFFFFFFu, (uint32_t)lo, 0) ^ (uint32_t)lo;
-        const uint32_t tn = t + STAGES * step;
-        if (lane == 0 && tn < n_tiles) {
-            mbar_arrive_expect_tx_a(bar, TILE_BYTES);
-            tma_load_2d_a(tile, &tmap, 0, (int32_t)(tn * 32 * BOX_ROWS_PER_GROUP + order), bar, policy, 0);
-        }
+        tiles.release((uint32_t)lo);
         WvFirst<N> f;
         bool undecided = false;
         int32_t o_code = KC_CODE_NONE;
@@ -724,90 +679,40 @@ __global__ void __launch_bounds__(256) weight_rows_kernel(const float *__restric
     }
 }
 
-__device__ __forceinline__ void bulk_load_1d_a(uint32_t smem_dst, const void *src, uint32_t bytes, uint32_t bar, uint32_t dep) {
-    asm volatile(
-        "{\n\t"
-        ".reg .b32 kc_dep1;\n\t"
-        "mov.b32 kc_dep1, %4;\n\t"
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];\n\t"
-        "}\n" ::"r"(smem_dst),
-        "l"(reinterpret_cast<uint64_t>(src)), "r"(bytes), "r"(bar), "r"(dep)
-        : "memory");
-}
-
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
 __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kernel(const __grid_constant__ CUtensorMap tmap, const float *__restrict__ wrows,
                                                                         uint32_t n_groups, FieldMap fm, bool has_nc, int rec_cap, uint64_t inv_fields,
                                                                         int32_t *__restrict__ win, uint32_t *__restrict__ meta,
                                                                         float *__restrict__ weight) {
-    constexpr int ROW_BYTES = N * 4;
-    constexpr int BOX_ROWS_PER_GROUP = ROW_BYTES > 128 ? ROW_BYTES / 128 : 1;
-    constexpr uint32_t TILE_BYTES = 32 * ROW_BYTES;
     constexpr int WROW = N + 4;
     constexpr int WSLOTS = STAGES + 1;  // the slot of the tile being voted is not the one the re-arm refills
     auto record_of = [&](uint32_t x) -> uint32_t { return fm.n_fields == 1u ? x : (uint32_t)__umul64hi((uint64_t)x, inv_fields); };
-    static_assert(TILE_BYTES % 1024 == 0, "warp tile must keep the swizzle atom alignment");
-    static_assert((STAGES & (STAGES - 1)) == 0, "STAGES must be a power of two");
     extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[WARPS * STAGES];
-
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warp = __shfl_sync(0xFFFFFFFFu, threadIdx.x >> 5, 0);
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t my_smem = smem_base + warp * (STAGES * TILE_BYTES);
-    const uint32_t my_bar = smem_u32(full_bar) + warp * (STAGES * 8);
+    WarpTiles<N * 4, WARPS, STAGES> tiles(&tmap, n_groups);
+    const uint32_t lane = tiles.lane;
     const uint32_t slot_bytes = (uint32_t)rec_cap * WROW * 4;
-    const uint32_t my_rows = smem_base + WARPS * STAGES * TILE_BYTES + warp * (WSLOTS * slot_bytes);     // shared-space address
+    const uint32_t my_rows = tiles.end() + tiles.warp * (WSLOTS * slot_bytes);                           // shared-space address
     const float *my_rows_p = reinterpret_cast<const float *>(smem_raw + (my_rows - smem_u32(smem_raw)));  // the same, generic
-
-    const uint32_t n_tiles = (n_groups + 31u) >> 5;
-    const uint32_t first = blockIdx.x * WARPS + warp;
-    const uint32_t step = gridDim.x * WARPS;
-    uint64_t policy = 0;
-    // one tile's copies: the 32 rows of cells and the weight rows of the records they belong to, on one barrier
-    auto request = [&](uint32_t t, uint32_t stage, uint32_t slot, uint32_t dep) {
-        const uint32_t a = t * 32, b = min(a + 31u, n_groups - 1u);
+    // the weight rows of the records tile tt belongs to, into the weight slot of the warp's tile number j
+    auto weight_rows = [&](uint32_t tt, uint32_t j) -> ExtraCopy {
+        const uint32_t a = tt * 32, b = min(a + 31u, n_groups - 1u);
         const uint32_t ra = record_of(a), rb = record_of(b);
-        const uint32_t wbytes = (rb - ra + 1u) * WROW * 4;
-        const uint32_t bar = my_bar + stage * 8;
-        mbar_arrive_expect_tx_a(bar, TILE_BYTES + wbytes);
-        tma_load_2d_a(my_smem + stage * TILE_BYTES, &tmap, 0, (int32_t)(t * 32 * BOX_ROWS_PER_GROUP + dep), bar, policy, 0);
-        bulk_load_1d_a(my_rows + slot * slot_bytes, wrows + (size_t)ra * WROW, wbytes, bar, dep);
+        return {wrows + (size_t)ra * WROW, my_rows + (j % WSLOTS) * slot_bytes, (rb - ra + 1u) * WROW * 4};
     };
-    if (lane == 0) {
-        tma_prefetch_desc(&tmap);
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) mbar_init_a(my_bar + s * 8, 1);
-        fence_barrier_init();
-        policy = policy_evict_first();
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) {
-            const uint32_t t = first + (uint32_t)s * step;
-            if (t < n_tiles) request(t, (uint32_t)s, (uint32_t)s, 0u);
-        }
-    }
-    __syncwarp();
-    uint32_t piece[N / 4];
-#pragma unroll
-    for (int q = 0; q < N / 4; ++q) piece[q] = Swizzle<ROW_BYTES>::apply(lane * ROW_BYTES + q * 16);
+    tiles.start(L2Policy::evict_first, weight_rows);
 
-    uint32_t it = 0, slot = 0;  // slot = it % WSLOTS
-    for (uint32_t t = first; t < n_tiles; t += step, ++it) {
-        const uint32_t stage = it & (STAGES - 1);
-        const uint32_t parity = (it / STAGES) & 1;
-        const uint32_t bar = my_bar + stage * 8;
-        const uint32_t tile = my_smem + stage * TILE_BYTES;
-        const uint32_t g0 = t * 32, g = g0 + lane;
+    for (; tiles.t < tiles.n_tiles; tiles.next()) {
+        const uint32_t g0 = tiles.t * 32, g = g0 + lane;
         const uint32_t r0 = record_of(g0);
         const uint32_t fpos = (g0 - r0 * fm.n_fields) + lane;  // offset inside the tile's first record: < n_fields + 32
         const uint32_t rec_local = g < n_groups ? fm.div_small(fpos) : 0u;
-        const float *wts = my_rows_p + slot * (slot_bytes / 4);
+        const float *wts = my_rows_p + (tiles.it % WSLOTS) * (slot_bytes / 4);
         const float *wrow = wts + rec_local * WROW;
-        mbar_wait_a(bar, parity);
+        const uint32_t tile = tiles.wait();
         int32_t raw[N];
 #pragma unroll
         for (int q = 0; q < N / 4; ++q) {
-            const int4 v4 = lds_v4(tile + piece[q]);
+            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
             raw[4 * q + 0] = v4.x;
             raw[4 * q + 1] = v4.y;
             raw[4 * q + 2] = v4.z;
@@ -817,14 +722,11 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kerne
         const int imax = __float_as_int(wrow[N]);
         int32_t graw = KC_CODE_NONE - 1;
         if (imax < N) {
-            asm volatile("ld.shared.s32 %0, [%1];" : "=r"(graw) : "r"(tile + Swizzle<ROW_BYTES>::apply(lane * ROW_BYTES + (uint32_t)imax * 4u)));
+            asm volatile("ld.shared.s32 %0, [%1];" : "=r"(graw) : "r"(tile + tiles.at((uint32_t)imax * 4u)));
         }
-        // hand the stage back only after every lane's row is in registers (see vote_tma_kernel); the shuffle also means that
-        // every lane has left the previous tile, whose weight slot the request below refills
+        // the release's shuffle also means that every lane has left the previous tile, whose weight slot it refills
         const int32_t lo = min(row_min<N>(raw), graw);
-        const uint32_t order = __shfl_sync(0xFFFFFFFFu, (uint32_t)lo, 0) ^ (uint32_t)lo;
-        const uint32_t tn = t + STAGES * step;
-        if (lane == 0 && tn < n_tiles) request(tn, stage, (slot + STAGES) % WSLOTS, order);
+        tiles.release((uint32_t)lo, weight_rows);
         WvFirst<N> f;
         bool undecided = false;
         int32_t o_code = KC_CODE_NONE;
@@ -848,7 +750,6 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kerne
             meta[g] = o_meta;
             weight[g] = o_weight;
         }
-        slot = slot + 1 == WSLOTS ? 0u : slot + 1;
     }
 }
 

@@ -22,7 +22,7 @@
 
 #include "kc_common.cuh"
 #include "kc_csa.cuh"
-#include "kc_vote.cuh"  // MaskOf, Swizzle, popc_m
+#include "kc_vote.cuh"  // MaskOf, popc_m
 
 namespace kc {
 
@@ -1061,58 +1061,27 @@ __global__ void __launch_bounds__(T) numeric_direct_fast_kernel(const double *__
 // and nothing is read twice.
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
 __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_fast_kernel(const __grid_constant__ CUtensorMap tmap,
-                                                                      const double *__restrict__ in, int64_t n_groups,
+                                                                      const double *__restrict__ in, uint32_t n_groups,
                                                                       double rel_eps, double abs_eps,
                                                                       double *__restrict__ out_value,
-                                                                      uint32_t *__restrict__ out_meta, const __grid_constant__ OutRoute /* local only: see the launcher */) {
-    constexpr int ROW_BYTES = N * 8;
-    constexpr int BOX_ROWS_PER_GROUP = ROW_BYTES > 128 ? ROW_BYTES / 128 : 1;
-    constexpr uint32_t TILE_BYTES = 32 * ROW_BYTES;
+                                                                      uint32_t *__restrict__ out_meta) {
     constexpr int T = WARPS * 32;
-    static_assert(TILE_BYTES % 1024 == 0, "warp tile must keep the swizzle atom alignment");
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ __align__(8) uint64_t full_bar[WARPS * STAGES];
-    __shared__ int64_t defer_q[WARPS][64];
+    WarpTiles<N * 8, WARPS, STAGES> tiles(&tmap, n_groups);
+    __shared__ uint32_t defer_q[WARPS][64];
 
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    uint8_t *my_smem = smem + (size_t)warp * STAGES * TILE_BYTES;
-    uint64_t *my_bar = full_bar + warp * STAGES;
-    int64_t *my_q = defer_q[warp];
+    const uint32_t lane = tiles.lane;
+    uint32_t *my_q = defer_q[tiles.warp];
     int q_count = 0;  // warp-uniform
-    const PlaneRow row{smem_u32(smem + (size_t)WARPS * STAGES * TILE_BYTES) + threadIdx.x * 8u, T * 8u};
+    const PlaneRow row{tiles.end() + threadIdx.x * 8u, T * 8u};
     const double thr = abs_eps > rel_eps ? abs_eps : rel_eps;
-
-    const int64_t n_tiles = (n_groups + 31) >> 5;
-    const int64_t first = (int64_t)blockIdx.x * WARPS + warp;
-    const int64_t step = (int64_t)gridDim.x * WARPS;
-    uint64_t policy = 0;
-
-    if (lane == 0) {
-        tma_prefetch_desc(&tmap);
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) mbar_init(&my_bar[s], 1);
-        fence_barrier_init();
-        policy = policy_evict_normal();
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) {
-            const int64_t t = first + (int64_t)s * step;
-            if (t < n_tiles) {
-                mbar_arrive_expect_tx(&my_bar[s], TILE_BYTES);
-                tma_load_2d(my_smem + (size_t)s * TILE_BYTES, &tmap, 0, (int32_t)(t * 32 * BOX_ROWS_PER_GROUP), &my_bar[s],
-                            policy);
-            }
-        }
-    }
-    __syncwarp();
+    tiles.start(L2Policy::evict_normal);
 
     // Deferred groups wait in the warp's 32 plane rows (slot s = the row of lane s) with their group index in my_q;
     // drain: the first `count` of them through the general path, one per lane.
-    const uint32_t warp_plane = smem_u32(smem + (size_t)WARPS * STAGES * TILE_BYTES) + (uint32_t)warp * 32u * 8u;
+    const uint32_t warp_plane = tiles.end() + tiles.warp * 32u * 8u;
     auto drain = [&](int count) {
-        if (lane < count) {
-            const int64_t g = my_q[lane];
+        if ((int)lane < count) {
+            const uint32_t g = my_q[lane];
             uint32_t hi[N];
 #pragma unroll
             for (int i = 0; i < N; ++i) hi[i] = lds_u32x2(row.addr(i)).y;
@@ -1125,17 +1094,13 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_fast_kernel(
         __syncwarp();
     };
 
-    int stage = 0;
-    uint32_t parity = 0;
-    for (int64_t t = first; t < n_tiles; t += step) {
-        mbar_wait(&my_bar[stage], parity);
-        const uint32_t base = smem_u32(my_smem + (size_t)stage * TILE_BYTES);
-        const uint32_t row_off = (uint32_t)lane * ROW_BYTES;
+    for (; tiles.t < tiles.n_tiles; tiles.next()) {
+        const uint32_t tile = tiles.wait();
         uint32_t x[N], lo[N];  // x = high word + kFastBias
         uint32_t touch = 0, top = 0;
 #pragma unroll
         for (int q = 0; q < N / 2; ++q) {
-            const int4 v4 = lds_v4(base + Swizzle<ROW_BYTES>::apply(row_off + q * 16));
+            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
             lo[2 * q + 0] = (uint32_t)v4.x;
             x[2 * q + 0] = (uint32_t)v4.y + kFastBias;
             lo[2 * q + 1] = (uint32_t)v4.z;
@@ -1143,17 +1108,8 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_fast_kernel(
             top = max(top, max((uint32_t)v4.y, (uint32_t)v4.w));
             touch |= (uint32_t)v4.w;  // one word of every LDS.128 is enough to depend on all of them
         }
-        // the tile is in registers: hand the stage back (see numeric_tma_kernel for the ordering argument)
-        const uint32_t order = __shfl_sync(0xFFFFFFFFu, touch, 0) ^ touch;
-        if (lane == 0) {
-            const int64_t tn = t + (int64_t)STAGES * step;
-            if (tn < n_tiles) {
-                mbar_arrive_expect_tx(&my_bar[stage], TILE_BYTES);
-                tma_load_2d(my_smem + (size_t)stage * TILE_BYTES, &tmap, 0,
-                            (int32_t)(tn * 32 * BOX_ROWS_PER_GROUP) + (int32_t)order, &my_bar[stage], policy);
-            }
-        }
-        const int64_t g = t * 32 + lane;
+        tiles.release(touch);
+        const uint32_t g = tiles.t * 32 + lane;
         FastDecision fd;
         const bool decided = numeric_fast_decide<N>(x, lo, top, rel_eps, thr, fd);
         const bool defer = !decided && g < n_groups;
@@ -1179,11 +1135,11 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_fast_kernel(
         if (q_count >= 32) {  // nothing of this tile is live in registers any more
             drain(32);
             q_count -= 32;
-            const int64_t moved = (lane < q_count) ? my_q[32 + lane] : 0;
+            const uint32_t moved = ((int)lane < q_count) ? my_q[32 + lane] : 0u;
             __syncwarp();
-            if (lane < q_count) {  // the overflow (a few groups at most): fetch their cells again
+            if ((int)lane < q_count) {  // the overflow (a few groups at most): fetch their cells again
                 my_q[lane] = moved;
-                const int4 *p4 = reinterpret_cast<const int4 *>(in + moved * N);
+                const int4 *p4 = reinterpret_cast<const int4 *>(in + (size_t)moved * N);
 #pragma unroll
                 for (int q = 0; q < N / 2; ++q) {
                     const int4 v4 = ldg_nc_v4(p4 + q);
@@ -1193,99 +1149,42 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_fast_kernel(
             }
             __syncwarp();
         }
-        if (++stage == STAGES) {
-            stage = 0;
-            parity ^= 1;
-        }
     }
     if (q_count > 0) drain(q_count);
 }
 
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
 __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_kernel(const __grid_constant__ CUtensorMap tmap,
-                                                                 int64_t n_groups, double rel_eps, double abs_eps,
+                                                                 uint32_t n_groups, double rel_eps, double abs_eps,
                                                                  double *__restrict__ out_value,
                                                                  uint32_t *__restrict__ out_meta, const __grid_constant__ OutRoute mc) {
-    constexpr int ROW_BYTES = N * 8;
-    constexpr int BOX_ROWS_PER_GROUP = ROW_BYTES > 128 ? ROW_BYTES / 128 : 1;
-    constexpr uint32_t TILE_BYTES = 32 * ROW_BYTES;
     constexpr int T = WARPS * 32;
-    static_assert(TILE_BYTES % 1024 == 0, "warp tile must keep the swizzle atom alignment");
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    uint8_t *smem = reinterpret_cast<uint8_t *>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-    __shared__ __align__(8) uint64_t full_bar[WARPS * STAGES];
-
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    uint8_t *my_smem = smem + (size_t)warp * STAGES * TILE_BYTES;
-    uint64_t *my_bar = full_bar + warp * STAGES;
-    const PlaneRow row{smem_u32(smem + (size_t)WARPS * STAGES * TILE_BYTES) + threadIdx.x * 8u, T * 8u};
+    WarpTiles<N * 8, WARPS, STAGES> tiles(&tmap, n_groups);
+    const PlaneRow row{tiles.end() + threadIdx.x * 8u, T * 8u};
     const double thr = abs_eps > rel_eps ? abs_eps : rel_eps;
+    tiles.start(L2Policy::evict_normal);
 
-    const int64_t n_tiles = (n_groups + 31) >> 5;
-    const int64_t first = (int64_t)blockIdx.x * WARPS + warp;
-    const int64_t step = (int64_t)gridDim.x * WARPS;
-    uint64_t policy = 0;
-
-    if (lane == 0) {
-        tma_prefetch_desc(&tmap);
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) mbar_init(&my_bar[s], 1);
-        fence_barrier_init();
-        policy = policy_evict_normal();
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) {
-            const int64_t t = first + (int64_t)s * step;
-            if (t < n_tiles) {
-                mbar_arrive_expect_tx(&my_bar[s], TILE_BYTES);
-                tma_load_2d(my_smem + (size_t)s * TILE_BYTES, &tmap, 0, (int32_t)(t * 32 * BOX_ROWS_PER_GROUP), &my_bar[s],
-                            policy);
-            }
-        }
-    }
-    __syncwarp();
-
-    int stage = 0;
-    uint32_t parity = 0;
-    for (int64_t t = first; t < n_tiles; t += step) {
-        mbar_wait(&my_bar[stage], parity);
-        const uint32_t base = smem_u32(my_smem + (size_t)stage * TILE_BYTES);
-        const uint32_t row_off = (uint32_t)lane * ROW_BYTES;
+    for (; tiles.t < tiles.n_tiles; tiles.next()) {
+        const uint32_t tile = tiles.wait();
         uint32_t hi[N];
         uint32_t touch = 0;
 #pragma unroll
         for (int q = 0; q < N / 2; ++q) {
-            const int4 v4 = lds_v4(base + Swizzle<ROW_BYTES>::apply(row_off + q * 16));
+            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
             hi[2 * q + 0] = (uint32_t)v4.y;
             hi[2 * q + 1] = (uint32_t)v4.w;
             sts_f64(row.addr(2 * q + 0), __hiloint2double(v4.y, v4.x));
             sts_f64(row.addr(2 * q + 1), __hiloint2double(v4.w, v4.z));
             touch |= (uint32_t)v4.w;  // one word of every LDS.128 is enough to depend on all of them
         }
-        // the tile is in registers (touch depends on every LDS, and a warp instruction issues only when all lanes'
-        // operands are ready): hand the stage back
-        // 0 on lane 0, but only the hardware knows (shuffle result): a true register dependency of the copy on the
-        // loaded data that neither nvvm nor ptxas can schedule away
-        const uint32_t order = __shfl_sync(0xFFFFFFFFu, touch, 0) ^ touch;
-        if (lane == 0) {
-            const int64_t tn = t + (int64_t)STAGES * step;
-            if (tn < n_tiles) {
-                mbar_arrive_expect_tx(&my_bar[stage], TILE_BYTES);
-                tma_load_2d(my_smem + (size_t)stage * TILE_BYTES, &tmap, 0,
-                            (int32_t)(tn * 32 * BOX_ROWS_PER_GROUP) + (int32_t)order, &my_bar[stage], policy);
-            }
-        }
-        const int64_t g = t * 32 + lane;
+        tiles.release(touch);
+        const uint32_t g = tiles.t * 32 + tiles.lane;
         if (g < n_groups) {
             double v;
             uint32_t m;
             numeric_core<N, PlaneRow>(hi, row, rel_eps, abs_eps, thr, v, m);
             store_out_f64(out_value + g, v, mc);
             store_out_u32(out_meta + g, m, mc);
-        }
-        if (++stage == STAGES) {
-            stage = 0;
-            parity ^= 1;
         }
     }
 }

@@ -4,9 +4,7 @@
 // One thread owns one group (the n candidate cells of one field of one record) in registers.
 // HBM-bound streaming op: 4n bytes in, 8 bytes out per group, O(1) integer ops per byte, no reuse,
 // no tensor cores.  Two front-ends feed the same register core:
-//   * vote_tma_kernel    — n in {8,16,32,64}: every WARP runs its own TMA pipeline: a ring of STAGES
-//                          shared-memory tiles of 32 groups, each filled by one cp.async.bulk.tensor.2d
-//                          (hardware swizzle) completing on the warp's own mbarrier; conflict-free LDS.128;
+//   * vote_tma_kernel    — n in {8,16,32,64}: every WARP runs its own TMA pipeline (WarpTiles, kc_common.cuh);
 //                          no block-wide barrier anywhere.
 //   * vote_direct_kernel — any n <= 64 (and n <= 4 where a thread's cells are one coalesced vector load).
 #pragma once
@@ -422,102 +420,36 @@ __global__ void __launch_bounds__(256) vote_i8_kernel(const int8_t *__restrict__
 
 // ---------------------------------------------------------------- TMA front-end
 
-template <int ROW_BYTES>
-struct Swizzle {  // TMA swizzle mode for a row of ROW_BYTES (rows wider than 128 B are split into 128 B box rows)
-    static constexpr uint32_t kMask = ROW_BYTES >= 128 ? 7u : (ROW_BYTES == 64 ? 3u : 1u);
-    __device__ static __forceinline__ uint32_t apply(uint32_t off) { return off ^ (((off >> 7) & kMask) << 4); }
-};
-
-// Persistent kernel, warp-private pipelines.  Global warp w owns warp-tiles w, w + W, ... (W = warps in the
-// grid); a warp-tile is 32 consecutive groups, lane l owns row l.  Each warp keeps STAGES tiles in flight:
-// lane 0 arms the stage's mbarrier with the tile's byte count and issues one cp.async.bulk.tensor.2d; all
-// lanes wait on the barrier, pull their row with swizzled (bank-conflict-free) LDS.128, and lane 0 re-arms the
-// stage for the tile STAGES ahead before the warp computes.  Out-of-range rows of the last tile are
-// zero-filled by TMA and never stored.  There is no __syncthreads(): warps never wait for each other.
+// Persistent kernel on WarpTiles (kc_common.cuh): lane l votes row l of the warp's current tile.
 template <int N, int WARPS, int STAGES, bool HAS_NC>
 __global__ void __launch_bounds__(WARPS * 32) vote_tma_kernel(const __grid_constant__ CUtensorMap tmap, uint32_t n_groups,
                                                               FieldMap fm, int32_t *__restrict__ win,
                                                               uint32_t *__restrict__ meta, const __grid_constant__ OutRoute mc) {
-    constexpr int ROW_BYTES = N * 4;
-    constexpr int BOX_ROWS_PER_GROUP = ROW_BYTES > 128 ? ROW_BYTES / 128 : 1;
-    constexpr uint32_t TILE_BYTES = 32 * ROW_BYTES;
-    static_assert(TILE_BYTES % 1024 == 0, "warp tile must keep the swizzle atom alignment");
-    static_assert((STAGES & (STAGES - 1)) == 0, "STAGES must be a power of two");
-    extern __shared__ __align__(1024) uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[WARPS * STAGES];
-
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warp = __shfl_sync(0xFFFFFFFFu, threadIdx.x >> 5, 0);  // warp-uniform by construction
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    const uint32_t my_smem = smem_base + warp * (STAGES * TILE_BYTES);
-    const uint32_t my_bar = smem_u32(full_bar) + warp * (STAGES * 8);
-
-    // all indices are 32-bit: the launcher cuts the input into slabs of < 2^28 groups
-    const uint32_t n_tiles = (n_groups + 31u) >> 5;
-    const uint32_t first = blockIdx.x * WARPS + warp;
-    const uint32_t step = gridDim.x * WARPS;
-    uint64_t policy = 0;
-
-    if (lane == 0) {
-        tma_prefetch_desc(&tmap);
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) mbar_init_a(my_bar + s * 8, 1);
-        fence_barrier_init();
-        policy = policy_evict_first();
-#pragma unroll
-        for (int s = 0; s < STAGES; ++s) {
-            const uint32_t t = first + (uint32_t)s * step;
-            if (t < n_tiles) {
-                mbar_arrive_expect_tx_a(my_bar + s * 8, TILE_BYTES);
-                tma_load_2d_a(my_smem + s * TILE_BYTES, &tmap, 0, (int32_t)(t * 32 * BOX_ROWS_PER_GROUP), my_bar + s * 8, policy, 0);
-            }
-        }
-    }
-    __syncwarp();
+    WarpTiles<N * 4, WARPS, STAGES> tiles(&tmap, n_groups);
+    tiles.start(L2Policy::evict_first);
 
     uint32_t f0 = 0, fstep = 0;  // field of the tile's first group, advanced without division
     if constexpr (HAS_NC) {
-        f0 = (uint32_t)(((uint64_t)first * 32) % fm.n_fields);
-        fstep = (uint32_t)(((uint64_t)step * 32) % fm.n_fields);
+        f0 = (uint32_t)(((uint64_t)tiles.t * 32) % fm.n_fields);
+        fstep = (uint32_t)(((uint64_t)tiles.step * 32) % fm.n_fields);
     }
-    // this lane's four (or N/4) 16-byte pieces inside a tile: constant across tiles
-    uint32_t piece[N / 4];
-#pragma unroll
-    for (int q = 0; q < N / 4; ++q) piece[q] = Swizzle<ROW_BYTES>::apply(lane * ROW_BYTES + q * 16);
-
-    uint32_t it = 0;
-    for (uint32_t t = first; t < n_tiles; t += step, ++it) {
-        const uint32_t stage = it & (STAGES - 1);
-        const uint32_t parity = (it / STAGES) & 1;
-        const uint32_t bar = my_bar + stage * 8;
-        const uint32_t tile = my_smem + stage * TILE_BYTES;
-        mbar_wait_a(bar, parity);
+    for (; tiles.t < tiles.n_tiles; tiles.next()) {
+        const uint32_t tile = tiles.wait();
         int32_t raw[N];
 #pragma unroll
         for (int q = 0; q < N / 4; ++q) {
-            const int4 v4 = lds_v4(tile + piece[q]);
+            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
             raw[4 * q + 0] = v4.x;
             raw[4 * q + 1] = v4.y;
             raw[4 * q + 2] = v4.z;
             raw[4 * q + 3] = v4.w;
         }
-        // Every row must be in registers before the stage is handed back to the TMA unit.  `lo` depends on all
-        // loaded words, a warp instruction issues only when its operands are ready in every lane, and the
-        // re-arm below consumes `lo`, so it is ordered after the warp's LDS have returned.
         const int32_t lo = row_min<N>(raw);
-        // `order` is 0 on lane 0 but only the hardware knows it (a shuffle result): folding it into the TMA
-        // coordinate gives the copy a true register dependency on the loaded data, which neither nvvm nor ptxas
-        // can schedule away.
-        const uint32_t order = __shfl_sync(0xFFFFFFFFu, (uint32_t)lo, 0) ^ (uint32_t)lo;
-        const uint32_t tn = t + STAGES * step;
-        if (lane == 0 && tn < n_tiles) {
-            mbar_arrive_expect_tx_a(bar, TILE_BYTES);
-            tma_load_2d_a(tile, &tmap, 0, (int32_t)(tn * 32 * BOX_ROWS_PER_GROUP + order), bar, policy, 0);
-        }
-        const uint32_t g = t * 32 + lane;
+        tiles.release((uint32_t)lo);
+        const uint32_t g = tiles.t * 32 + tiles.lane;
         int32_t nc = KC_CODE_NONE;
         if constexpr (HAS_NC) {
-            nc = __ldg(fm.none_code + fm.mod_small(f0 + lane));
+            nc = __ldg(fm.none_code + fm.mod_small(f0 + tiles.lane));
             f0 += fstep;
             f0 = f0 >= fm.n_fields ? f0 - fm.n_fields : f0;
         }

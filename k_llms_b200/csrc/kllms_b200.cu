@@ -254,18 +254,18 @@ int launch_numeric_tma(const double *vals, int64_t G, double rel_eps, double abs
     auto kernel = kc::numeric_tma_kernel<N, WARPS, STAGES, MIN_CTAS>;
     const size_t smem = (size_t)WARPS * STAGES * 32 * N * 8 + (size_t)WARPS * 32 * N * 8 + 1024;
     return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
-        kernel<<<grid, WARPS * 32, smem, st>>>(map, gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
+        kernel<<<grid, WARPS * 32, smem, st>>>(map, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
     });
 }
 
 // fast path in front (kc::numeric_fast), general path for the groups it leaves open
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
 int launch_numeric_tma_fast(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
-                            cudaStream_t st, kc::OutRoute mc) {
+                            cudaStream_t st) {
     auto kernel = kc::numeric_tma_fast_kernel<N, WARPS, STAGES, MIN_CTAS>;
     const size_t smem = (size_t)WARPS * STAGES * 32 * N * 8 + (size_t)WARPS * 32 * N * 8 + 1024;
     return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
-        kernel<<<grid, WARPS * 32, smem, st>>>(map, vals + g0 * N, gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
+        kernel<<<grid, WARPS * 32, smem, st>>>(map, vals + g0 * N, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0);
     });
 }
 
@@ -320,10 +320,11 @@ int launch_numeric_direct_fast(const double *vals, int64_t G, double rel_eps, do
     return KC_OK;
 }
 
-// Never launched (n = 4 and 8 take other K2 kernels).  Without these two instantiations, 13 other K2 kernels, which share
-// __noinline__ helpers with them, compile to different SASS; they stay so that the K2 kernels are the ones that were timed.
-[[maybe_unused]] void *const kPinNumericSass[] = {(void *)kc::numeric_tma_kernel<4, 8, 2, 3>, (void *)kc::numeric_tma_kernel<8, 8, 2, 3>};
 
+// Never launched (n = 4 and 8 take other K2 kernels).  The K2 kernels share __noinline__ helpers with these two
+// instantiations, and without them compile to different SASS: numeric_tma_fast_kernel<16, 4, 1, 6> spills 12 bytes and
+// numeric_tma_kernel<32, 4, 1, 4> needs 127 registers instead of 113 (DESIGN §6).
+[[maybe_unused]] void *const kPinNumericSass[] = {(void *)kc::numeric_tma_kernel<4, 8, 2, 3>, (void *)kc::numeric_tma_kernel<8, 8, 2, 3>};
 }  // namespace
 
 // ---------------------------------------------------------------- host-buffer context
@@ -603,8 +604,8 @@ static int numeric_f64_routed(const double *d_vals, int64_t n_groups, int32_t n,
             case 2: return launch_numeric_units<2, 4>(kc::numeric_pairs_kernel, d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
             case 4: return launch_numeric_units<4, 2>(kc::numeric_quads_kernel, d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
             case 8: return launch_numeric_direct_fast<8>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 16: return launch_numeric_tma_fast<16, 4, 1, 6>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 32: return launch_numeric_tma_fast<32, 4, 1, 4>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 16: return launch_numeric_tma_fast<16, 4, 1, 6>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st);
+            case 32: return launch_numeric_tma_fast<32, 4, 1, 4>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st);
             default: break;
         }
     }
