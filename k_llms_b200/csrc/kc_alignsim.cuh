@@ -22,7 +22,7 @@
 // source on the host, which is what the CPU tests check.
 #pragma once
 
-#include "kc_internal.h"
+#include "kc_internal.h"  // py_isclose, kSimFloor
 #include "kc_medoid.cuh"  // alnum_index, myers_table, myers, kAlphabet, kPeqStride
 
 namespace kc {
@@ -30,7 +30,6 @@ namespace kc {
 constexpr int kAlignSimMaxT = 512;        // the host's dense memo limit (ListAligner)
 constexpr int kAlignSimMaxPattern = 64;   // the shorter normalised string of a pair must fit one 64-bit word
 constexpr int kAlignSimEmbedLen = 50;     // both raw strings longer than this: embeddings pair (cu:813)
-constexpr double kAlignSimFloor = 1e-8;   // SIMILARITY_SCORE_LOWER_BOUND, cu:78
 
 __host__ __device__ __forceinline__ double alignsim_nan() {
     const uint64_t bits = 0x7FF8000000000000ull;
@@ -39,17 +38,10 @@ __host__ __device__ __forceinline__ double alignsim_nan() {
     return d;
 }
 
-__host__ __device__ __forceinline__ bool alignsim_isclose(double a, double b) {  // math.isclose(a, b, rel_tol=0.01)
-    if (a == b) return true;
-    if (fabs(a) == INFINITY || fabs(b) == INFINITY) return false;
-    const double diff = fabs(b - a);
-    return diff <= fabs(0.01 * b) || diff <= fabs(0.01 * a);
-}
-
 // generic_similarity of two scalars (or None); tab: the lane's match table (kPeqStride u64)
 __host__ __device__ inline double alignsim_value(const KcAsVal &x, const KcAsVal &y, const uint8_t *__restrict__ chars, uint64_t *tab) {
     if ((x.flags & y.flags & KC_AS_FALSY) != 0) return 1.0;
-    if (x.type == KC_AS_NONE || y.type == KC_AS_NONE) return kAlignSimFloor;
+    if (x.type == KC_AS_NONE || y.type == KC_AS_NONE) return kSimFloor;
     if (x.type == KC_AS_STR && y.type == KC_AS_STR) {  // string_similarity, cu:797-824
         if (x.raw_len > kAlignSimEmbedLen && y.raw_len > kAlignSimEmbedLen) return alignsim_nan();
         if (x.raw_id == y.raw_id) return 1.0;
@@ -65,17 +57,17 @@ __host__ __device__ inline double alignsim_value(const KcAsVal &x, const KcAsVal
             d = p.len <= 32 ? myers<uint32_t>(tab, p.len, chars + t.off, t.len) : myers<uint64_t>(tab, p.len, chars + t.off, t.len);
         }
         const double sim = 1.0 - (double)d / (double)t.len;
-        return sim > kAlignSimFloor ? sim : kAlignSimFloor;
+        return sim > kSimFloor ? sim : kSimFloor;
     }
     const bool xn = x.type == KC_AS_BOOL || x.type == KC_AS_INT || x.type == KC_AS_FLOAT;
     const bool yn = y.type == KC_AS_BOOL || y.type == KC_AS_INT || y.type == KC_AS_FLOAT;
     if (xn && yn) {  // numerical_similarity, cu:827-841
-        if (x.type == KC_AS_BOOL && y.type == KC_AS_BOOL) return x.num == y.num ? 1.0 : kAlignSimFloor;
-        if (alignsim_isclose(x.num, y.num)) return 1.0;
+        if (x.type == KC_AS_BOOL && y.type == KC_AS_BOOL) return x.num == y.num ? 1.0 : kSimFloor;
+        if (py_isclose(x.num, y.num)) return 1.0;
         // int vs int compares the decimal texts: equal canonical keys (texts that fit int64) are equal texts
         const bool eq = (x.type == KC_AS_INT && y.type == KC_AS_INT) ? (x.ikey == y.ikey && ((x.flags | y.flags) & KC_AS_BIGINT) == 0)
                                                                     : x.num == y.num;
-        return eq ? 1.0 : kAlignSimFloor;
+        return eq ? 1.0 : kSimFloor;
     }
     return alignsim_nan();  // lists, nested dicts, mixed shapes: the host's
 }

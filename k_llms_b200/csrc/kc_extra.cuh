@@ -1,53 +1,11 @@
-// kc_extra.cuh — confidences (exact Python round(x, 5)) and K3, the per-candidate logprob sum.
+// kc_extra.cuh — confidences (kc::confidence, kc_internal.h) and K3, the per-candidate logprob sum.
 #pragma once
 
 #include "kc_common.cuh"
+#include "kc_internal.h"
 #include "kc_vote.cuh"
 
 namespace kc {
-
-// CPython float.__round__(x, 5) for finite x >= 0 (Objects/floatobject.c double_round: dtoa mode 3, i.e. the
-// EXACT binary value rounded half-even to 5 decimals, then strtod).  x = M * 2^-sh exactly; q = x*1e5 rounded
-// half-even in 128-bit integer arithmetic; q / 1e5 in IEEE double is the double nearest to the decimal
-// q*10^-5, which is what strtod returns.  Used by cu:982,1178,1187,1219.
-__device__ __forceinline__ double py_round5(double x) {
-    const uint64_t bits = (uint64_t)__double_as_longlong(x);
-    const int biased = (int)((bits >> 52) & 0x7FF);
-    uint64_t mant = bits & 0xFFFFFFFFFFFFFull;
-    int exp2;  // x = mant * 2^exp2
-    if (biased == 0) {
-        exp2 = -1074;
-    } else {
-        mant |= 1ull << 52;
-        exp2 = biased - 1075;
-    }
-    if (mant == 0) return x;
-    if (exp2 >= 0) return x;  // integer-valued: nothing to round
-    const int sh = -exp2;     // >= 1
-    if (sh >= 128) return 0.0;
-    const uint64_t lo = mant * 100000ull;  // low 64 bits of the 70-bit product
-    const uint64_t hi = __umul64hi(mant, 100000ull);
-    uint64_t q, rem_hi, rem_lo, half_hi, half_lo;
-    if (sh >= 64) {
-        const int s = sh - 64;  // 0..63
-        q = s == 0 ? hi : (hi >> s);
-        rem_hi = s == 0 ? 0 : (hi & ((1ull << s) - 1));
-        rem_lo = lo;
-        half_hi = s == 0 ? 0 : (1ull << (s - 1));
-        half_lo = s == 0 ? (1ull << 63) : 0;
-    } else {
-        q = (hi << (64 - sh)) | (lo >> sh);  // sh in 1..63; hi < 2^6 so no bits are lost for sh >= 6,
-                                             // and for sh < 6 the product fits 64 bits only if hi == 0 (x >= 2^46: not a confidence)
-        rem_hi = 0;
-        rem_lo = lo & ((1ull << sh) - 1);
-        half_hi = 0;
-        half_lo = 1ull << (sh - 1);
-    }
-    const bool gt = rem_hi > half_hi || (rem_hi == half_hi && rem_lo > half_lo);
-    const bool eq = rem_hi == half_hi && rem_lo == half_lo;
-    if (gt || (eq && (q & 1))) ++q;
-    return __ddiv_rn((double)q, 100000.0);
-}
 
 // One thread per group: the confidence the reference attaches to the group's consensus value.
 __global__ void __launch_bounds__(256) confidence_kernel(const uint32_t *__restrict__ meta, int64_t n_groups, bool numeric,
@@ -56,22 +14,7 @@ __global__ void __launch_bounds__(256) confidence_kernel(const uint32_t *__restr
     for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += stride) {
         const uint32_t m = __ldg(meta + g);
         const double pvf = pvf_in ? __ldg(pvf_in + g) : 1.0;
-        const double support = (double)KC_META_SUPPORT(m), nn = (double)KC_META_NN(m), present = (double)KC_META_PRESENT(m);
-        const uint32_t flags = KC_META_FLAGS(m);
-        double c;
-        if (flags & KC_FLAG_HAS_VALUE) {
-            if (!numeric)
-                c = py_round5(__dmul_rn(pvf, __ddiv_rn(support, present)));  // cu:973,982
-            else if (flags & KC_FLAG_SINGLE)
-                c = __dmul_rn(__dmul_rn(pvf, __ddiv_rn(1.0, present)), 1.0);  // cu:1444,1086 (unrounded)
-            else
-                c = py_round5(__ddiv_rn(support, nn));  // cu:1177-1178,1186-1187,1218-1219
-        } else if (flags & KC_FLAG_NO_FINITE) {
-            c = __dmul_rn(pvf, __ddiv_rn(nn, present));  // cu:1444,1116
-        } else {
-            c = present == 0.0 ? pvf : 0.0;  // cu:1396 / cu:1402
-        }
-        conf[g] = c;
+        conf[g] = confidence(m, numeric, pvf);
     }
 }
 

@@ -1,8 +1,114 @@
 // kc_internal.h — helpers shared by the translation units of libkllms_b200.so (not part of the C ABI).
+//
+// It also holds the one copy of each small CPython rule that the kernels and the host code must apply bit for bit
+// (kc_json.cpp is host C++ and cannot include the .cuh headers, so these live here, __host__ __device__):
+//     py_round5            round(x, 5)                                 (consensus_utils.py:982,1178,1187,1219)
+//     confidence           the confidence of a vote / numeric result word (cu:971-982,1085-1086,1116,1177-1219,1396,1402)
+//     medoid_confidence    the confidence of a similarity medoid        (cu:1085-1086,1233-1237)
+//     py_isclose           math.isclose(a, b, rel_tol=0.01)             (cu:827-841)
+//     kSimFloor            SIMILARITY_SCORE_LOWER_BOUND                 (cu:78)
+// float.__repr__ is kc::js::float_repr (kc_jsoncore.cuh); the edit distance is kc_levenshtein (kc_json.cpp) on the host
+// and K4's Myers loop (kc_medoid.cuh) on the device.
 #pragma once
 #include <cuda_runtime.h>
+#include <math.h>
 #include <stddef.h>
 #include <stdint.h>
+#include <string.h>
+
+#include "../../include/kllms_b200.h"
+
+#ifdef __CUDACC__
+#define KC_HD __host__ __device__
+#else
+#define KC_HD
+#endif
+
+namespace kc {
+
+KC_HD inline uint64_t umul64hi(uint64_t a, uint64_t b) {  // the high 64 bits of a * b
+#ifdef __CUDA_ARCH__
+    return __umul64hi(a, b);
+#else
+    return (uint64_t)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+
+// CPython float.__round__(x, 5) (Objects/floatobject.c double_round: dtoa mode 3, i.e. the EXACT binary value rounded
+// half-even to 5 decimals, then strtod).  x = mant * 2^-sh exactly; q = x * 1e5 rounded half-even in integer arithmetic on
+// two 64-bit halves; q / 1e5 in IEEE double is the double nearest to the decimal q * 10^-5, which is what strtod returns.
+// Domain: finite x >= 0 and below 2^46 (every confidence is in [0, 1]).  Zero, NaN and infinities come back unchanged.
+KC_HD inline double py_round5(double x) {
+    uint64_t bits;
+    memcpy(&bits, &x, 8);
+    const int biased = (int)((bits >> 52) & 0x7FF);
+    uint64_t mant = bits & 0xFFFFFFFFFFFFFull;
+    int exp2;  // x = mant * 2^exp2
+    if (biased == 0) {
+        exp2 = -1074;
+    } else {
+        mant |= 1ull << 52;
+        exp2 = biased - 1075;
+    }
+    if (mant == 0) return x;
+    if (exp2 >= 0) return x;  // integer-valued: nothing to round
+    const int sh = -exp2;     // >= 1
+    if (sh >= 128) return 0.0;
+    const uint64_t lo = mant * 100000ull;  // low 64 bits of the 70-bit product
+    const uint64_t hi = umul64hi(mant, 100000ull);
+    uint64_t q, rem_hi, rem_lo, half_hi, half_lo;
+    if (sh >= 64) {
+        const int s = sh - 64;  // 0..63
+        q = s == 0 ? hi : (hi >> s);
+        rem_hi = s == 0 ? 0 : (hi & ((1ull << s) - 1));
+        rem_lo = lo;
+        half_hi = s == 0 ? 0 : (1ull << (s - 1));
+        half_lo = s == 0 ? (1ull << 63) : 0;
+    } else {
+        q = (hi << (64 - sh)) | (lo >> sh);  // sh in 1..63; hi < 2^6 so no bits are lost for sh >= 6,
+                                             // and for sh < 6 the product fits 64 bits only if hi == 0 (x >= 2^46: outside the domain)
+        rem_hi = 0;
+        rem_lo = lo & ((1ull << sh) - 1);
+        half_hi = 0;
+        half_lo = 1ull << (sh - 1);
+    }
+    const bool gt = rem_hi > half_hi || (rem_hi == half_hi && rem_lo > half_lo);
+    const bool eq = rem_hi == half_hi && rem_lo == half_lo;
+    if (gt || (eq && (q & 1))) ++q;
+    return (double)q / 100000.0;
+}
+
+// The confidence the reference attaches to the consensus value of a vote (numeric == false) or numeric group, from its
+// result word (KC_META_*) and the parent's valid fraction pvf.  Every operation is one IEEE operation in this order.
+KC_HD inline double confidence(uint32_t m, bool numeric, double pvf) {
+    const double support = (double)KC_META_SUPPORT(m), nn = (double)KC_META_NN(m), present = (double)KC_META_PRESENT(m);
+    const uint32_t flags = KC_META_FLAGS(m);
+    if (flags & KC_FLAG_HAS_VALUE) {
+        if (!numeric) return py_round5(pvf * (support / present));  // cu:973,982
+        if (flags & KC_FLAG_SINGLE) return pvf * (1.0 / present) * 1.0;  // cu:1444,1086 (unrounded)
+        return py_round5(support / nn);  // cu:1177-1178,1186-1187,1218-1219
+    }
+    if (flags & KC_FLAG_NO_FINITE) return pvf * (nn / present);  // cu:1444,1116
+    return present == 0.0 ? pvf : 0.0;  // cu:1396 / cu:1402
+}
+
+// The confidence of a similarity medoid among the `live` non-None strings of n candidates, avg = the medoid's mean
+// similarity: cu:1444 then cu:1085-1086 (one string: itself, unrounded) or cu:1233-1237 (the medoid, rounded).
+KC_HD inline double medoid_confidence(uint32_t live, int32_t n, double avg) {
+    const double sub = 1.0 * ((double)live / (double)n);
+    return live >= 2 ? py_round5(sub * avg) : sub * (1.0 / 1.0);
+}
+
+constexpr double kSimFloor = 1e-8;  // SIMILARITY_SCORE_LOWER_BOUND, cu:78
+
+KC_HD inline bool py_isclose(double a, double b) {  // math.isclose(a, b, rel_tol=0.01), numerical_similarity cu:827-841
+    if (a == b) return true;
+    if (fabs(a) == INFINITY || fabs(b) == INFINITY) return false;
+    const double diff = fabs(b - a);
+    return diff <= fabs(0.01 * b) || diff <= fabs(0.01 * a);
+}
+
+}  // namespace kc
 
 // records the thread-local text kc_last_error() returns and hands `code` back
 __attribute__((visibility("hidden"))) int kc_fail(int code, const char *fmt, ...) __attribute__((format(printf, 2, 3)));

@@ -21,7 +21,7 @@
 #include <atomic>
 #include <chrono>
 #include <cstdio>
-#include <charconv>
+#include <charconv>  // from_chars (kc_align.inl)
 #include <cmath>
 #include <cstdint>
 #include <cstdlib>
@@ -36,7 +36,7 @@
 
 #include "../../include/kllms_b200.h"
 #include "kc_internal.h"    // kc_alignsim: element similarities of the alignment pre-pass (kc_alignsim.cuh)
-#include "kc_jsoncore.cuh"  // to_double: exact decimal -> float64 without strtod (host-callable)
+#include "kc_jsoncore.cuh"  // to_double, float_repr: the device path's exact number conversions (host-callable)
 
 namespace {
 
@@ -311,54 +311,12 @@ bool parse_object(const char *s, size_t len, std::vector<Item> &out, bool &not_o
 
 // ---------------------------------------------------------------- CPython text formats
 
-// float.__repr__: shortest round-trip digits; fixed notation for -4 <= exponent10 < 16, else d[.ddd]e+XX.
-void py_float_repr(double x, std::string &out) {
-    if (std::isnan(x)) { out += "nan"; return; }
-    if (std::isinf(x)) { out += x < 0 ? "-inf" : "inf"; return; }
-    char buf[40];
-    auto r = std::to_chars(buf, buf + sizeof buf, x, std::chars_format::scientific);  // shortest digits: d[.ddd]e+XX
-    std::string_view sv(buf, (size_t)(r.ptr - buf));
-    size_t i = 0;
-    if (sv[i] == '-') { out.push_back('-'); ++i; }
-    const size_t epos = sv.find('e');
-    std::string digits;
-    for (size_t k = i; k < epos; ++k)
-        if (sv[k] != '.') digits.push_back(sv[k]);
-    const int exp10 = atoi(std::string(sv.substr(epos + 1)).c_str());
-    const int decpt = exp10 + 1;  // position of the decimal point relative to the digit string
-    const int nd = (int)digits.size();
-    if (decpt > 16 || decpt < -3) {
-        out.push_back(digits[0]);
-        if (nd > 1) {
-            out.push_back('.');
-            out.append(digits, 1, std::string::npos);
-        }
-        out.push_back('e');
-        const int e = decpt - 1;
-        out.push_back(e < 0 ? '-' : '+');
-        const int ae = e < 0 ? -e : e;
-        if (ae < 10) out.push_back('0');
-        out += std::to_string(ae);
-    } else if (decpt <= 0) {
-        out += "0.";
-        out.append((size_t)(-decpt), '0');
-        out += digits;
-    } else if (decpt >= nd) {
-        out += digits;
-        out.append((size_t)(decpt - nd), '0');
-        out += ".0";
-    } else {
-        out.append(digits, 0, (size_t)decpt);
-        out.push_back('.');
-        out.append(digits, (size_t)decpt, std::string::npos);
-    }
-}
-
-// json.dumps float: repr, but NaN / Infinity / -Infinity spelled the JSON way
-void json_float(double x, std::string &out) {
-    if (std::isnan(x)) out += "NaN";
-    else if (std::isinf(x)) out += x < 0 ? "-Infinity" : "Infinity";
-    else py_float_repr(x, out);
+// json.dumps(x) for a float: float.__repr__, NaN / Infinity / -Infinity spelled the JSON way (kc::js::float_repr)
+void put_float(double x, std::string &out) {
+    uint8_t buf[32];  // the longest repr is 24 characters
+    kc::js::Sink o{buf, 0};
+    kc::js::float_repr(x, o);
+    out.append((const char *)buf, (size_t)o.n);
 }
 
 // json.dumps(str) with ensure_ascii=True (input is ASCII)
@@ -399,7 +357,11 @@ void py_str(const Tok &t, std::string &out) {
         case T_TRUE: out += "True"; break;
         case T_FALSE: out += "False"; break;
         case T_INT: int_text(t, out); break;
-        case T_FLOAT: py_float_repr(t.num, out); break;
+        case T_FLOAT:  // str(float): repr, but non-finite values spelled nan / inf / -inf
+            if (std::isnan(t.num)) out += "nan";
+            else if (std::isinf(t.num)) out += t.num < 0 ? "-inf" : "inf";
+            else put_float(t.num, out);
+            break;
         case T_STR: {
             if (t.esc) {
                 std::string tmp;
@@ -442,7 +404,7 @@ void json_value(const Tok &t, std::string &out) {
         case T_TRUE: out += "true"; break;
         case T_FALSE: out += "false"; break;
         case T_INT: int_text(t, out); break;
-        case T_FLOAT: json_float(t.num, out); break;
+        case T_FLOAT: put_float(t.num, out); break;
         case T_STR: {
             std::string tmp;
             tok_string(t, tmp);
@@ -740,27 +702,6 @@ void encode_numeric(const Tok *toks, int n, double *cells) {
     }
 }
 
-// CPython round(x, 5) on the host (same algorithm as kc::py_round5): exact value * 1e5, half-even, one division
-double py_round5(double x) {
-    if (!(x > 0.0) || !std::isfinite(x)) return x;
-    uint64_t bits;
-    memcpy(&bits, &x, 8);
-    const int biased = (int)((bits >> 52) & 0x7FF);
-    uint64_t mant = bits & 0xFFFFFFFFFFFFFull;
-    int exp2;
-    if (biased == 0) exp2 = -1074;
-    else { mant |= 1ull << 52; exp2 = biased - 1075; }
-    if (exp2 >= 0) return x;
-    const int sh = -exp2;
-    if (sh >= 128) return 0.0;
-    const unsigned __int128 prod = (unsigned __int128)mant * 100000u;
-    unsigned __int128 q = prod >> sh;
-    const unsigned __int128 rem = prod - (q << sh);
-    const unsigned __int128 half = (unsigned __int128)1 << (sh - 1);
-    if (rem > half || (rem == half && (q & 1))) ++q;
-    return (double)(uint64_t)q / 100000.0;
-}
-
 struct EmitCtx {
     const Record &rec;
     int n;
@@ -784,34 +725,27 @@ void emit_leaf(const EmitCtx &cx, size_t gi, std::string &content, std::string &
         Tok value;  // T_MISSING == None
         if (g.kind == G_VOTE_STR || g.kind == G_VOTE_BOOL) {
             const uint32_t m = vmeta[g.row];
-            const uint32_t idx = KC_META_IDX(m), support = KC_META_SUPPORT(m), present = KC_META_PRESENT(m);
+            const uint32_t idx = KC_META_IDX(m);
             if (g.kind == G_VOTE_BOOL) {
                 value.type = (cells[idx].type == T_TRUE) ? T_TRUE : T_FALSE;  // the processed key (cu:958)
             } else {
                 value = cells[idx];  // first original whose sanitised form wins (cu:971)
             }
-            conf = py_round5(1.0 * ((double)support / (double)present));
+            // always the HAS_VALUE arm: a string group has a non-None cell, and a bool group turns None into False
+            conf = kc::confidence(m, false, 1.0);
         } else if (g.kind == G_NUMERIC) {
             const uint32_t m = nmeta[g.row];
-            const uint32_t idx = KC_META_IDX(m), support = KC_META_SUPPORT(m), nn = KC_META_NN(m), present = KC_META_PRESENT(m);
             const uint32_t flags = KC_META_FLAGS(m);
             if (flags & KC_FLAG_HAS_VALUE) {
                 if (flags & KC_FLAG_SINGLE) {
-                    value = cells[idx];
-                    conf = 1.0 * (1.0 / (double)present) * (1.0 / 1.0);
+                    value = cells[KC_META_IDX(m)];
                 } else {
                     value.type = T_FLOAT;
                     value.num = nvalue[g.row];
-                    conf = py_round5((double)support / (double)nn);
                 }
-            } else if (flags & KC_FLAG_NO_FINITE) {
-                conf = 1.0 * ((double)nn / (double)present);
-            } else {
-                conf = present == 0 ? 1.0 : 0.0;
             }
+            conf = kc::confidence(m, true, 1.0);
         } else if (g.kind == G_MEDOID) {
-            // cu:1444 then cu:1085-1086 (one non-None cell, unrounded) or cu:1233-1237 (the medoid, rounded)
-            const double sub = 1.0 * ((double)g.m_count / (double)n);
             int want = g.m_count >= 2 ? midx[g.row] : 0;
             for (int c = 0; c < n; ++c) {
                 if (cells[c].type <= T_NULL) continue;
@@ -820,10 +754,10 @@ void emit_leaf(const EmitCtx &cx, size_t gi, std::string &content, std::string &
                     break;
                 }
             }
-            conf = g.m_count >= 2 ? py_round5(sub * mavg[g.row]) : sub * (1.0 / 1.0);
+            conf = kc::medoid_confidence(g.m_count, n, g.m_count >= 2 ? mavg[g.row] : 0.0);
         }  // G_ALLNULL: None, 0.0 (cu:1401-1402)
         json_value(value, content);
-        json_float(conf, lik);
+        put_float(conf, lik);
 }
 
 void emit_node(const EmitCtx &cx, int32_t ni, std::string &content, std::string &lik) {

@@ -1,5 +1,5 @@
 // kc_jsoncore.cuh — the per-thread building blocks of the device JSON path (H1g): a validating scanner for flat JSON objects,
-// exact decimal -> float64 and float64 -> float.__repr__ conversions, sanitised string comparison, CPython round(x, 5).
+// exact decimal -> float64 and float64 -> float.__repr__ conversions, sanitised string comparison.
 //
 // Everything here is __host__ __device__ and free of warp intrinsics: the kernels in kc_jsongpu.cuh call these functions
 // per lane, and the CPU tests instantiate THE SAME code on the host (kc_debug_jsongpu_* in kllms_b200.cu) to check the logic
@@ -7,21 +7,15 @@
 //     scan_object      json.loads of one candidate content (consolidation.py:25-38) for objects of scalar values
 //     to_double        float(text) / float(int(text)) as json.loads + consensus_utils.py:1105-1114 produce them (correctly rounded)
 //     sanitized_equal  sanitize_value(a) == sanitize_value(b)  (consensus_utils.py:925-933, ASCII)
-//     py_round5        round(x, 5) (consensus_utils.py:982,1178,1187,1219)
 //     float_repr       json.dumps of a float = float.__repr__ (shortest round-trip digits, Ryu), _format_consensus_content
-//                      (consolidation.py:41-60)
+//                      (consolidation.py:41-60); the host path H1 (kc_json.cpp) prints its floats through it as well
 #pragma once
 
 #include <stdint.h>
 #include <string.h>
 
+#include "kc_internal.h"  // KC_HD
 #include "kc_ryu_tables.cuh"
-
-#ifdef __CUDACC__
-#define KC_HD __host__ __device__
-#else
-#define KC_HD
-#endif
 
 namespace kc {
 namespace js {
@@ -430,32 +424,6 @@ KC_HD inline bool to_double(const uint8_t *s, uint32_t len, double &out) {
     }
     out = neg ? -r : r;
     return true;
-}
-
-// ---------------------------------------------------------------- CPython round(x, 5)
-
-// exact value * 10^5 in integer arithmetic, half-even, one IEEE division (same algorithm as kc::py_round5 / kc_json.cpp)
-KC_HD inline double py_round5(double x) {
-    const uint64_t bits = f64_bits(x);
-    if ((bits >> 63) || x == 0.0 || ((bits >> 52) & 0x7FF) == 0x7FF) return x;  // confidences are finite and >= 0
-    const int biased = (int)((bits >> 52) & 0x7FF);
-    uint64_t mant = bits & 0xFFFFFFFFFFFFFull;
-    int exp2;
-    if (biased == 0) {
-        exp2 = -1074;
-    } else {
-        mant |= 1ull << 52;
-        exp2 = biased - 1075;
-    }
-    if (exp2 >= 0) return x;
-    const int sh = -exp2;
-    if (sh >= 128) return 0.0;
-    const u128 prod = (u128)mant * 100000u;
-    u128 q = prod >> sh;
-    const u128 rem = prod - (q << sh);
-    const u128 half = ((u128)1) << (sh - 1);
-    if (rem > half || (rem == half && (q & 1))) ++q;
-    return (double)(uint64_t)q / 100000.0;
 }
 
 // ---------------------------------------------------------------- output sink

@@ -792,7 +792,7 @@ int kc_debug_float_reprs(const double *xs, int64_t count, char *out /* [count][3
 
 int kc_debug_round5(const double *xs, int64_t count, double *out) {
     if (!xs || !out) return KC_EINVAL;
-    for (int64_t i = 0; i < count; ++i) out[i] = kc::js::py_round5(xs[i]);
+    for (int64_t i = 0; i < count; ++i) out[i] = kc::py_round5(xs[i]);
     return KC_OK;
 }
 

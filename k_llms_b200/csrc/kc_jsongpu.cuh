@@ -401,25 +401,24 @@ KC_HD inline void encode_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t
 // ---------------------------------------------------------------- C0 / C1
 
 // value and confidence of one field, formatted into the two sinks (the epilogue emit_leaf of kc_json.cpp:
-// cu:971-982, cu:1085-1086, cu:1116, cu:1177-1219)
+// cu:971-982, cu:1085-1086, cu:1116, cu:1177-1219); the confidences are kc::confidence / kc::medoid_confidence
 KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &content, Sink &lik) {
     const int32_t n = ch.n;
     const Tok *row = ch.toks + ((int64_t)ch.slot[r] + j) * n;
     const uint32_t d = ch.fdesc[ch.slot[r] + j], kind = fdesc_kind(d), g = fdesc_gidx(d);
     double conf = 0.0;
+    uint32_t m = 0;  // vote / numeric: the result word
     if (kind == F_VOTE_STR || kind == F_VOTE_BOOL) {
-        const uint32_t m = ch.vmeta[(int64_t)ch.vbase[r] + g];
-        const uint32_t idx = KC_META_IDX(m), support = KC_META_SUPPORT(m), present = KC_META_PRESENT(m);
+        m = ch.vmeta[(int64_t)ch.vbase[r] + g];
+        const uint32_t idx = KC_META_IDX(m);
         if (kind == F_VOTE_BOOL) {
             content.lit(row[idx].kind == K_TRUE ? "true" : "false");  // the processed key (cu:958)
         } else {
             content.json_string(ch.text + row[idx].vstart, row[idx].vlen, row[idx].flags & TOK_ESCAPED);  // first original whose sanitised form wins (cu:971)
         }
-        conf = py_round5(1.0 * ((double)support / (double)present));
     } else if (kind == F_NUMERIC) {
-        const uint32_t m = ch.xmeta[(int64_t)ch.xbase[r] + g];
-        const uint32_t idx = KC_META_IDX(m), support = KC_META_SUPPORT(m), nn = KC_META_NN(m), present = KC_META_PRESENT(m);
-        const uint32_t flags = KC_META_FLAGS(m);
+        m = ch.xmeta[(int64_t)ch.xbase[r] + g];
+        const uint32_t idx = KC_META_IDX(m), flags = KC_META_FLAGS(m);
         if (flags & KC_FLAG_HAS_VALUE) {
             if (flags & KC_FLAG_SINGLE) {  // the original object, confidence unrounded (cu:1085-1086)
                 const Tok &t = row[idx];
@@ -435,29 +434,23 @@ KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &cont
                 } else {
                     content.lit(t.kind == K_TRUE ? "true" : (t.kind == K_FALSE ? "false" : "null"));
                 }
-                conf = 1.0 * (1.0 / (double)present) * (1.0 / 1.0);
             } else {
                 float_repr(ch.xvalue[(int64_t)ch.xbase[r] + g], content);
-                conf = py_round5((double)support / (double)nn);
             }
         } else {
             content.lit("null");
-            if (flags & KC_FLAG_NO_FINITE) conf = 1.0 * ((double)nn / (double)present);
-            else conf = present == 0 ? 1.0 : 0.0;
         }
     } else if (kind == F_MEDOID) {
-        // cu:1444 then cu:1085-1086 (one non-None string: itself, unrounded) or cu:1233-1237 (the medoid, rounded)
         uint32_t live = 0;
         for (int32_t c = 0; c < n; ++c) live += row[c].kind != K_NULL ? 1u : 0u;
-        const double sub = 1.0 * ((double)live / (double)n);
-        int32_t want = 0;
+        int32_t want = 0;  // one non-None string: itself
+        double avg = 0.0;
         if (live >= 2) {
             const uint32_t gi = ch.mcount[r] + g;
             want = ch.midx[gi];
-            conf = py_round5(sub * ch.mavg[gi]);
-        } else {
-            conf = sub * (1.0 / 1.0);
+            avg = ch.mavg[gi];
         }
+        conf = medoid_confidence(live, n, avg);
         for (int32_t c = 0; c < n; ++c) {
             if (row[c].kind == K_NULL) continue;
             if (want-- == 0) {
@@ -468,6 +461,9 @@ KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &cont
     } else {
         content.lit("null");  // all None: (None, 0.0) (cu:1401-1402)
     }
+    // one call for both kinds keeps one inlined copy (two made write_kernel save convergence barriers); a vote group always
+    // reaches the HAS_VALUE arm: a string group has a non-None cell, and a bool group turns None into False
+    if (kind == F_VOTE_STR || kind == F_VOTE_BOOL || kind == F_NUMERIC) conf = confidence(m, kind == F_NUMERIC, 1.0);
     float_repr(conf, lik);
 }
 

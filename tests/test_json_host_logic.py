@@ -24,6 +24,14 @@ def test_two_phase_native_json_matches_client_order_cpu():
             native += 1
             assert got == _expected(texts), texts
     assert native > 600
+    # string votes holding floats: the classes are sanitize_value(str(v)), so NaN / Infinity / -0.0 / 1e16 must be spelled
+    # as str(float) spells them ("nan", "inf", "-0.0", "1e+16"), not as json.dumps does
+    specials = [['{"s": "inf"}', '{"s": Infinity}', '{"s": -Infinity}', '{"s": NaN}'],
+                ['{"s": "nan"}', '{"s": NaN}', '{"s": "x"}', '{"s": Infinity}'],
+                ['{"s": "00"}', '{"s": -0.0}', '{"s": 1e16}', '{"s": -0.0}'],
+                ['{"s": "1e16"}', '{"s": 1e16}', '{"s": -0.0}', '{"s": 1e16}']]
+    for texts, got in zip(specials, consolidate_json_with_oracle(specials)):
+        assert got is not None and got == _expected(texts), texts
 
 
 def test_two_phase_native_json_list_records_cpu():

@@ -2,7 +2,8 @@
 __host__ __device__, and the kc_debug_jsongpu_* hooks run them on the host lane by lane with the C oracle in the place of
 K1 / K2.  Everything the path accepts must be byte-identical to the reference's client order (json.loads -> align ->
 consensus -> json.dumps, restated by the object-level oracle); everything else it must decline.  Also pins the exact
-decimal -> float64 conversion, the shortest-digits float.__repr__ and round(x, 5) of kc_jsoncore.cuh against CPython."""
+decimal -> float64 conversion and the shortest-digits float.__repr__ of kc_jsoncore.cuh, and round(x, 5) of kc_internal.h,
+against CPython."""
 import json
 import random
 
@@ -374,7 +375,14 @@ def test_exact_number_conversions_match_cpython():
     for i, x in enumerate(xs):
         assert bytes(buf[i, :lens[i]]).decode() == json.dumps(float(x)), repr(float(x))
 
-    cs = np.array([rng.random() for _ in range(50000)] + [k / n for n in range(1, 65) for k in range(n + 1)])
+    # and the products of tests/test_gpu_kernels.py::test_round5_random_products: pvf * support / present, near-half cases first
+    prng = np.random.default_rng(3)
+    present = prng.integers(1, 65, 200000)
+    support = np.minimum((prng.random(200000) * present).astype(np.int64) + 1, present)
+    pvf = prng.random(200000)
+    pvf[:1000] = np.round(pvf[:1000], 5) + 5e-6
+    cs = np.concatenate([[rng.random() for _ in range(50000)], [k / n for n in range(1, 65) for k in range(n + 1)],
+                         pvf * (support / present)])
     out = np.zeros(len(cs))
     K.check(lib.kc_debug_round5(cs.ctypes.data, len(cs), out.ctypes.data))
     assert all(round(float(x), 5) == o for x, o in zip(cs, out))
