@@ -127,6 +127,8 @@ template <int ROW_BYTES, int WARPS, int STAGES>
 struct WarpTiles {
     static constexpr uint32_t BOX_ROWS_PER_GROUP = ROW_BYTES > 128 ? ROW_BYTES / 128 : 1;
     static constexpr uint32_t TILE_BYTES = 32 * ROW_BYTES;
+    // dynamic shared memory up to end(): the WARPS rings and the slack for aligning them to 1024 bytes
+    static constexpr uint32_t RING_BYTES = 1024 + WARPS * STAGES * TILE_BYTES;
     static_assert(TILE_BYTES % 1024 == 0, "warp tile must keep the swizzle atom alignment");
     static_assert((STAGES & (STAGES - 1)) == 0, "STAGES must be a power of two");
 

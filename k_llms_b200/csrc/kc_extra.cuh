@@ -189,8 +189,33 @@ __global__ void __launch_bounds__(128) weighted_vote_kernel(const int32_t *__res
     }
 }
 
+// Candidate weights w_c = kexp(s_c - max_k s_k) of ONE record by a warp, lane = candidate: s_lo, s_hi = the sequence logprobs of
+// candidates lane and lane + 32 (-3.0e38f where there is none).  Writes w[lane] (and w[lane + 32] for N > 32); returns the
+// record's heaviest candidate, the first of the largest sums (N if there is none, e.g. all NaN).  The max is the fmaxf butterfly
+// 16..1, so every lane holds the same one.
+template <int N>
+__device__ __forceinline__ int record_weights(float s_lo, float s_hi, float *w, uint32_t lane) {
+    float smax = fmaxf(s_lo, s_hi);
+#pragma unroll
+    for (int st = 16; st >= 1; st >>= 1) smax = fmaxf(smax, __shfl_xor_sync(0xFFFFFFFFu, smax, st));
+    if (N >= 32 || lane < N) w[lane] = kexp(__fadd_rn(s_lo, -smax));
+    if (N > 32) w[lane + 32] = kexp(__fadd_rn(s_hi, -smax));
+    const uint32_t b_lo = __ballot_sync(0xFFFFFFFFu, s_lo == smax), b_hi = __ballot_sync(0xFFFFFFFFu, N > 32 && s_hi == smax);
+    return b_lo ? __ffs((int)b_lo) - 1 : (b_hi ? 31 + __ffs((int)b_hi) : N);
+}
+
+// Where every walk below stops.  Each class not summed yet sums a subset of the weights not consumed yet, so its fp32 sum is at
+// most (total - consumed) up to rounding (< 64 * 2^-23 relative on each side); kWvSlack * total covers that.  A class below
+// this bound can neither win nor tie.
+constexpr float kWvSlack = 5e-5f;
+__device__ __forceinline__ float wv_rest_bound(float total, float consumed) {
+    return __fadd_rn(__fadd_rn(total, -consumed), __fmul_rn(total, kWvSlack));
+}
+
 // The weighted vote of ONE group by one thread: rawrow = the group's cells (code >= 0, KC_CODE_NONE, absent < KC_CODE_NONE), nc = the
-// code None votes as (KC_CODE_NONE: it does not), w = the candidate weights of the group's record (shared memory).
+// code None votes as (KC_CODE_NONE: it does not), w = the candidate weights of the group's record.  The outcome: the heaviest
+// class (its cells' weights summed in ascending candidate order, fp32) wins, equal weights go to the class seen first (the
+// smaller first index), `tie` says whether another class equals the winner.
 template <int NP>
 __device__ __forceinline__ void weighted_core(const int32_t (&rawrow)[NP], int32_t nc, const float *w, int32_t &out_code,
                                               uint32_t &out_meta, float &out_weight) {
@@ -233,10 +258,7 @@ __device__ __forceinline__ void weighted_core(const int32_t (&rawrow)[NP], int32
     // over the cells finds the next class itself — no shared memory for the codes at all.)
     int32_t c = cmax;
     while (live) {
-        // Every class still waiting sums a subset of the unconsumed weights, so its fp32 sum is at most
-        // (total - consumed) up to rounding (< 32 * 2^-23 relative on each side); 5e-5 * total is a safe slack.
-        // Below best_w it can neither win nor tie: stop.
-        if (__fadd_rn(__fadd_rn(total, -consumed), __fmul_rn(total, 5e-5f)) < best_w) break;
+        if (wv_rest_bound(total, consumed) < best_w) break;
         M eq = 0;
         float cw = 0.0f, nw = -1.0f;
         int32_t nc2 = KC_CODE_NONE;
@@ -278,15 +300,13 @@ __device__ __forceinline__ void weighted_core(const int32_t (&rawrow)[NP], int32
 }
 
 // K3b, weights once per record: the candidate weights depend on the record only, not on the field.  A CTA of T threads
-// covers T consecutive groups (fields of a handful of records); its warps first compute w_c = kexp(s_c - max s) for
-// those records into shared memory (lane = candidate, warp max by shuffles), then every thread votes its group with the
-// weights read from there (same class sums, same order as weighted_vote_kernel).
+// covers T consecutive groups (fields of a handful of records); its warps first compute the weights of those records into
+// shared memory (record_weights), then every thread votes its group with the weights read from there.
 template <int NP, int T>
 __global__ void __launch_bounds__(T) weighted_vote_rec_kernel(const int32_t *__restrict__ codes, const float *__restrict__ seq_lp,
                                                               int64_t n_groups, int n, FieldMap fm, bool has_nc,
                                                               int32_t *__restrict__ win, uint32_t *__restrict__ meta,
                                                               float *__restrict__ weight) {
-    using M = typename MaskOf<NP>::type;
     extern __shared__ float wts[];  // [records of the tile][NP]
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int64_t n_tiles = (n_groups + T - 1) / T;
@@ -294,14 +314,9 @@ __global__ void __launch_bounds__(T) weighted_vote_rec_kernel(const int32_t *__r
         const int64_t g0 = tile * T, g1 = min(g0 + T, n_groups);
         const int64_t r0 = g0 / fm.n_fields, r1 = (g1 - 1) / fm.n_fields;
         for (int64_t r = r0 + warp; r <= r1; r += T / 32) {
-            float s_lo = (lane < n) ? __ldg(seq_lp + r * n + lane) : -3.0e38f;
-            float s_hi = (NP > 32 && lane + 32 < n) ? __ldg(seq_lp + r * n + lane + 32) : -3.0e38f;
-            float smax = fmaxf(s_lo, s_hi);
-#pragma unroll
-            for (int st = 16; st >= 1; st >>= 1) smax = fmaxf(smax, __shfl_xor_sync(0xFFFFFFFFu, smax, st));
-            float *w = wts + (r - r0) * NP;
-            if (lane < NP) w[lane] = kexp(__fadd_rn(s_lo, -smax));
-            if (NP > 32) w[lane + 32] = kexp(__fadd_rn(s_hi, -smax));
+            const float s_lo = (lane < n) ? __ldg(seq_lp + r * n + lane) : -3.0e38f;
+            const float s_hi = (NP > 32 && lane + 32 < n) ? __ldg(seq_lp + r * n + lane + 32) : -3.0e38f;
+            record_weights<NP>(s_lo, s_hi, wts + (r - r0) * NP, (uint32_t)lane);
         }
         __syncthreads();
         const int64_t g = g0 + tid;
@@ -384,9 +399,7 @@ __device__ __forceinline__ void wv_first_pass(const int32_t (&raw)[N], int32_t l
         f.voters = popc_m(live);
         f.present = present;
     }
-    // every other class sums a subset of the remaining weights: at most (total - cw_g) up to rounding (< 64 * 2^-23 relative on
-    // each side; 5e-5 * total is a safe slack).  Strictly below cw_g it can neither win nor tie.
-    f.decided = f.guess >= 0 && f.cw_g > __fadd_rn(__fadd_rn(f.total, -f.cw_g), __fmul_rn(f.total, 5e-5f));
+    f.decided = f.guess >= 0 && f.cw_g > wv_rest_bound(f.total, f.cw_g);
 }
 
 // The general walk (see weighted_core) for ONE group by the WHOLE warp: lane j holds cells j and j + 32 of the owner's group.  A
@@ -429,7 +442,7 @@ __device__ __forceinline__ void wv_warp_walk(uint32_t lane, uint32_t owner, cons
         live_hi &= ~g_hi;
     }
     while (live_lo | live_hi) {
-        if (__fadd_rn(__fadd_rn(total, -consumed), __fmul_rn(total, 5e-5f)) < best_w) break;  // the rest can neither win nor tie
+        if (wv_rest_bound(total, consumed) < best_w) break;
         // the heaviest cell still waiting, first of equals
         float mx = fmaxf(((live_lo >> lane) & 1u) ? w_lo : -1.0f, (N > 32 && ((live_hi >> lane) & 1u)) ? w_hi : -1.0f);
 #pragma unroll
@@ -470,21 +483,32 @@ __device__ __forceinline__ void wv_warp_walk(uint32_t lane, uint32_t owner, cons
     }
 }
 
+// x / n_fields for any 32-bit x without a division: the multiply-high by inv_fields = wv_inv_fields(n_fields) =
+// floor(2^64 / n_fields) + 1, exact for n_fields >= 2 (n_fields = 1 takes x itself).
+KC_HD inline uint64_t wv_inv_fields(uint32_t n_fields) { return n_fields > 1u ? ~uint64_t(0) / n_fields + 1u : 0u; }
+__device__ __forceinline__ uint32_t wv_record_of(uint32_t x, const FieldMap &fm, uint64_t inv_fields) {
+    return fm.n_fields == 1u ? x : (uint32_t)__umul64hi((uint64_t)x, inv_fields);
+}
+
 // K3b with K1's TMA front-end (n in {32, 64} cells per group = 128 / 256 byte rows; WarpTiles, kc_common.cuh) instead of one
 // 128-byte row per thread straight from global memory (latency-bound at 0.39 of the HBM peak: a warp's 32 rows are 32 separate
-// lines per load instruction).  The weights of the tile's records (32 groups span
-// 32 / n_fields + 2 records at most) are computed by the warp itself into its own shared-memory rows (lane = candidate, warp
-// max by shuffles), padded by one float so that lanes of different records read different banks; the pad slot carries the index of
-// the record's heaviest candidate, whose class weighted_core sums in its first pass (one pass decides most groups).  No block-wide
-// barrier.
+// lines per load instruction).  The weights of the tile's records (32 groups span 31 / n_fields + 2 records at most) are computed
+// by the warp itself (record_weights) into its own shared-memory rows of kWRowTile<N> = N + 1 floats: the odd pitch puts lanes of
+// different records in different banks, and the pad slot carries the index of the record's heaviest candidate, whose class
+// wv_first_pass sums in its one pass (which decides most groups).  No block-wide barrier.
+template <int N>
+constexpr int kWRowTile = N + 1;
+template <int N, int WARPS, int STAGES>
+constexpr size_t weighted_vote_tma_smem(int rec_cap) {
+    return WarpTiles<N * 4, WARPS, STAGES>::RING_BYTES + (size_t)WARPS * rec_cap * kWRowTile<N> * 4;
+}
+
 template <int N, int WARPS, int STAGES, int MIN_CTAS, bool PREFETCH>
 __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel(const __grid_constant__ CUtensorMap tmap, const float *__restrict__ seq_lp,
                                                                        uint32_t n_groups, FieldMap fm, bool has_nc, int rec_cap, uint64_t inv_fields,
                                                                        int32_t *__restrict__ win, uint32_t *__restrict__ meta,
                                                                        float *__restrict__ weight) {
-    constexpr int WROW = N + 1;
-    // x / n_fields for any 32-bit x without a division: inv_fields = floor(2^64 / n_fields) + 1 (exact for n_fields >= 2)
-    auto record_of = [&](uint32_t x) -> uint32_t { return fm.n_fields == 1u ? x : (uint32_t)__umul64hi((uint64_t)x, inv_fields); };
+    constexpr int WROW = kWRowTile<N>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     WarpTiles<N * 4, WARPS, STAGES> tiles(&tmap, n_groups);
     const uint32_t lane = tiles.lane;
@@ -500,7 +524,7 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
     float cur_lo[PF], cur_hi[PF], nxt_lo[PF], nxt_hi[PF];
     auto fetch = [&](uint32_t tt, float (&lo)[PF], float (&hi)[PF]) {
         const uint32_t a = tt * 32, b = min(a + 31u, n_groups - 1u);
-        const uint32_t ra = record_of(a), rb = record_of(b);
+        const uint32_t ra = wv_record_of(a, fm, inv_fields), rb = wv_record_of(b, fm, inv_fields);
 #pragma unroll
         for (int k = 0; k < PF; ++k) {
             lo[k] = hi[k] = -3.0e38f;
@@ -518,7 +542,7 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
         if (prefetch && t + tiles.step < tiles.n_tiles) fetch(t + tiles.step, nxt_lo, nxt_hi);
         // the weights of this tile's records, while the tile is still on its way
         const uint32_t g0 = t * 32, g_last = min(g0 + 31u, n_groups - 1u);
-        const uint32_t r0 = record_of(g0), r_last = record_of(g_last);
+        const uint32_t r0 = wv_record_of(g0, fm, inv_fields), r_last = wv_record_of(g_last, fm, inv_fields);
         for (uint32_t r = r0; r <= r_last; ++r) {
             const float *s = seq_lp + (size_t)r * N;
             float s_lo, s_hi = -3.0e38f;
@@ -530,15 +554,8 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
                 s_lo = __ldg(s + lane);
                 if (N > 32) s_hi = __ldg(s + lane + 32);
             }
-            float smax = fmaxf(s_lo, s_hi);
-#pragma unroll
-            for (int st = 16; st >= 1; st >>= 1) smax = fmaxf(smax, __shfl_xor_sync(0xFFFFFFFFu, smax, st));
             float *w = wts + (r - r0) * WROW;
-            w[lane] = kexp(__fadd_rn(s_lo, -smax));
-            if (N > 32) w[lane + 32] = kexp(__fadd_rn(s_hi, -smax));
-            // the record's heaviest candidate (first of the largest sums; N = none, e.g. all NaN) rides in the row's pad slot
-            const uint32_t b_lo = __ballot_sync(0xFFFFFFFFu, s_lo == smax), b_hi = __ballot_sync(0xFFFFFFFFu, N > 32 && s_hi == smax);
-            const int imax = b_lo ? __ffs((int)b_lo) - 1 : (b_hi ? 31 + __ffs((int)b_hi) : N);
+            const int imax = record_weights<N>(s_lo, s_hi, w, lane);
             if (lane == 0) w[N] = __int_as_float(imax);
         }
         __syncwarp();
@@ -599,25 +616,28 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
 }
 
 // ---- K3b with the weights OUT of the tile loop.  A pre-pass writes, once per record, the row [w_0 .. w_{N-1}, index of the heaviest
-// candidate, 3 pad words] (N + 4 floats: rows stay 16-byte multiples and consecutive rows start 4 banks apart); the vote kernel
-// fetches the rows of a tile's records with ONE cp.async.bulk next to the tile's tensor copy, completing on the same mbarrier.
+// candidate, 3 pad words] (kWRowBulk<N> = N + 4 floats: rows stay 16-byte multiples and consecutive rows start 4 banks apart); the
+// vote kernel fetches the rows of a tile's records with ONE cp.async.bulk next to the tile's tensor copy, completing on the same
+// mbarrier, into one of kWSlots<STAGES> = STAGES + 1 slots per warp: the slot of the tile being voted is not the one the re-arm refills.
+template <int N>
+constexpr int kWRowBulk = N + 4;
+template <int STAGES>
+constexpr int kWSlots = STAGES + 1;
+template <int N, int WARPS, int STAGES>
+constexpr size_t weighted_vote_rows_smem(int rec_cap) {
+    return WarpTiles<N * 4, WARPS, STAGES>::RING_BYTES + (size_t)WARPS * kWSlots<STAGES> * rec_cap * kWRowBulk<N> * 4;
+}
 
 template <int N>
 __global__ void __launch_bounds__(256) weight_rows_kernel(const float *__restrict__ seq_lp, int64_t n_records, float *__restrict__ rows) {
-    constexpr int WROW = N + 4;
+    constexpr int WROW = kWRowBulk<N>;
     const uint32_t lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = warp; r < n_records; r += n_warps) {
         const float *s = seq_lp + r * N;
         const float s_lo = __ldg(s + lane), s_hi = N > 32 ? __ldg(s + lane + 32) : -3.0e38f;
-        float smax = fmaxf(s_lo, s_hi);
-#pragma unroll
-        for (int st = 16; st >= 1; st >>= 1) smax = fmaxf(smax, __shfl_xor_sync(0xFFFFFFFFu, smax, st));
         float *w = rows + r * WROW;
-        w[lane] = kexp(__fadd_rn(s_lo, -smax));
-        if (N > 32) w[lane + 32] = kexp(__fadd_rn(s_hi, -smax));
-        const uint32_t b_lo = __ballot_sync(0xFFFFFFFFu, s_lo == smax), b_hi = __ballot_sync(0xFFFFFFFFu, N > 32 && s_hi == smax);
-        const int imax = b_lo ? __ffs((int)b_lo) - 1 : (b_hi ? 31 + __ffs((int)b_hi) : N);
+        const int imax = record_weights<N>(s_lo, s_hi, w, lane);
         if (lane < 4) w[N + lane] = lane == 0 ? __int_as_float(imax) : 0.0f;
     }
 }
@@ -627,9 +647,7 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kerne
                                                                         uint32_t n_groups, FieldMap fm, bool has_nc, int rec_cap, uint64_t inv_fields,
                                                                         int32_t *__restrict__ win, uint32_t *__restrict__ meta,
                                                                         float *__restrict__ weight) {
-    constexpr int WROW = N + 4;
-    constexpr int WSLOTS = STAGES + 1;  // the slot of the tile being voted is not the one the re-arm refills
-    auto record_of = [&](uint32_t x) -> uint32_t { return fm.n_fields == 1u ? x : (uint32_t)__umul64hi((uint64_t)x, inv_fields); };
+    constexpr int WROW = kWRowBulk<N>, WSLOTS = kWSlots<STAGES>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     WarpTiles<N * 4, WARPS, STAGES> tiles(&tmap, n_groups);
     const uint32_t lane = tiles.lane;
@@ -639,14 +657,14 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kerne
     // the weight rows of the records tile tt belongs to, into the weight slot of the warp's tile number j
     auto weight_rows = [&](uint32_t tt, uint32_t j) -> ExtraCopy {
         const uint32_t a = tt * 32, b = min(a + 31u, n_groups - 1u);
-        const uint32_t ra = record_of(a), rb = record_of(b);
+        const uint32_t ra = wv_record_of(a, fm, inv_fields), rb = wv_record_of(b, fm, inv_fields);
         return {wrows + (size_t)ra * WROW, my_rows + (j % WSLOTS) * slot_bytes, (rb - ra + 1u) * WROW * 4};
     };
     tiles.start(L2Policy::evict_first, weight_rows);
 
     for (; tiles.t < tiles.n_tiles; tiles.next()) {
         const uint32_t g0 = tiles.t * 32, g = g0 + lane;
-        const uint32_t r0 = record_of(g0);
+        const uint32_t r0 = wv_record_of(g0, fm, inv_fields);
         const uint32_t fpos = (g0 - r0 * fm.n_fields) + lane;  // offset inside the tile's first record: < n_fields + 32
         const uint32_t rec_local = g < n_groups ? fm.div_small(fpos) : 0u;
         const float *wts = my_rows_p + (tiles.it % WSLOTS) * (slot_bytes / 4);

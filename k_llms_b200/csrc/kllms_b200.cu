@@ -178,7 +178,7 @@ template <int N, int WARPS, int STAGES>
 int launch_vote_tma(const int32_t *codes, int64_t G, const int32_t *none_code, int n_fields, int32_t *win, uint32_t *meta,
                     cudaStream_t st, kc::OutRoute mc) {
     if (none_code && n_fields >= 60000) return kc_fail(KC_EINVAL, "kc_vote_i32: more than 60000 fields with none_code is not supported");
-    const size_t smem = (size_t)WARPS * STAGES * 32 * N * 4 + 1024;
+    const size_t smem = kc::WarpTiles<N * 4, WARPS, STAGES>::RING_BYTES;
     const kc::FieldMap fm = make_field_map(none_code, n_fields);
     auto go = [&](auto kernel) {
         return launch_tma_slabs(kernel, WARPS, smem, codes, G, N * 4, n_fields, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
@@ -252,7 +252,7 @@ template <int N, int WARPS, int STAGES, int MIN_CTAS>
 int launch_numeric_tma(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
                        cudaStream_t st, kc::OutRoute mc) {
     auto kernel = kc::numeric_tma_kernel<N, WARPS, STAGES, MIN_CTAS>;
-    const size_t smem = (size_t)WARPS * STAGES * 32 * N * 8 + (size_t)WARPS * 32 * N * 8 + 1024;
+    const size_t smem = kc::WarpTiles<N * 8, WARPS, STAGES>::RING_BYTES + (size_t)WARPS * 32 * N * 8;  // + the [cell][thread] plane
     return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
         kernel<<<grid, WARPS * 32, smem, st>>>(map, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
     });
@@ -263,7 +263,7 @@ template <int N, int WARPS, int STAGES, int MIN_CTAS>
 int launch_numeric_tma_fast(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
                             cudaStream_t st) {
     auto kernel = kc::numeric_tma_fast_kernel<N, WARPS, STAGES, MIN_CTAS>;
-    const size_t smem = (size_t)WARPS * STAGES * 32 * N * 8 + (size_t)WARPS * 32 * N * 8 + 1024;
+    const size_t smem = kc::WarpTiles<N * 8, WARPS, STAGES>::RING_BYTES + (size_t)WARPS * 32 * N * 8;  // + the [cell][thread] plane
     return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
         kernel<<<grid, WARPS * 32, smem, st>>>(map, vals + g0 * N, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0);
     });
@@ -673,7 +673,7 @@ int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     if ((n == 32 || n == 64) && n_fields < 60000) {  // rows through K1's warp-private TMA pipelines
         const int rec_cap = std::min(32, 31 / n_fields + 2);  // records a tile of 32 groups can span
-        const uint64_t inv_fields = n_fields > 1 ? ~uint64_t(0) / (uint64_t)n_fields + 1 : 0;
+        const uint64_t inv_fields = kc::wv_inv_fields((uint32_t)n_fields);
         // weights: `wrow` floats per record, from `wts`
         auto launch_tma = [&](auto kernel, int N, int warps, size_t smem, const float *wts, int wrow) {
             return launch_tma_slabs(kernel, warps, smem, d_codes, G, N * 4, n_fields, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
@@ -682,7 +682,7 @@ int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int
             });
         };
         if (n == 32 && rec_cap <= 8) {  // weights by a pre-pass, fetched per tile by a bulk copy (n_fields >= 6; n = 32 only)
-            constexpr int N = 32, WARPS = 8, STAGES = 2, WROW = N + 4;
+            constexpr int N = 32, WARPS = 8, STAGES = 2, WROW = kc::kWRowBulk<N>;
             int pre_grid = 0;
             int rc = stride_grid((n_records + 7) / 8, pre_grid);
             if (rc) return rc;
@@ -690,16 +690,16 @@ int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int
             KC_CUDA_I(cudaMallocAsync(reinterpret_cast<void **>(&d_rows), (size_t)n_records * WROW * 4, st));
             kc::weight_rows_kernel<N><<<pre_grid, 256, 0, st>>>(d_seq_logprob, n_records, d_rows);
             rc = cudaGetLastError() == cudaSuccess ? KC_OK : kc_fail(KC_ECUDA, "kc_weighted_vote_i32: weight_rows_kernel launch failed");
-            const size_t smem = (size_t)WARPS * STAGES * 32 * N * 4 + 1024 + (size_t)WARPS * (STAGES + 1) * rec_cap * WROW * 4;
+            const size_t smem = kc::weighted_vote_rows_smem<N, WARPS, STAGES>(rec_cap);
             if (!rc) rc = launch_tma(kc::weighted_vote_rows_kernel<N, WARPS, STAGES, 3>, N, WARPS, smem, d_rows, WROW);
             cudaFreeAsync(d_rows, st);
             return rc;
         }
         // n = 32 with 3 CTAs / SM (80 registers) and the logprobs requested a tile ahead; n = 64 (2 x the registers per row)
         // without the prefetch (not re-timed on H100)
-        auto tma_smem = [&](int N, int warps, int stages) { return (size_t)warps * stages * 32 * N * 4 + 1024 + (size_t)warps * rec_cap * (N + 1) * 4; };
-        if (n == 32) return launch_tma(kc::weighted_vote_tma_kernel<32, 8, 2, 3, true>, 32, 8, tma_smem(32, 8, 2), d_seq_logprob, 32);
-        return launch_tma(kc::weighted_vote_tma_kernel<64, 4, 2, 3, false>, 64, 4, tma_smem(64, 4, 2), d_seq_logprob, 64);
+        if (n == 32)
+            return launch_tma(kc::weighted_vote_tma_kernel<32, 8, 2, 3, true>, 32, 8, kc::weighted_vote_tma_smem<32, 8, 2>(rec_cap), d_seq_logprob, 32);
+        return launch_tma(kc::weighted_vote_tma_kernel<64, 4, 2, 3, false>, 64, 4, kc::weighted_vote_tma_smem<64, 4, 2>(rec_cap), d_seq_logprob, 64);
     }
     // n < 8: one group per thread, weights computed per group; faster there than the per-record kernel below (H100 SXM,
     // 700 W, 256 K records x 24 fields: 0.07 against 0.16 ms at n = 2, 0.11 against 0.16 ms at n = 4)
