@@ -213,6 +213,18 @@ int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int
                          void *stream);
 
 /*
+ * K3b over ragged records (self-defined, DESIGN.md §5): the same vote as kc_weighted_vote_i32, bit for bit, for groups that
+ * belong to records in any order and any number — what a planner produces when records differ in their vote fields.
+ *   d_codes int8[n_groups][n] as kc_vote_i8 (-1 None: does not vote, -2 absent, local codes >= 0; 16-byte aligned)
+ *   d_group_record int32[n_groups]: the record of group g, in [0, n_records) (another index: the group gets meta 0, weight 0)
+ *   d_seq_logprob float32[n_records][n]: the records' candidate sums (kc_logprob_sum_f32)
+ *   d_win_code int32[n_groups], d_meta uint32[n_groups] (KC_META_*), d_weight float32[n_groups] as kc_weighted_vote_i32
+ */
+int kc_weighted_vote_groups_i8(const int8_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_group_record,
+                               const float *d_seq_logprob, int64_t n_records, int32_t *d_win_code, uint32_t *d_meta, float *d_weight,
+                               void *stream);
+
+/*
  * K4 — similarity medoid of string groups (consensus_as_primitive fallback, consensus_utils.py:1221-1237, with
  * levenshtein_similarity :745-761): pairwise 1 - dist/max_len (floored at 1e-8) on NORMALISED strings (lower-case [a-z0-9],
  * normalize_string :660-673, done by the caller), np.nanmean of each row in numpy's summation order, first argmax.
@@ -350,6 +362,12 @@ typedef struct {
 } kc_json_stats;
 int kc_consolidate_json_packed(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, double rel_eps, double abs_eps,
                                int device, int32_t threads, uint32_t flags, kc_json_result **out);
+/* Likelihood-weighted variant (self-defined, DESIGN.md §5): h_seq_logprob float32[n_records * n] = the candidates' sequence
+ * logprobs (kc_logprob_sum_f32), record-major like h_off.  The vote leaves are decided by K3b over ragged records
+ * (kc_weighted_vote_groups_i8) in K1's place and their likelihood is round(weight, 5) (kc::weighted_vote_confidence); everything
+ * else as above.  The host path votes by count, so records the device path declines are NOT handed to it: they keep status 1. */
+int kc_consolidate_json_packed_weighted(const char *h_text, const int64_t *h_off, const float *h_seq_logprob, int64_t n_records, int32_t n,
+                                        double rel_eps, double abs_eps, int device, int32_t threads, uint32_t flags, kc_json_result **out);
 /* record r: content = text[content_off[r] .. +content_len[r]), likelihoods likewise; `why` = the device path's reason code for
  * declining (0 = not declined; kc_jsoncore.cuh D_*).  Pointers stay valid until kc_json_result_free.  Any output may be NULL. */
 int kc_json_result_view(kc_json_result *res, const char **text, const int64_t **content_off, const int64_t **content_len,
@@ -365,6 +383,12 @@ int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells
                             int64_t *n_num_groups, const uint8_t **status);
 int kc_debug_jsongpu_emit(kc_debug_jsongpu *h, const uint32_t *vote_meta, const double *num_value, const uint32_t *num_meta,
                           const char **content, const int64_t **content_off, const char **likelihoods, const int64_t **likelihoods_off);
+/* the weighted variant's phases: the (batch-local) record of every vote group, what kc_weighted_vote_groups_i8 takes; and the
+ * emit with K3b's weights (vote_weight NULL: count votes, as kc_debug_jsongpu_emit) */
+int kc_debug_jsongpu_group_records(const kc_debug_jsongpu *h, const int32_t **group_record);
+int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_meta, const float *vote_weight, const double *num_value,
+                                   const uint32_t *num_meta, const char **content, const int64_t **content_off, const char **likelihoods,
+                                   const int64_t **likelihoods_off);
 /* the batch's medoid groups (multi-word string fields) in kc_medoid_str's CSR form; K4's results go in through _set_medoid
  * (before _emit; the arrays must stay alive until _emit has returned) */
 int kc_debug_jsongpu_medoid_inputs(const kc_debug_jsongpu *h, const uint8_t **chars, const int32_t **str_off, const int32_t **grp_off,

@@ -47,6 +47,7 @@ _SIGNATURES = {
     "kc_confidence_f64": (_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "kc_logprob_sum_f32": (_int, [_vp, _vp, _i64, _vp, _vp]),
     "kc_weighted_vote_i32": (_int, [_vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
+    "kc_weighted_vote_groups_i8": (_int, [_vp, _i64, _i32, _vp, _vp, _i64, _vp, _vp, _vp, _vp]),
     "kc_consensus_host": (_int, _CONSENSUS_HOST),
     "kc_consensus_host_i8": (_int, _CONSENSUS_HOST),
     "kc_host_alloc": (_vp, [_u64]),
@@ -64,6 +65,7 @@ _SIGNATURES = {
     "kc_json_emit": (_int, [_vp] * 9),
     "kc_json_free": (None, [_vp]),
     "kc_consolidate_json_packed": (_int, [_vp, _vp, _i64, _i32, _f64, _f64, _int, _i32, _u32, _pp]),
+    "kc_consolidate_json_packed_weighted": (_int, [_vp, _vp, _vp, _i64, _i32, _f64, _f64, _int, _i32, _u32, _pp]),
     "kc_json_result_view": (_int, [_vp] + [_pp] * 7 + [_vp]),
     "kc_json_result_free": (None, [_vp]),
     "kc_debug_similarity_json": (_int, [_str, _str, ctypes.POINTER(_f64)]),
@@ -72,6 +74,8 @@ _SIGNATURES = {
     "kc_debug_jsongpu_plan": (_int, [_vp, _vp, _i64, _i32, _pp]),
     "kc_debug_jsongpu_inputs": (_int, [_vp] * 6),
     "kc_debug_jsongpu_emit": (_int, [_vp, _vp, _vp, _vp] + [_pp] * 4),
+    "kc_debug_jsongpu_group_records": (_int, [_vp, _pp]),
+    "kc_debug_jsongpu_emit_weighted": (_int, [_vp, _vp, _vp, _vp, _vp] + [_pp] * 4),
     "kc_debug_jsongpu_medoid_inputs": (_int, [_vp] + [_pp] * 3 + [ctypes.POINTER(_i64)]),
     "kc_debug_jsongpu_set_medoid": (_int, [_vp, _vp, _vp]),
     "kc_debug_jsongpu_free": (None, [_vp]),
@@ -224,6 +228,25 @@ def weighted_vote(codes, seq_logprob, none_code=None, stream=None):
     _bind(torch, codes)
     check(load().kc_weighted_vote_i32(codes.data_ptr(), seq_logprob.data_ptr(), R, F, n, nc, win.data_ptr(), meta.data_ptr(),
                                       weight.data_ptr(), _stream_ptr(torch, stream)))
+    return win, meta, weight
+
+
+def weighted_vote_groups(codes, group_record, seq_logprob, stream=None):
+    """K3b over ragged records: codes int8 [G, n] (kc_vote_i8 cells), group_record int32 [G] (the record of each group),
+    seq_logprob float32 [R, n] (cuda).  Returns (win_code int32 [G], meta int32 [G], weight float32 [G])."""
+    torch = _require_cuda()
+    assert codes.is_cuda and codes.dtype == torch.int8 and codes.dim() == 2 and codes.is_contiguous()
+    G, n = codes.shape
+    assert group_record.is_cuda and group_record.dtype == torch.int32 and group_record.is_contiguous() and group_record.numel() == G
+    assert seq_logprob.is_cuda and seq_logprob.dtype == torch.float32 and seq_logprob.dim() == 2 and seq_logprob.is_contiguous()
+    R = seq_logprob.shape[0]
+    assert R == 0 or seq_logprob.shape[1] == n
+    win = torch.empty(G, dtype=torch.int32, device=codes.device)
+    meta = torch.empty(G, dtype=torch.int32, device=codes.device)
+    weight = torch.empty(G, dtype=torch.float32, device=codes.device)
+    _bind(torch, codes)
+    check(load().kc_weighted_vote_groups_i8(codes.data_ptr(), G, n, group_record.data_ptr(), seq_logprob.data_ptr() if R else None, R,
+                                            win.data_ptr(), meta.data_ptr(), weight.data_ptr(), _stream_ptr(torch, stream)))
     return win, meta, weight
 
 
@@ -491,6 +514,21 @@ def consolidate_json_packed(blob, off, n, rel_eps: float = 0.03, abs_eps: float 
     h = ctypes.c_void_p()
     check(lib.kc_consolidate_json_packed(blob.ctypes.data, off.ctypes.data, R, n, float(rel_eps), float(abs_eps), device, threads,
                                          flags, ctypes.byref(h)))
+    return PackedResult(h, R)
+
+
+def consolidate_json_packed_weighted(blob, off, n, seq_logprob, rel_eps: float = 0.03, abs_eps: float = 1e-6, device: int = 0,
+                                     threads: int = 0, flags: int = 0) -> PackedResult:
+    """H1g with likelihood-weighted vote leaves (kc_consolidate_json_packed_weighted, DESIGN.md §5): seq_logprob float32
+    [R*n] = the candidates' sequence logprobs, record-major.  Records the device path declines keep status 1 (no host path)."""
+    import numpy as np
+    lib = load()
+    R = (len(off) - 1) // n if n else 0
+    seq = np.ascontiguousarray(seq_logprob, dtype=np.float32).reshape(-1)
+    assert seq.size == R * n, "one sequence logprob per candidate"
+    h = ctypes.c_void_p()
+    check(lib.kc_consolidate_json_packed_weighted(blob.ctypes.data, off.ctypes.data, seq.ctypes.data if seq.size else None, R, n,
+                                                  float(rel_eps), float(abs_eps), device, threads, flags, ctypes.byref(h)))
     return PackedResult(h, R)
 
 

@@ -82,10 +82,11 @@ class _Const:
 
 
 class _VoteLeaf:
-    __slots__ = ("row", "cells", "pvf")
+    __slots__ = ("row", "cells", "pvf", "where")
 
-    def __init__(self, row: int, cells: list, pvf: float):
+    def __init__(self, row: int, cells: list, pvf: float, where: Optional[dict] = None):
         self.row, self.cells, self.pvf = row, cells, pvf  # cells[i] = value returned when cell i wins
+        self.where = where  # weighted plans: candidate position of a cell -> its index in `cells`
 
 
 class _NumLeaf:
@@ -117,10 +118,16 @@ class _ListNode:
 
 
 class Plan:
-    """Leaf groups of one or many records, ready for one K1, one K2 and one K4 launch."""
+    """Leaf groups of one or many records, ready for one K1, one K2 and one K4 launch.
+
+    Weighted plans (`weighted=True`, DESIGN.md §5, likelihood-weighted consensus): every record starts with `begin_record(sums)`,
+    the fp32 sequence logprobs of its candidates.  Vote cells then stay at their CANDIDATE's position (a candidate that is not a
+    dict / list at some node is an absent cell below it, instead of being compacted away), each vote row remembers its record,
+    and `run()` votes with one launch of K3b over ragged records (kc_weighted_vote_groups_i8) instead of K1.  Everything else —
+    numeric clusters, medoids, parent_valid_frac, key order — is planned exactly as in count mode."""
 
     def __init__(self, n: int, allow_none_as_candidate: bool, rel_eps: float, abs_eps: float, host_primitive: Callable,
-                 numeric_branch: bool = True):
+                 numeric_branch: bool = True, weighted: bool = False):
         if n > MAX_CANDIDATES:
             raise ValueError(f"{n} candidates per request: k_llms_b200 consolidates at most {MAX_CANDIDATES} (one kernel row per "
                              "field holds every candidate; the package has no CPU path to fall back to)")
@@ -135,9 +142,19 @@ class Plan:
         self.num_rows: List[List[float]] = []
         self.medoid_groups: List[List[str]] = []  # normalised strings of the groups K4 handles
         self.string_method = "embeddings"         # set by the caller (ConsensusSettings.string_similarity_method)
+        self.weighted = weighted
+        self.vote_record: List[int] = []          # weighted: the record of each vote row
+        self.seq_logprobs: List[List[float]] = []  # weighted: the candidates' sums of each record, padded to n
+
+    def begin_record(self, seq_logprobs: Sequence[float]) -> None:
+        """Weighted plans: the records' candidate sums, in the order of the add() calls that plan them."""
+        if len(seq_logprobs) > self.n:
+            raise ValueError(f"{len(seq_logprobs)} sequence logprobs for at most {self.n} candidates")
+        # a candidate the record does not have weighs nothing, and does not shift the record's maximum (kc_weighted_vote_groups_i8)
+        self.seq_logprobs.append([float(s) for s in seq_logprobs] + [-3.0e38] * (self.n - len(seq_logprobs)))
 
     # -- leaves ---------------------------------------------------------------------------------------
-    def _vote(self, values: Sequence[Any], pvf: float) -> _VoteLeaf:
+    def _vote(self, values: Sequence[Any], pvf: float, pos: Optional[Sequence[int]] = None) -> _VoteLeaf:
         first = next(v for v in values if v is not None)
         codes: List[int] = []
         table: dict = {}
@@ -153,9 +170,16 @@ class Plan:
                 else:
                     k = None if v is None else sanitize_value(v)
                     codes.append(table.setdefault(k, len(table)))
+        where = None
+        if pos is not None:  # weighted: cell i at candidate pos[i], the candidates filtered out above are absent
+            row = [_native.CODE_ABSENT] * self.n
+            for p, c in zip(pos, codes):
+                row[p] = c
+            codes, where = row, {p: i for i, p in enumerate(pos)}
+            self.vote_record.append(len(self.seq_logprobs) - 1)
         codes.extend([_native.CODE_ABSENT] * (self.n - len(codes)))
         self.vote_rows.append(codes)
-        return _VoteLeaf(len(self.vote_rows) - 1, cells, pvf)
+        return _VoteLeaf(len(self.vote_rows) - 1, cells, pvf, where)
 
     def _numeric(self, values: Sequence[Any], pvf: float) -> _NumLeaf:
         row: List[float] = []
@@ -174,7 +198,13 @@ class Plan:
         return _NumLeaf(len(self.num_rows) - 1, list(values), pvf)
 
     # -- dispatcher (cu:1376-1454) ----------------------------------------------------------------------
-    def add(self, values: Sequence[Any], pvf: float, embed: Optional[Callable]):
+    def add(self, values: Sequence[Any], pvf: float, embed: Optional[Callable], pos: Optional[Sequence[int]] = None):
+        """Plan one record's candidate values (or, recursively, one node's).  pos (weighted plans): the candidate position of
+        each value; a weighted record's top-level call leaves it to default to 0..len(values)-1."""
+        if self.weighted and pos is None:
+            if len(self.seq_logprobs) == 0:
+                raise ValueError("a weighted plan needs begin_record(seq_logprobs) before each record")
+            pos = range(len(values))
         if not values:
             return _Const(None, pvf)  # cu:1395-1396
         live = [v for v in values if v is not None]
@@ -182,9 +212,11 @@ class Plan:
             return _Const(None, 0.0)  # cu:1401-1402
         head = live[0]
         if isinstance(head, (str, bool)) and all(len(str(v).strip().split()) < 3 for v in live):
-            return self._vote(values, pvf)  # cu:1405-1411
+            return self._vote(values, pvf, pos)  # cu:1405-1411
         if isinstance(head, dict):  # cu:1414-1426 -> consensus_dict cu:1269-1306
-            dicts = [v for v in values if isinstance(v, dict)]
+            keep = [i for i, v in enumerate(values) if isinstance(v, dict)]
+            dicts = [values[i] for i in keep]
+            sub_pos = None if pos is None else [pos[i] for i in keep]
             sub = pvf * (len(dicts) / len(values))
             keys: dict = {}
             for d in dicts:
@@ -194,13 +226,15 @@ class Plan:
             for k in keys:
                 if any(mark in k for mark in SKIPPED_KEY_MARKERS):
                     continue
-                children[k] = self.add([d.get(k) for d in dicts], sub, embed)
+                children[k] = self.add([d.get(k) for d in dicts], sub, embed, sub_pos)
             return _DictNode(children)
         if isinstance(head, list):  # cu:1429-1441 -> consensus_list cu:1309-1352
-            lists = [v for v in values if isinstance(v, list)]
+            keep = [i for i, v in enumerate(values) if isinstance(v, list)]
+            lists = [values[i] for i in keep]
+            sub_pos = None if pos is None else [pos[i] for i in keep]
             sub = pvf * (len(lists) / len(values))
             longest = max(len(l) for l in lists)
-            return _ListNode([self.add([l[i] if i < len(l) else None for l in lists], sub, embed) for i in range(longest)])
+            return _ListNode([self.add([l[i] if i < len(l) else None for l in lists], sub, embed, sub_pos) for i in range(longest)])
         if embed is None:  # cu:1445-1446
             raise ValueError("sync_get_openai_embeddings_from_text is required for primitive consensus")
         try:
@@ -242,7 +276,14 @@ class Plan:
             raise RuntimeError("k_llms_b200: no CUDA device — the consensus hot path has no CPU fallback")
         dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         out = {}
-        if self.vote_rows:
+        if self.vote_rows and self.weighted:  # K3b over ragged records: every cell is a local code < 64, so int8 holds it
+            codes = torch.from_numpy(np.asarray(self.vote_rows, dtype=np.int8)).to(dev)
+            rec = torch.from_numpy(np.asarray(self.vote_record, dtype=np.int32)).to(dev)
+            seq = torch.from_numpy(np.asarray(self.seq_logprobs, dtype=np.float32).reshape(-1, self.n)).to(dev)
+            _, meta, weight = _native.weighted_vote_groups(codes, rec, seq)
+            out["vote_meta"] = meta.cpu().numpy().view(np.uint32)
+            out["vote_weight"] = weight.cpu().numpy()
+        elif self.vote_rows:
             codes = torch.from_numpy(np.asarray(self.vote_rows, dtype=np.int32)).to(dev)
             _, meta = _native.vote(codes, None)
             out["vote_meta"] = meta.cpu().numpy().view(np.uint32)
@@ -288,6 +329,8 @@ class Plan:
             idx, support, _nn, present, flags = self._fields(int(res["vote_meta"][node.row]))
             if not flags & _native.FLAG_HAS_VALUE:  # cannot happen for a planned vote group (>= 1 voter)
                 return None, (node.pvf if present == 0 else 0.0)
+            if node.where is not None:  # weighted (DESIGN.md §5): idx is a candidate position; pvf x the winner's share of the weight
+                return node.cells[node.where[idx]], round(node.pvf * float(res["vote_weight"][node.row]), 5)
             return node.cells[idx], round(node.pvf * (support / present), 5)  # cu:971,973,982
         idx, support, nn, present, flags = self._fields(int(res["num_meta"][node.row]))
         if flags & _native.FLAG_HAS_VALUE:

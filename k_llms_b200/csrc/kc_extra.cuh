@@ -628,18 +628,35 @@ constexpr size_t weighted_vote_rows_smem(int rec_cap) {
     return WarpTiles<N * 4, WARPS, STAGES>::RING_BYTES + (size_t)WARPS * kWSlots<STAGES> * rec_cap * kWRowBulk<N> * 4;
 }
 
-template <int N>
-__global__ void __launch_bounds__(256) weight_rows_kernel(const float *__restrict__ seq_lp, int64_t n_records, float *__restrict__ rows) {
+// The weight-row pre-pass, one warp per record.  FULL: n == N candidates per record (N >= 32).  Otherwise N is a bucket (a
+// power of two >= n): records of n sums each, the lanes from n on weigh nothing (-3.0e38f, as for the missing candidates of
+// record_weights).
+template <int N, bool FULL>
+__device__ __forceinline__ void weight_rows(const float *__restrict__ seq_lp, int64_t n_records, int n, float *__restrict__ rows) {
     constexpr int WROW = kWRowBulk<N>;
     const uint32_t lane = threadIdx.x & 31;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
     for (int64_t r = warp; r < n_records; r += n_warps) {
-        const float *s = seq_lp + r * N;
-        const float s_lo = __ldg(s + lane), s_hi = N > 32 ? __ldg(s + lane + 32) : -3.0e38f;
+        const float *s = seq_lp + r * (FULL ? N : n);
+        const float s_lo = (FULL || (int)lane < n) ? __ldg(s + lane) : -3.0e38f;
+        const float s_hi = (N > 32 && (FULL || (int)lane + 32 < n)) ? __ldg(s + lane + 32) : -3.0e38f;
         float *w = rows + r * WROW;
         const int imax = record_weights<N>(s_lo, s_hi, w, lane);
         if (lane < 4) w[N + lane] = lane == 0 ? __int_as_float(imax) : 0.0f;
     }
+}
+
+template <int N>
+__global__ void __launch_bounds__(256) weight_rows_kernel(const float *__restrict__ seq_lp, int64_t n_records, float *__restrict__ rows) {
+    static_assert(N >= 32, "every lane holds a candidate");
+    weight_rows<N, true>(seq_lp, n_records, N, rows);
+}
+
+// the rows of records of n <= NP candidates (kc_weighted_vote_groups_i8)
+template <int NP>
+__global__ void __launch_bounds__(256) weight_rows_n_kernel(const float *__restrict__ seq_lp, int64_t n_records, int n,
+                                                            float *__restrict__ rows) {
+    weight_rows<NP, false>(seq_lp, n_records, n, rows);
 }
 
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
@@ -711,6 +728,33 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kerne
             meta[g] = o_meta;
             weight[g] = o_weight;
         }
+    }
+}
+
+// ---- K3b over ragged records (kc_weighted_vote_groups_i8): group g belongs to record group_record[g], in any order, and a
+// record has any number of groups — the shape a planner produces when records differ in their vote fields.  Cells are K1's
+// int8 cells (kc_vote_i8: -1 None, -2 absent, local codes >= 0, no none_code table).  The weight rows [R][kWRowBulk<NP>] come
+// from weight_rows_kernel<NP, n == NP>; one thread votes one group with weighted_core, reading its record's row from global
+// memory (rows of the same record are shared by its groups: L1 / L2 hits).  A group whose record index is outside
+// [0, n_records) gets no value (meta 0, weight 0).
+template <int NP, bool VEC>
+__global__ void __launch_bounds__(128) weighted_vote_groups_kernel(const int8_t *__restrict__ codes, int64_t n_groups, int n,
+                                                                   const int32_t *__restrict__ group_record, int64_t n_records,
+                                                                   const float *__restrict__ wrows, int32_t *__restrict__ win,
+                                                                   uint32_t *__restrict__ meta, float *__restrict__ weight) {
+    constexpr int WROW = kWRowBulk<NP>;
+    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
+    for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += stride) {
+        const int32_t rec = __ldg(group_record + g);
+        int32_t raw[NP];
+        load_row_i8<NP, VEC>(codes, g, n, raw);
+        if (rec < 0 || rec >= n_records) {
+            win[g] = KC_CODE_NONE;
+            meta[g] = 0u;
+            weight[g] = 0.0f;
+            continue;
+        }
+        weighted_core<NP>(raw, KC_CODE_NONE, wrows + (int64_t)rec * WROW, win[g], meta[g], weight[g]);
     }
 }
 

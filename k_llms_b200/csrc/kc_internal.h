@@ -5,6 +5,7 @@
 //     py_round5            round(x, 5)                                 (consensus_utils.py:982,1178,1187,1219)
 //     confidence           the confidence of a vote / numeric result word (cu:971-982,1085-1086,1116,1177-1219,1396,1402)
 //     medoid_confidence    the confidence of a similarity medoid        (cu:1085-1086,1233-1237)
+//     weighted_vote_confidence  the likelihood of a likelihood-weighted vote leaf (self-defined, DESIGN.md §5)
 //     py_isclose           math.isclose(a, b, rel_tol=0.01)             (cu:827-841)
 //     kSimFloor            SIMILARITY_SCORE_LOWER_BOUND                 (cu:78)
 // float.__repr__ is kc::js::float_repr (kc_jsoncore.cuh); the edit distance is kc_levenshtein (kc_json.cpp) on the host
@@ -91,6 +92,11 @@ KC_HD inline double confidence(uint32_t m, bool numeric, double pvf) {
     if (flags & KC_FLAG_NO_FINITE) return pvf * (nn / present);  // cu:1444,1116
     return present == 0.0 ? pvf : 0.0;  // cu:1396 / cu:1402
 }
+
+// The likelihood of a likelihood-weighted vote leaf (DESIGN.md §5, self-defined): pvf times K3b's fp32 weight (the winning
+// class's share of the voting weight), rounded like every vote confidence.  The Python epilogue (columnar.Plan.materialise)
+// computes the same round(pvf * float(w), 5).
+KC_HD inline double weighted_vote_confidence(double pvf, float weight) { return py_round5(pvf * (double)weight); }
 
 // The confidence of a similarity medoid among the `live` non-None strings of n candidates, avg = the medoid's mean
 // similarity: cu:1444 then cu:1085-1086 (one string: itself, unrounded) or cu:1233-1237 (the medoid, rounded).

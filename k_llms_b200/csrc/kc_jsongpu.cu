@@ -75,7 +75,7 @@ struct Worker {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[7] = {};
     DBuf text, off, fcount, slot, status, vbase, xbase, counters, toks, fdesc, piece_c, piece_l, vcells, xcells, win, vmeta, xvalue, xmeta,
-        len_c, len_l, out_c, out_l, scan_tmp, mcount, scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, gpos;
+        len_c, len_l, out_c, out_l, scan_tmp, mcount, scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, gpos, seq, vrec, vweight;
     PBuf h_small;  // totals and counters (pinned so the small D2H copies are asynchronous)
     PBuf h_scan;   // the scanned record offsets and the statuses of a chunk
     bool busy = false;
@@ -185,9 +185,10 @@ struct ChunkStage {  // per-chunk device-time split (CUDA events on the chunk's 
     float h2d = 0, plan = 0, kernels = 0, emit = 0, d2h = 0;
 };
 
-// One chunk on one worker: records [r0, r1) of the batch.
-int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, int64_t r0, int64_t r1, int32_t n, double rel_eps, double abs_eps,
-              int sm_count, kc_json_result &res, ChunkStage &st) {
+// One chunk on one worker: records [r0, r1) of the batch.  h_seq (NULL: count votes): the batch's candidate sums [R][n], the
+// vote leaves are likelihood-weighted (K3b over ragged records in K1's place).
+int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, int64_t r0, int64_t r1, int32_t n, double rel_eps,
+              double abs_eps, int sm_count, kc_json_result &res, ChunkStage &st) {
     const int64_t Rc = r1 - r0;
     const int64_t b0 = h_off[r0 * n], b1 = h_off[r1 * n];
     const size_t bytes = (size_t)(b1 - b0);
@@ -215,6 +216,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, int64_t r0, i
     R_(w.len_l.reserve((size_t)(Rc + 1) * 8));
     R_(w.h_small.reserve(64));
     R_(w.h_scan.reserve((size_t)(Rc + 1) * 16 + (size_t)Rc));
+    if (h_seq) R_(w.seq.reserve((size_t)std::max<int64_t>(Rc * n, 1) * 4));
     size_t tmp_bytes = 0, tmp_bytes32 = 0;
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (const int64_t *)nullptr, (int64_t *)nullptr, (int)(Rc + 1), s);
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes32, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(Rc + 1), s);
@@ -242,6 +244,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, int64_t r0, i
     KC_CUDA_I(cudaEventRecord(w.ev[0], s));
     KC_CUDA_I(cudaMemcpyAsync(w.text.p, h_text + b0, bytes, cudaMemcpyHostToDevice, s));
     KC_CUDA_I(cudaMemcpyAsync(w.off.p, h_off + r0 * n, (size_t)(Rc * n + 1) * 8, cudaMemcpyHostToDevice, s));
+    if (h_seq) KC_CUDA_I(cudaMemcpyAsync(w.seq.p, h_seq + r0 * n, (size_t)(Rc * n) * 4, cudaMemcpyHostToDevice, s));  // the chunk's sums
     KC_CUDA_I(cudaEventRecord(w.ev[1], s));
     nvtxRangePop();
     nvtxRangePushA("kc_json: plan (A0 count, A1 scan/type/encode)");
@@ -284,6 +287,12 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, int64_t r0, i
     ch.vmeta = w.vmeta.as<uint32_t>();
     ch.xvalue = w.xvalue.as<double>();
     ch.xmeta = w.xmeta.as<uint32_t>();
+    if (h_seq) {
+        R_(w.vrec.reserve(std::max<size_t>(T, 1) * 4));
+        R_(w.vweight.reserve(std::max<size_t>(T, 1) * 4));
+        ch.vrec = w.vrec.as<int32_t>();
+        ch.vweight = w.vweight.as<float>();
+    }
     KC_CUDA_I(cudaMemsetAsync(w.counters.p, 0, 24, s));
     // records declined before slots_phase own no medoid groups
     KC_CUDA_I(cudaMemsetAsync(w.mcount.p, 0, (size_t)(Rc + 1) * 4, s));
@@ -329,7 +338,11 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, int64_t r0, i
     nvtxRangePop();
     nvtxRangePushA("kc_json: K1 vote + K2 numeric + K4 medoid");
     // K1 / K2 / K4: the same kernels as the columnar path (one "field" per group: local codes, no none_code table)
-    if (gv) R_(kc_vote_i8(ch.vcells, gv, n, nullptr, 1, w.win.as<int32_t>(), w.vmeta.as<uint32_t>(), s));
+    if (gv && h_seq)
+        R_(kc_weighted_vote_groups_i8(ch.vcells, gv, n, ch.vrec, w.seq.as<float>(), Rc, w.win.as<int32_t>(), w.vmeta.as<uint32_t>(),
+                                      w.vweight.as<float>(), s));
+    else if (gv)
+        R_(kc_vote_i8(ch.vcells, gv, n, nullptr, 1, w.win.as<int32_t>(), w.vmeta.as<uint32_t>(), s));
     if (gx) R_(kc_numeric_f64(ch.xcells, gx, n, rel_eps, abs_eps, w.xvalue.as<double>(), w.xmeta.as<uint32_t>(), s));
     if (gm) R_(kc_medoid_str(ch.mchars, ch.mstr_off, ch.mgrp_off, gm, std::max(2, n), w.midx.as<int32_t>(), w.mavg.as<double>(), s));
     KC_CUDA_I(cudaEventRecord(w.ev[3], s));
@@ -405,9 +418,14 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, int64_t r0, i
 
 extern "C" {
 
-int kc_consolidate_json_packed(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, double rel_eps, double abs_eps,
-                               int device, int32_t threads, uint32_t flags, kc_json_result **out) {
+namespace {
+
+// kc_consolidate_json_packed, and with h_seq its likelihood-weighted variant (which hands no record to the host path: that
+// path votes by count)
+int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_seq, int64_t n_records, int32_t n, double rel_eps,
+                       double abs_eps, int device, int32_t threads, uint32_t flags, kc_json_result **out) {
     if (!out) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: NULL out");
+    if (h_seq) flags |= KC_JSON_DEVICE_ONLY;
     *out = nullptr;
     if (n < 2 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: n=%d outside [2,%d]", n, KC_MAX_CANDIDATES);
     if (n_records < 0 || (n_records && (!h_text || !h_off))) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: bad arguments");
@@ -478,7 +496,7 @@ int kc_consolidate_json_packed(const char *h_text, const int64_t *h_off, int64_t
         while (!rc) {
             const int k = next.fetch_add(1);
             if (k >= n_chunks) break;
-            rc = run_chunk(w, h_text, h_off, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res, stages[(size_t)wi]);
+            rc = run_chunk(w, h_text, h_off, h_seq, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res, stages[(size_t)wi]);
         }
         if (rc) {
             cudaStreamSynchronize(w.stream);
@@ -581,6 +599,20 @@ int kc_consolidate_json_packed(const char *h_text, const int64_t *h_off, int64_t
     return KC_OK;
 }
 
+}  // namespace
+
+int kc_consolidate_json_packed(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, double rel_eps, double abs_eps,
+                               int device, int32_t threads, uint32_t flags, kc_json_result **out) {
+    return consolidate_packed(h_text, h_off, nullptr, n_records, n, rel_eps, abs_eps, device, threads, flags, out);
+}
+
+int kc_consolidate_json_packed_weighted(const char *h_text, const int64_t *h_off, const float *h_seq_logprob, int64_t n_records, int32_t n,
+                                        double rel_eps, double abs_eps, int device, int32_t threads, uint32_t flags, kc_json_result **out) {
+    if (n_records > 0 && !h_seq_logprob) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed_weighted: NULL h_seq_logprob");
+    static const float none = 0.0f;
+    return consolidate_packed(h_text, h_off, h_seq_logprob ? h_seq_logprob : &none, n_records, n, rel_eps, abs_eps, device, threads, flags, out);
+}
+
 int kc_json_result_view(kc_json_result *res, const char **text, const int64_t **content_off, const int64_t **content_len,
                         const int64_t **likelihoods_off, const int64_t **likelihoods_len, const uint8_t **status, const uint8_t **why,
                         kc_json_stats *stats) {
@@ -617,6 +649,7 @@ struct kc_debug_jsongpu {
     std::vector<uint8_t> mchars;
     std::vector<int32_t> mstr_off, mgrp_off;
     std::vector<int8_t> vcells;
+    std::vector<int32_t> vrec;
     std::vector<double> xcells;
     std::vector<int64_t> len_c, len_l;
     std::vector<uint8_t> out_c, out_l;
@@ -668,6 +701,7 @@ int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_re
     h->piece_c.assign(std::max<size_t>(T, 1), 0);
     h->piece_l.assign(std::max<size_t>(T, 1), 0);
     h->vcells.assign(std::max<size_t>(T * n, 16), (int8_t)-1);
+    h->vrec.assign(std::max<size_t>(T, 1), -1);
     h->xcells.assign(std::max<size_t>(T * n, 2), 0.0);
     ch.toks = h->toks.data();
     ch.fdesc = h->fdesc.data();
@@ -675,6 +709,7 @@ int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_re
     ch.piece_c = h->piece_c.data();
     ch.piece_l = h->piece_l.data();
     ch.vcells = h->vcells.data();
+    ch.vrec = h->vrec.data();
     ch.xcells = h->xcells.data();
     const int team = team_size(n);
     for (int32_t r = 0; r < R; ++r) {
@@ -735,9 +770,22 @@ int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells
 
 int kc_debug_jsongpu_emit(kc_debug_jsongpu *h, const uint32_t *vote_meta, const double *num_value, const uint32_t *num_meta,
                           const char **content, const int64_t **content_off, const char **likelihoods, const int64_t **likelihoods_off) {
+    return kc_debug_jsongpu_emit_weighted(h, vote_meta, nullptr, num_value, num_meta, content, content_off, likelihoods, likelihoods_off);
+}
+
+int kc_debug_jsongpu_group_records(const kc_debug_jsongpu *h, const int32_t **group_record) {
+    if (!h) return KC_EINVAL;
+    if (group_record) *group_record = h->vrec.data();
+    return KC_OK;
+}
+
+int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_meta, const float *vote_weight, const double *num_value,
+                                   const uint32_t *num_meta, const char **content, const int64_t **content_off, const char **likelihoods,
+                                   const int64_t **likelihoods_off) {
     if (!h) return KC_EINVAL;
     Chunk &ch = h->ch;
     ch.vmeta = vote_meta;
+    ch.vweight = vote_weight;
     ch.xvalue = num_value;
     ch.xmeta = num_meta;
     const int64_t R = h->R;

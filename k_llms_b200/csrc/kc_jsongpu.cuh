@@ -67,7 +67,9 @@ struct Chunk {
     int32_t *mstr_off, *mgrp_off;        //           [strings + 1], [groups + 1]
     const int32_t *midx;                 // K4 results: medoid's index within its group,
     const double *mavg;                  //             its mean similarity
-    const uint32_t *vmeta;   // K1 result words
+    int32_t *vrec;           // [vote groups] or NULL: the (chunk-local) record of each vote group, for K3b over ragged records
+    const float *vweight;    // [vote groups] or NULL: K3b's weights — the vote leaves are likelihood-weighted (DESIGN.md §5)
+    const uint32_t *vmeta;   // K1 (or K3b) result words
     const double *xvalue;    // K2 values
     const uint32_t *xmeta;   // K2 result words
     uint32_t *piece_c, *piece_l;  // [slots] by (slot + rank): piece length, then (after the leader's pass) piece offset
@@ -317,6 +319,8 @@ KC_HD inline void slots_phase(const Chunk &ch, int32_t r) {
     ch.counters[1] += nx;
     ch.counters[2] += nm;
 #endif
+    if (ch.vrec)
+        for (uint32_t k = 0; k < nv; ++k) ch.vrec[ch.vbase[r] + k] = r;
 }
 
 // A2, after the exclusive scans of mcount / scount / ccount: lane j writes its medoid group in K4's CSR form.  Group, string
@@ -464,6 +468,8 @@ KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &cont
     // one call for both kinds keeps one inlined copy (two made write_kernel save convergence barriers); a vote group always
     // reaches the HAS_VALUE arm: a string group has a non-None cell, and a bool group turns None into False
     if (kind == F_VOTE_STR || kind == F_VOTE_BOOL || kind == F_NUMERIC) conf = confidence(m, kind == F_NUMERIC, 1.0);
+    // likelihood-weighted calls: a vote leaf's likelihood is pvf (1 on this path) times K3b's weight share
+    if (ch.vweight && (kind == F_VOTE_STR || kind == F_VOTE_BOOL)) conf = weighted_vote_confidence(1.0, ch.vweight[(int64_t)ch.vbase[r] + g]);
     float_repr(conf, lik);
 }
 

@@ -729,6 +729,45 @@ int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int
     });
 }
 
+int kc_weighted_vote_groups_i8(const int8_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_group_record,
+                               const float *d_seq_logprob, int64_t n_records, int32_t *d_win_code, uint32_t *d_meta, float *d_weight,
+                               void *stream) {
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_weighted_vote_groups_i8: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
+    if (n_groups < 0 || n_records < 0) return kc_fail(KC_EINVAL, "kc_weighted_vote_groups_i8: negative sizes");
+    if (n_groups == 0) return KC_OK;
+    if (!d_codes || !d_group_record || !d_win_code || !d_meta || !d_weight || (n_records > 0 && !d_seq_logprob))
+        return kc_fail(KC_EINVAL, "kc_weighted_vote_groups_i8: NULL buffer");
+    if (!aligned16(d_codes)) return kc_fail(KC_EINVAL, "kc_weighted_vote_groups_i8: d_codes must be 16-byte aligned");
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    // the buckets and row loads of kc_vote_i8: n a power of two from 4 on reads whole rows, any other n the next power of two
+    // with the cells beyond n absent
+    return with_pow2<4>(n, [&](auto np) -> int {
+        constexpr int NP = decltype(np)::value, WROW = kc::kWRowBulk<NP>;
+        float *d_rows = nullptr;
+        if (n_records > 0) {
+            int pre_grid = 0;
+            int rc = stride_grid((n_records + 7) / 8, pre_grid);
+            if (rc) return rc;
+            KC_CUDA_I(cudaMallocAsync(reinterpret_cast<void **>(&d_rows), (size_t)n_records * WROW * 4, st));
+            kc::weight_rows_n_kernel<NP><<<pre_grid, 256, 0, st>>>(d_seq_logprob, n_records, n, d_rows);
+            if (cudaGetLastError() != cudaSuccess) {
+                cudaFreeAsync(d_rows, st);
+                return kc_fail(KC_ECUDA, "kc_weighted_vote_groups_i8: weight_rows_kernel launch failed");
+            }
+        }
+        const int threads = 128;
+        int grid = 0;
+        int rc = stride_grid((n_groups + threads - 1) / threads, grid);
+        if (!rc) {
+            auto kernel = n == NP ? kc::weighted_vote_groups_kernel<NP, true> : kc::weighted_vote_groups_kernel<NP, false>;
+            kernel<<<grid, threads, 0, st>>>(d_codes, n_groups, n, d_group_record, n_records, d_rows, d_win_code, d_meta, d_weight);
+            if (cudaGetLastError() != cudaSuccess) rc = kc_fail(KC_ECUDA, "kc_weighted_vote_groups_i8: launch failed");
+        }
+        if (d_rows) cudaFreeAsync(d_rows, st);
+        return rc;
+    });
+}
+
 int kc_medoid_str(const uint8_t *d_chars, const int32_t *d_str_off, const int32_t *d_grp_off, int64_t n_groups,
                   int32_t max_group, int32_t *d_best_idx, double *d_best_avg, void *stream) {
     return kc_medoid_str_method(d_chars, d_str_off, d_grp_off, n_groups, max_group, KC_SIM_LEVENSHTEIN, d_best_idx, d_best_avg, stream);

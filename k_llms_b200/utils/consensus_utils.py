@@ -56,11 +56,24 @@ def _host_primitive(settings: ConsensusSettings):
     return run
 
 
-def _plan_for(n: int, settings: ConsensusSettings, numeric_branch: bool = True) -> columnar.Plan:
+def _plan_for(n: int, settings: ConsensusSettings, numeric_branch: bool = True, weighted: bool = False) -> columnar.Plan:
     plan = columnar.Plan(n, settings.allow_none_as_candidate, settings.rel_eps, settings.abs_eps, _host_primitive(settings),
-                         numeric_branch=numeric_branch)
+                         numeric_branch=numeric_branch, weighted=weighted)
     plan.string_method = settings.string_similarity_method if settings.string_consensus_method == "centroid" else "host"
     return plan
+
+
+def _record_sums(seq: Sequence[float], n_values: int, where: str) -> List[float]:
+    """The sequence logprobs of one record's candidates, checked: one number per candidate, finite as float32 (extra entries of
+    a padded row are ignored)."""
+    import numpy as np
+    if len(seq) < n_values:
+        raise ValueError(f"{where}: {len(seq)} sequence logprobs for {n_values} candidates")
+    with np.errstate(over="ignore"):  # a sum beyond the float32 range becomes inf and is refused below
+        out = np.asarray([float(s) for s in list(seq)[:n_values]], dtype=np.float64).astype(np.float32)
+    if not np.isfinite(out).all():  # checked as the kernel sees them: float32
+        raise ValueError(f"{where}: sequence logprobs must be finite as float32, got {list(seq)[:n_values]}")
+    return [float(s) for s in out]
 
 
 def consensus_values(
@@ -70,9 +83,15 @@ def consensus_values(
     client: Any,
     parent_valid_frac: float = 1.0,
     _numeric_branch: bool = True,
+    seq_logprobs: Optional[Sequence[float]] = None,
 ) -> Tuple[Any, Any]:
-    """(consensus value, confidence) for one record's n candidate values — cu:1376-1454."""
-    plan = _plan_for(len(values), consensus_settings, _numeric_branch)
+    """(consensus value, confidence) for one record's n candidate values — cu:1376-1454.  seq_logprobs (n floats, the
+    candidates' summed token logprobs): the vote leaves are likelihood-weighted (DESIGN.md §5)."""
+    weighted = seq_logprobs is not None
+    sums = _record_sums(seq_logprobs, len(values), "consensus_values") if weighted else None
+    plan = _plan_for(len(values), consensus_settings, _numeric_branch, weighted)
+    if weighted:
+        plan.begin_record(sums)
     root = plan.add(values, parent_valid_frac, sync_get_openai_embeddings_from_text)
     res = plan.run() if (plan.vote_rows or plan.num_rows or plan.medoid_groups) else {}
     return plan.materialise(root, res)
@@ -84,12 +103,26 @@ def consensus_values_batch(
     sync_get_openai_embeddings_from_text: Optional[SYNC_GET_OPENAI_EMBEDDINGS_FROM_TEXT_TYPE] = None,
     client: Any = None,
     parent_valid_frac: float = 1.0,
+    seq_logprobs: Optional[Any] = None,
 ) -> List[Tuple[Any, Any]]:
-    """Batched entry (new): consensus_values for many independent records with ONE K1 and ONE K2 launch."""
+    """Batched entry (new): consensus_values for many independent records with ONE K1 and ONE K2 launch.
+
+    seq_logprobs: float32 [R][n] (n >= every record's candidate count; row r's first len(records[r]) entries are record r's
+    candidate sums, e.g. from K3): the vote leaves are likelihood-weighted (DESIGN.md §5), with ONE K3b launch for the batch."""
     settings = consensus_settings or ConsensusSettings()
     embed = sync_get_openai_embeddings_from_text if sync_get_openai_embeddings_from_text is not None else _no_embeddings
-    plan = _plan_for(max((len(r) for r in records), default=1), settings)
-    roots = [plan.add(values, parent_valid_frac, embed) for values in records]
+    weighted = seq_logprobs is not None
+    if weighted:
+        if len(seq_logprobs) != len(records):
+            raise ValueError(f"consensus_values_batch: {len(seq_logprobs)} rows of sequence logprobs for {len(records)} records")
+        sums = [_record_sums(s, len(values), f"consensus_values_batch, record {r}")
+                for r, (values, s) in enumerate(zip(records, seq_logprobs))]
+    plan = _plan_for(max((len(r) for r in records), default=1), settings, weighted=weighted)
+    roots = []
+    for r, values in enumerate(records):
+        if weighted:
+            plan.begin_record(sums[r])
+        roots.append(plan.add(values, parent_valid_frac, embed))
     res = plan.run() if (plan.vote_rows or plan.num_rows or plan.medoid_groups) else {}
     return [plan.materialise(root, res) for root in roots]
 
@@ -104,11 +137,12 @@ async def async_consensus_values(
     async_get_openai_embeddings_from_text: ASYNC_GET_OPENAI_EMBEDDINGS_FROM_TEXT_TYPE,
     client: Any,
     parent_valid_frac: float = 1.0,
+    seq_logprobs: Optional[Sequence[float]] = None,
 ) -> Tuple[Any, Any]:
     """Async twin (cu:1779-1860).  The reference's async primitive has NO numeric clustering (cu:1638-1688, SURVEY.md §0.5):
     a non-unanimous numeric field takes the similarity medoid — [10, 10, 11] gives (10, 0.5) here and (10.0, 0.66667) in the
     sync path.  That difference is part of the reference's behaviour and is reproduced; votes still run on the GPU, off the
-    event loop."""
+    event loop.  seq_logprobs: as for consensus_values."""
     loop = asyncio.get_running_loop()
 
     def embed(texts):
@@ -117,7 +151,7 @@ async def async_consensus_values(
 
     return await asyncio.to_thread(consensus_values, values, consensus_settings,
                                    embed if async_get_openai_embeddings_from_text is not None else None, client,
-                                   parent_valid_frac, False)
+                                   parent_valid_frac, False, seq_logprobs)
 
 
 # ----------------------------------------------------------------------------- alignment pre-pass
