@@ -309,9 +309,11 @@ int kc_align_json_batch(const char *const *texts, const int64_t *lens, int64_t n
                         int32_t threads, char **out_texts, int32_t *out_status, int64_t *out_counts);
 /* test hooks of H2: generic_similarity (consensus_utils.py:892-917) of two JSON values; scipy.optimize.linear_sum_assignment;
  * the similarity pass of kc_align_json_batch on the host for one list of T JSON elements (out: T x T, NaN = left to the host;
- * returns the pairs i < j it decided) */
+ * returns the pairs i < j it decided); the same pass for n_nodes lists in one call (node g = the next node_len[g] texts, its
+ * matrix after node g-1's in out) on `device`, or on the host (device < 0) with each node's pairs split over `lanes` lanes */
 int kc_debug_similarity_json(const char *a, const char *b, double *out);
 int kc_debug_alignsim(const char *const *texts, int32_t T, double *out);
+int kc_debug_alignsim_nodes(const char *const *texts, const int32_t *node_len, int32_t n_nodes, int32_t lanes, int device, double *out);
 int kc_debug_lsap(int32_t nr, int32_t nc, const double *cost, int32_t *row_ind, int32_t *col_ind);
 
 /*
@@ -397,6 +399,9 @@ int kc_debug_jsongpu_set_medoid(kc_debug_jsongpu *h, const int32_t *medoid_idx, 
 void kc_debug_jsongpu_free(kc_debug_jsongpu *h);
 int kc_debug_parse_doubles(const char *text, const int64_t *off, int64_t count, double *out, uint8_t *ok);
 int kc_debug_float_reprs(const double *xs, int64_t count, char *out /* [count][32] */, int32_t *lens);
+/* the same two conversions run on `device`, one thread per value (host buffers in and out) */
+int kc_debug_parse_doubles_device(const char *text, const int64_t *off, int64_t count, double *out, uint8_t *ok, int device);
+int kc_debug_float_reprs_device(const double *xs, int64_t count, char *out /* [count][32] */, int32_t *lens, int device);
 int kc_debug_round5(const double *xs, int64_t count, double *out);
 /* Bench / test input: n_records records of schema S32 (SURVEY.md §8d) as candidate texts, exactly as json.dumps prints them.
  * Call with out == NULL to get the offsets (off[n_records*n] = bytes needed), then with a buffer of that size. */

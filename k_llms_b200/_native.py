@@ -71,6 +71,7 @@ _SIGNATURES = {
     "kc_debug_similarity_json": (_int, [_str, _str, ctypes.POINTER(_f64)]),
     "kc_debug_lsap": (_int, [_i32, _i32, _vp, _vp, _vp]),
     "kc_debug_alignsim": (_int, [_vp, _i32, _vp]),
+    "kc_debug_alignsim_nodes": (_int, [_vp, _vp, _i32, _i32, _int, _vp]),
     "kc_debug_jsongpu_plan": (_int, [_vp, _vp, _i64, _i32, _pp]),
     "kc_debug_jsongpu_inputs": (_int, [_vp] * 6),
     "kc_debug_jsongpu_emit": (_int, [_vp, _vp, _vp, _vp] + [_pp] * 4),
@@ -81,6 +82,8 @@ _SIGNATURES = {
     "kc_debug_jsongpu_free": (None, [_vp]),
     "kc_debug_parse_doubles": (_int, [_vp, _vp, _i64, _vp, _vp]),
     "kc_debug_float_reprs": (_int, [_vp, _i64, _vp, _vp]),
+    "kc_debug_parse_doubles_device": (_int, [_vp, _vp, _i64, _vp, _vp, _int]),
+    "kc_debug_float_reprs_device": (_int, [_vp, _i64, _vp, _vp, _int]),
     "kc_debug_round5": (_int, [_vp, _i64, _vp]),
     "kc_debug_s32_texts": (_int, [_u64, _i64, _i32, _i32, _vp, _i64, _vp]),
 }

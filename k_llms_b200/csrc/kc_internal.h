@@ -142,11 +142,12 @@ struct KcAsNode {
 };
 
 // Similarity matrices of the nodes into h_out (host memory; NaN where the phase does not model the pair, and on the
-// diagonal).  device >= 0: one kernel launch on that device; device < 0: the same phase instantiated on the host.
+// diagonal).  device >= 0: one kernel launch on that device; device < 0: the same phase instantiated on the host, each node's
+// pairs split over `host_lanes` lanes run one after another (1 in the product; 32 walks the pairs as a warp does).
 // *pairs (optional) = element pairs a < b the phase decided.
 extern "C" __attribute__((visibility("hidden"))) int kc_alignsim(const KcAsNode *nodes, int64_t n_nodes, const KcAsVal *vals, int64_t n_vals,
                                                                  const uint8_t *chars, int64_t n_chars, double *h_out, int64_t n_out,
-                                                                 int device, int64_t *pairs);
+                                                                 int device, int host_lanes, int64_t *pairs);
 
 #define KC_CUDA_I(call)                                                                                               \
     do {                                                                                                              \

@@ -1298,24 +1298,34 @@ int kc_align_json_batch(const char *const *texts, const int64_t *lens, int64_t n
 // The similarity phase of kc_align_json_batch instantiated on the host for one node whose T elements are given as JSON
 // texts: out[i * T + j] as kc_alignsim computes it (NaN where it leaves the pair to the host).  Test hook.  Returns the
 // number of pairs i < j it decided, KC_EINVAL on invalid / non-ASCII JSON or T outside [2, 512].
-int kc_debug_alignsim(const char *const *texts, int32_t T, double *out) {
-    if (!texts || !out || T < 2 || T > 512) return KC_EINVAL;
+int kc_debug_alignsim(const char *const *texts, int32_t T, double *out) { return kc_debug_alignsim_nodes(texts, &T, 1, 1, -1, out); }
+
+// The same for n_nodes list nodes in one kc_alignsim pass: node g holds the next node_len[g] texts, its T x T matrix follows
+// the previous node's in out.  device >= 0 launches the kernel; device < 0 runs the phase on the host with `lanes` lanes.
+int kc_debug_alignsim_nodes(const char *const *texts, const int32_t *node_len, int32_t n_nodes, int32_t lanes, int device, double *out) {
+    if (!texts || !node_len || !out || n_nodes < 1 || lanes < 1) return KC_EINVAL;
     AlignCtx cx;
-    const int32_t list = cx.tr.add(A_LIST);
-    for (int32_t k = 0; k < T; ++k) {
-        Scanner sc{texts[k], texts[k] + strlen(texts[k])};
-        int32_t id;
-        if (!aparse(sc, cx.tr, id, 0) || sc.non_ascii) return KC_EINVAL;
-        sc.ws();
-        if (sc.p != sc.end) return KC_EINVAL;
-        cx.tr.v[(size_t)list].items.push_back(id);
+    int64_t k = 0;
+    for (int32_t g = 0; g < n_nodes; ++g) {
+        const int32_t T = node_len[g];
+        if (T < 2 || T > 512) return KC_EINVAL;
+        const int32_t list = cx.tr.add(A_LIST);
+        for (int32_t i = 0; i < T; ++i, ++k) {
+            Scanner sc{texts[k], texts[k] + strlen(texts[k])};
+            int32_t id;
+            if (!aparse(sc, cx.tr, id, 0) || sc.non_ascii) return KC_EINVAL;
+            sc.ws();
+            if (sc.p != sc.end) return KC_EINVAL;
+            cx.tr.v[(size_t)list].items.push_back(id);
+        }
+        sim_add_node(cx, std::vector<int32_t>{list}, cx.sims);
     }
-    sim_add_node(cx, std::vector<int32_t>{list}, cx.sims);
     int64_t pairs = 0;
     const SimTable &t = cx.sims;
     const int rc = kc_alignsim(t.nodes.data(), (int64_t)t.nodes.size(), t.vals.data(), (int64_t)t.vals.size(),
-                               reinterpret_cast<const uint8_t *>(t.chars.data()), (int64_t)t.chars.size(), out, t.out_len, -1, &pairs);
-    return rc ? rc : (int)pairs;
+                               reinterpret_cast<const uint8_t *>(t.chars.data()), (int64_t)t.chars.size(), out, t.out_len, device, lanes, &pairs);
+    if (rc) return rc;
+    return pairs > INT32_MAX ? kc_fail(KC_EINVAL, "kc_debug_alignsim_nodes: more than 2^31 pairs") : (int)pairs;
 }
 
 // generic_similarity (consensus_utils.py:892-917, default string method) of two JSON values; test hook of the native alignment.

@@ -846,6 +846,90 @@ int kc_debug_round5(const double *xs, int64_t count, double *out) {
 
 }  // extern "C"
 
+// ---------------------------------------------------------------- the number conversions' device instantiation (test hooks)
+
+namespace {
+
+__global__ void parse_doubles_kernel(const uint8_t *__restrict__ text, const int64_t *__restrict__ off, int64_t count, double *__restrict__ out,
+                                     uint8_t *__restrict__ ok) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
+        double v = 0.0;
+        ok[i] = kc::js::to_double(text + off[i], (uint32_t)(off[i + 1] - off[i]), v) ? 1 : 0;
+        out[i] = v;
+    }
+}
+
+__global__ void float_reprs_kernel(const double *__restrict__ xs, int64_t count, uint8_t *__restrict__ out, int32_t *__restrict__ lens) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < count; i += (int64_t)gridDim.x * blockDim.x) {
+        kc::js::Sink s{out + i * 32, 0};
+        kc::js::float_repr(xs[i], s);
+        lens[i] = (int32_t)s.n;
+    }
+}
+
+// One device allocation cut into `n` buffers of bytes[i] (each 256-byte aligned), freed on scope exit.
+struct DebugDev {
+    uint8_t *base = nullptr;
+    ~DebugDev() {
+        if (base) cudaFree(base);
+    }
+    int alloc(const size_t *bytes, uint8_t **ptrs, int n, const char *who) {
+        size_t total = 0;
+        for (int i = 0; i < n; ++i) total += (bytes[i] + 255) & ~size_t(255);
+        if (cudaMalloc(&base, total ? total : 256) != cudaSuccess) {
+            cudaGetLastError();
+            base = nullptr;
+            return kc_fail(KC_ENOMEM, "%s: cudaMalloc(%zu) failed", who, total);
+        }
+        size_t o = 0;
+        for (int i = 0; i < n; o += (bytes[i] + 255) & ~size_t(255), ++i) ptrs[i] = base + o;
+        return KC_OK;
+    }
+};
+
+constexpr int kDebugBlock = 256, kDebugGrid = 264;  // a grid stride of 67,584 threads: large batches loop
+
+}  // namespace
+
+extern "C" {
+
+// kc_debug_parse_doubles / kc_debug_float_reprs with the conversions run on `device`, one thread per value
+int kc_debug_parse_doubles_device(const char *text, const int64_t *off, int64_t count, double *out, uint8_t *ok, int device) {
+    if (!text || !off || !out || !ok || count < 0) return KC_EINVAL;
+    if (count == 0) return KC_OK;
+    KC_CUDA_I(cudaSetDevice(device));
+    const size_t n_text = (size_t)off[count];
+    const size_t bytes[4] = {n_text, ((size_t)count + 1) * 8, (size_t)count * 8, (size_t)count};
+    uint8_t *d[4];
+    DebugDev mem;
+    if (const int rc = mem.alloc(bytes, d, 4, "kc_debug_parse_doubles_device")) return rc;
+    if (n_text) KC_CUDA_I(cudaMemcpy(d[0], text, n_text, cudaMemcpyHostToDevice));
+    KC_CUDA_I(cudaMemcpy(d[1], off, bytes[1], cudaMemcpyHostToDevice));
+    parse_doubles_kernel<<<kDebugGrid, kDebugBlock>>>(d[0], reinterpret_cast<const int64_t *>(d[1]), count, reinterpret_cast<double *>(d[2]), d[3]);
+    KC_CUDA_I(cudaGetLastError());
+    KC_CUDA_I(cudaMemcpy(out, d[2], bytes[2], cudaMemcpyDeviceToHost));
+    KC_CUDA_I(cudaMemcpy(ok, d[3], bytes[3], cudaMemcpyDeviceToHost));
+    return KC_OK;
+}
+
+int kc_debug_float_reprs_device(const double *xs, int64_t count, char *out /* [count][32] */, int32_t *lens, int device) {
+    if (!xs || !out || !lens || count < 0) return KC_EINVAL;
+    if (count == 0) return KC_OK;
+    KC_CUDA_I(cudaSetDevice(device));
+    const size_t bytes[3] = {(size_t)count * 8, (size_t)count * 32, (size_t)count * 4};
+    uint8_t *d[3];
+    DebugDev mem;
+    if (const int rc = mem.alloc(bytes, d, 3, "kc_debug_float_reprs_device")) return rc;
+    KC_CUDA_I(cudaMemcpy(d[0], xs, bytes[0], cudaMemcpyHostToDevice));
+    float_reprs_kernel<<<kDebugGrid, kDebugBlock>>>(reinterpret_cast<const double *>(d[0]), count, d[1], reinterpret_cast<int32_t *>(d[2]));
+    KC_CUDA_I(cudaGetLastError());
+    KC_CUDA_I(cudaMemcpy(out, d[1], bytes[1], cudaMemcpyDeviceToHost));
+    KC_CUDA_I(cudaMemcpy(lens, d[2], bytes[2], cudaMemcpyDeviceToHost));
+    return KC_OK;
+}
+
+}  // extern "C"
+
 // ---------------------------------------------------------------- bench / test input: schema S32 as candidate texts
 
 namespace {

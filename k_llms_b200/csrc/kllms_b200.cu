@@ -831,17 +831,19 @@ int kc_medoid_str_host(const uint8_t *h_chars, int64_t n_chars, const int32_t *h
 }
 
 // Element similarities of the list-alignment pre-pass (kc_alignsim.cuh): H2D of the value table, one launch, D2H of the
-// matrices (synchronous); device < 0 runs the same phase on the calling host thread.
+// matrices (synchronous); device < 0 runs the same phase on the calling host thread, lane 0 .. host_lanes - 1 of each node in turn.
 int kc_alignsim(const KcAsNode *nodes, int64_t n_nodes, const KcAsVal *vals, int64_t n_vals, const uint8_t *chars, int64_t n_chars,
-                double *h_out, int64_t n_out, int device, int64_t *pairs) {
+                double *h_out, int64_t n_out, int device, int host_lanes, int64_t *pairs) {
     if (pairs) *pairs = 0;
     if (n_nodes < 0 || n_vals < 0 || n_chars < 0 || n_out < 0) return kc_fail(KC_EINVAL, "kc_alignsim: negative size");
+    if (device < 0 && host_lanes < 1) return kc_fail(KC_EINVAL, "kc_alignsim: host_lanes < 1");
     if (n_nodes == 0) return KC_OK;
     if (!nodes || !vals || !h_out || (n_chars && !chars)) return kc_fail(KC_EINVAL, "kc_alignsim: NULL buffer");
     if (device < 0) {
         uint64_t tab[kc::kPeqStride];
         int64_t decided = 0;
-        for (int64_t g = 0; g < n_nodes; ++g) decided += kc::alignsim_node(nodes[g], vals, chars, h_out, 0, 1, tab);
+        for (int64_t g = 0; g < n_nodes; ++g)
+            for (int lane = 0; lane < host_lanes; ++lane) decided += kc::alignsim_node(nodes[g], vals, chars, h_out, lane, host_lanes, tab);
         if (pairs) *pairs = decided;
         return KC_OK;
     }

@@ -29,6 +29,104 @@ def element_pool(rng):
     return pool
 
 
+def edge_pairs():
+    """Pairs on the boundaries the pass models: isclose at 1 % and one ulp past, big ints, 50 / 51 raw characters, 64 / 65
+    normalised characters, empty normalised forms, falsy values, dict keys."""
+    cases = []
+    for base in (1.0, 100.0, 3.7, -2.5, 1e10, 7e-300):
+        edge = base + abs(base) * 0.01
+        cases += [(base, edge), (base, math.nextafter(edge, math.inf)), (base, math.nextafter(edge, -math.inf))]
+        edge = base - abs(base) * 0.01
+        cases += [(base, edge), (base, math.nextafter(edge, math.inf)), (base, math.nextafter(edge, -math.inf))]
+    cases += [(100, 101), (100, 102), (100, 101.0), (100, 101.00000000001), (True, 1), (True, 1.0), (False, 0), (True, False),
+              (10 ** 20, 10 ** 20), (10 ** 20, 10 ** 20 + 1), (10 ** 30, 10 ** 31), (-(10 ** 25), -(10 ** 25)), (2 ** 63, 2 ** 63 - 1),
+              (0, 0.0), (0, ""), (0.0, False), ("", None), (None, {}), ({}, []), (None, []), (0, None), (None, None), (1, None),
+              ("a" * 50, "b" * 50), ("a" * 51, "b" * 50), ("a" * 51, "b" * 51), ("a" * 51, "a" * 51),
+              ("x" * 64, "y" * 70), ("x" * 65, "y" * 70), ("x" * 64 + "!", "x" * 64), ("!!!", "?"), ("!!!", "abc"), ("", "abc"),
+              ("Hello, World", "hello world"), ("abc", 1), ("abc", {"a": 1}), ({"a": 1}, 1),
+              ({"a": 1, "b": "x"}, {"c": 2, "d": "y"}), ({"a": 1, "b": "x"}, {"b": "x", "c": 2}), ({"a": 1, "reasoning___a": "z"}, {"a": 1}),
+              ({"reasoning___a": "z"}, {}), ({"source___b": [1]}, {"source___b": 2}), ({"a": [1]}, {"a": [1]}), ({"a": {"b": 1}}, {"a": 1}),
+              ({"a": "a" * 60}, {"a": "b" * 60}), ({"a": None}, {"b": None}), ({"a": 1.0}, {"a": True}), ([1], [1]), ([], [])]
+    return cases
+
+
+NODE_SIZES = (2, 3, 31, 32, 33, 63, 64, 65, 200, 511, 512)
+
+
+def node_sets(rng):
+    """List nodes for the batched pass (kc_debug_alignsim_nodes), shuffled: every size of NODE_SIZES (one lane's pair, a warp's
+    pairs exactly, one more, several rows per step, the 512 limit), thousands of small nodes so that every warp of the grid takes
+    several, and the edge pairs as nodes of two.  Returns (pool of distinct elements, [pool indices of each node's elements])."""
+    pool = element_pool(rng)
+    for a, b in edge_pairs():
+        pool += [a, b]
+    texts, uniq = set(), []
+    for e in pool:  # one pool entry per JSON text
+        t = json.dumps(e)
+        if t not in texts:
+            texts.add(t)
+            uniq.append(e)
+    index = {json.dumps(e): i for i, e in enumerate(uniq)}
+    counts = {2: 2500, 3: 2500, 31: 1000, 32: 1000, 33: 1000, 63: 100, 64: 100, 65: 100, 200: 10, 511: 3, 512: 3}
+    nodes = [[rng.randrange(len(uniq)) for _ in range(T)] for T in NODE_SIZES for _ in range(counts[T])]
+    nodes += [[index[json.dumps(a)], index[json.dumps(b)]] for a, b in edge_pairs()]
+    rng.shuffle(nodes)
+    return uniq, nodes
+
+
+def run_nodes(pool, nodes, lanes=1, device=-1):
+    """kc_debug_alignsim_nodes over `nodes` (pool indices) -> (pairs decided, every node's matrix back to back, float64)."""
+    import ctypes
+
+    import numpy as np
+    from k_llms_b200 import _native as K
+    enc = [json.dumps(e).encode() for e in pool]
+    flat = [enc[i] for nd in nodes for i in nd]
+    texts = (ctypes.c_char_p * len(flat))(*flat)
+    lens = np.array([len(nd) for nd in nodes], dtype=np.int32)
+    # a NaN payload the pass never writes: a cell the host phase skips keeps it
+    out = np.full(int((lens.astype(np.int64) ** 2).sum()), 0x7FF4DEAD0000BEEF, dtype=np.uint64).view(np.float64)
+    rc = K.load().kc_debug_alignsim_nodes(ctypes.cast(texts, ctypes.c_void_p), lens.ctypes.data, len(nodes), lanes, device, out.ctypes.data)
+    if rc < 0:
+        K.check(rc)
+    return rc, out
+
+
+def expected_matrices(pool, nodes):
+    """What the pass must write for `nodes`: generic_similarity (kc_debug_similarity_json) where it models the pair, NaN
+    elsewhere and on the diagonal, every node's matrix back to back; and the number of modelled pairs a < b."""
+    import ctypes
+
+    import numpy as np
+    from k_llms_b200 import _native as K
+    from tests.test_alignsim_host_logic import models
+    lib = K.load()
+    enc = [json.dumps(e).encode() for e in pool]
+    S = np.full((len(pool), len(pool)), np.nan)
+    v = ctypes.c_double()
+    for i in range(len(pool)):
+        for j in range(len(pool)):
+            if models(pool[i], pool[j]):
+                assert lib.kc_debug_similarity_json(enc[i], enc[j], ctypes.byref(v)) == 0
+                S[i, j] = v.value
+    parts, modelled = [], 0
+    for nd in nodes:
+        idx = np.asarray(nd)
+        E = S[np.ix_(idx, idx)]
+        np.fill_diagonal(E, np.nan)
+        parts.append(E.reshape(-1))
+        modelled += int(np.count_nonzero(~np.isnan(E[np.triu_indices(len(nd), 1)])))
+    return np.concatenate(parts), modelled
+
+
+def assert_matrices(got, exp):
+    """NaN exactly where exp has NaN, the same bits everywhere else."""
+    import numpy as np
+    nan = np.isnan(exp)
+    bad = np.nonzero((np.isnan(got) != nan) | (~nan & (got.view(np.uint64) != exp.view(np.uint64))))[0]
+    assert len(bad) == 0, (len(bad), bad[:10], got[bad[:10]], exp[bad[:10]])
+
+
 def _perturb(rng, v):
     if isinstance(v, dict):
         return {k: _perturb(rng, x) for k, x in v.items() if rng.random() > 0.05}

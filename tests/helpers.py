@@ -106,6 +106,148 @@ def raising_embeddings(texts):
     raise RuntimeError("no network in tests")
 
 
+# ----------------------------------------------------------------------------- exact number conversions (kc_jsoncore.cuh)
+
+def number_texts():
+    """JSON number texts for to_double: random floats, 19-digit ints, fixed and exponent notation, a few known hard cases."""
+    import random
+    rng = random.Random(5)
+    texts = [repr(rng.random() * 1e4 + 1) for _ in range(20000)]
+    texts += [str(rng.randrange(-10 ** 19, 10 ** 19)) for _ in range(20000)]
+    texts += ["%.*f" % (rng.randrange(0, 12), rng.random() * 10 ** rng.randrange(-3, 9)) for _ in range(20000)]
+    texts += ["%.*e" % (rng.randrange(0, 18), rng.random() * 10.0 ** rng.randrange(-25, 25)) for _ in range(20000)]
+    texts += ["0.0", "-0.0", "1e0", "1E+5", "1e-5", "1234567890123456789", "0.30000000000000004", "9007199254740993", "4.35", "1e19",
+              "5e-20", "0.5000000000000000000000000", "9.999999999999999e22", "1e22"]
+    return texts
+
+
+def near_halfway_texts(seed=17, count=12000):
+    """Decimal texts on both sides of rounding decisions: for random doubles d in the range to_double takes, the exact midpoint
+    m of d and nextafter(d, inf) printed to 17, 18 and 19 significant digits, rounded down and up, and m itself where it has
+    at most 19 significant digits (every d in [2^50, 10^19) gives one: exact ties, decided to even).  Both signs."""
+    import decimal
+    import random
+    rng = random.Random(seed)
+    ds = []
+    for _ in range(count):
+        r = rng.random()
+        if r < 0.5:       # any magnitude the 19-digit long division reaches
+            d = rng.uniform(1.0, 10.0) * 10.0 ** rng.randrange(-3, 38)
+        elif r < 0.8:     # integers above 2^53: the midpoint is an odd integer or ends in .5 / .25 / .125
+            d = float(rng.randrange(2 ** 50, 10 ** 19))
+        else:             # the Clinger range: short mantissas, |exponent| <= 22
+            d = rng.uniform(1.0, 10.0) * 10.0 ** rng.randrange(-22, 16)
+        ds.append(d)
+    texts = []
+    with decimal.localcontext() as ctx:
+        ctx.prec = 1000
+        for d in ds:
+            mid = (decimal.Decimal(d) + decimal.Decimal(math.nextafter(d, math.inf))) / 2
+            sign = "-" if rng.random() < 0.2 else ""
+            if len(mid.normalize().as_tuple().digits) <= 19:
+                texts.append(sign + str(mid.normalize()))
+            for prec in (17, 18, 19):
+                for rounding in (decimal.ROUND_FLOOR, decimal.ROUND_CEILING):
+                    c = decimal.Context(prec=prec, rounding=rounding)
+                    texts.append(sign + str(c.plus(mid)))
+    return texts
+
+
+def boundary_texts():
+    """(texts, must_decline): powers of ten 1e-22 .. 1e19 in several spellings, mantissas at 2^53 and 2^53 + 1, 19- and
+    20-significant-digit texts (the latter declined), leading-zero fractions, signed zeros."""
+    texts, decline = [], []
+    for k in range(-22, 20):
+        texts += ["1e%d" % k, "1E%+d" % k, "10e%d" % (k - 1), "%se%d" % ("1" + "0" * 5, k - 5)]
+        if k < 0:
+            texts.append("0." + "0" * (-k - 1) + "1")
+        else:
+            texts.append("1" + "0" * k)
+    for w in (2 ** 53 - 1, 2 ** 53, 2 ** 53 + 1, 2 ** 53 + 2, 2 ** 54 - 1, 2 ** 54 + 1, 10 ** 19 - 1):
+        for e in (-22, -20, -19, -18, -10, -1, 0, 1, 5, 19):
+            texts.append("%de%d" % (w, e))
+    nineteen = ["1234567890123456789", "9999999999999999999", "1000000000000000001", "9223372036854775807", "9223372036854775808",
+                "18446744073709551615"[:19]]
+    for m in nineteen:
+        texts += [m, m[:1] + "." + m[1:], "0." + m, m + "e19", m + "e-19", m[:10] + "." + m[10:] + "e-5", m + "0", m + ".000"]
+        decline += [m + "1", m[:1] + "." + m[1:] + "7", "0." + m + "3", m + "5e-3", m[:12] + "." + m[12:] + "9"]
+    texts += ["0." + "0" * 21 + "1", "0." + "0" * 21 + "12345", "0.0000000000000000000001", "-0.0000000000000000000001", "-0", "-0.0",
+              "0e5", "0E-5", "-0e0", "0.000", "0.5", "-1.5e-22", "9.999999999999999999", "1.0000000000000000000"]
+    decline += ["0." + "0" * 22 + "1", "1e20", "1e-23", "12345678901234567891", "1.2345678901234567891"]
+    return texts, decline
+
+
+def repr_doubles():
+    """float64 values for float.__repr__: random in every range, random bit patterns, every power of two and of ten,
+    subnormals, the extremes, inf and NaN."""
+    rng = np.random.default_rng(1)
+    bits = rng.integers(0, 2 ** 63, 40000, dtype=np.uint64).view(np.float64)
+    xs = np.concatenate([rng.random(40000) * 1e4 + 1, np.floor(rng.random(20000) * 1e6), bits[np.isfinite(bits)], -bits[:500],
+                         rng.random(40000) * 10.0 ** rng.integers(-30, 30, 40000), np.round(rng.random(20000), 5),
+                         [2.0 ** k for k in range(-1074, 1024)], [10.0 ** k for k in range(-323, 309)],
+                         [0.0, -0.0, 1.0, 1e16, 1e15, 123456789012345680.0, 1e-5, 1e-4, 5e-324, 1.7976931348623157e308,
+                          2.2250738585072014e-308, 1e22, 1e23, float("inf"), float("-inf"), float("nan")]])
+    return np.ascontiguousarray(xs)
+
+
+def pack_number_texts(texts):
+    """texts -> (blob uint8, off int64 [len + 1]) for kc_debug_parse_doubles(_device)."""
+    enc = [t.encode() for t in texts]
+    off = np.zeros(len(enc) + 1, dtype=np.int64)
+    np.cumsum([len(b) for b in enc], out=off[1:])
+    blob = np.frombuffer(b"".join(enc) or b"\0", dtype=np.uint8).copy()
+    return blob, off
+
+
+def cpython_doubles(texts):
+    """float(t) for every JSON number text (CPython's correctly rounded conversion), as a float64 array.  This is
+    float(json.loads(t)) except for "-0", which json.loads reads as the int 0: to_double keeps the sign, and the JSON paths
+    carry the int-ness of the text apart from the value."""
+    assert all(isinstance(json.loads(t), (int, float)) for t in texts)
+    return np.array([float(t) for t in texts], dtype=np.float64)
+
+
+# ----------------------------------------------------------------------------- mutated candidate texts
+
+MUTATE_ALPHABET = '{}[]",:0123456789.eE-+ntf \n\t\\u00e9abcxyzNI'
+
+
+def mutate(rng, text):
+    """One or two random character substitutions, deletions or insertions (JSON punctuation, digits, escapes, letters)."""
+    chars = list(text)
+    for _ in range(rng.randrange(1, 3)):
+        i, r = rng.randrange(len(chars)), rng.random()
+        if r < 0.4:
+            chars[i] = rng.choice(MUTATE_ALPHABET)
+        elif r < 0.7:
+            del chars[i]
+        else:
+            chars.insert(i, rng.choice(MUTATE_ALPHABET))
+    return "".join(chars)
+
+
+def general_and_mutated_records(seed=11):
+    """{n: records}: general flat records with phrases, big ints and missing keys, nested records, and flat records with about
+    half their candidate texts mutated (most of those are invalid JSON or change a value's type)."""
+    import random
+    from tests.test_gpu_json import _random_nested_record, _random_record
+    from tests.test_jsongpu_host_logic import _flat_record
+    rng = random.Random(seed)
+    by_n = {}
+    for _ in range(600):
+        n = rng.choice([2, 3, 5, 8, 16])
+        by_n.setdefault(n, []).append(_random_record(rng, n))
+    for _ in range(200):
+        n = rng.choice([2, 3, 5])
+        by_n.setdefault(n, []).append(_random_nested_record(rng, n))
+    for _ in range(800):
+        n = rng.choice([2, 3, 5])
+        texts = [mutate(rng, t) if rng.random() < 0.5 else t for t in _flat_record(rng, n)]
+        if all(texts):
+            by_n.setdefault(n, []).append(texts)
+    return by_n
+
+
 def oracle_run(plan):
     """Stand-in for Plan.run(): evaluate the recorded groups with the columnar C ORACLE instead of the GPU.
     Used by CPU tests of the host prologue/epilogue only."""

@@ -9,7 +9,8 @@ import numpy as np
 import pytest
 
 from k_llms_b200 import _native as K
-from tests.test_gpu_json import _expected, _expected_with_lists, _random_nested_record, _random_record
+from tests.helpers import general_and_mutated_records
+from tests.test_gpu_json import _expected, _expected_with_lists
 from tests.test_jsongpu_host_logic import _flat_record, _phrase_record, _shaped_record, s32_texts
 
 pytestmark = pytest.mark.gpu
@@ -97,33 +98,7 @@ def test_nested_objects_on_the_device():
 
 
 def test_general_and_mutated_records_never_wrong():
-    rng = random.Random(11)
-    by_n = {}
-    for _ in range(600):
-        n = rng.choice([2, 3, 5, 8, 16])
-        by_n.setdefault(n, []).append(_random_record(rng, n))
-    for _ in range(200):
-        n = rng.choice([2, 3, 5])
-        by_n.setdefault(n, []).append(_random_nested_record(rng, n))
-    alphabet = '{}[]",:0123456789.eE-+ntf \n\t\\u00e9abcxyzNI'
-
-    def mutate(text):
-        chars = list(text)
-        for _ in range(rng.randrange(1, 3)):
-            i, r = rng.randrange(len(chars)), rng.random()
-            if r < 0.4:
-                chars[i] = rng.choice(alphabet)
-            elif r < 0.7:
-                del chars[i]
-            else:
-                chars.insert(i, rng.choice(alphabet))
-        return "".join(chars)
-
-    for _ in range(800):
-        n = rng.choice([2, 3, 5])
-        texts = [mutate(t) if rng.random() < 0.5 else t for t in _flat_record(rng, n)]
-        if all(texts):
-            by_n.setdefault(n, []).append(texts)
+    by_n = general_and_mutated_records(11)
     counts = {0: 0, 1: 0, 2: 0}
     for _n, recs in by_n.items():
         res = run(recs)

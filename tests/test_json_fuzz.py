@@ -76,11 +76,11 @@ def build_truth(rng, shape):
     return [build_truth(rng, kind) if isinstance(kind, list) else truth(rng, kind) for k, kind in shape]
 
 
-def _records(count, seed):
+def _records(count, seed, ns=(2, 3, 5, 8, 16)):
     rng = random.Random(seed)
     by_n = {}
     for _ in range(count):
-        n = rng.choice([2, 3, 5, 8, 16])
+        n = rng.choice(ns)
         shape = make_shape(rng, 1)
         tr = build_truth(rng, shape)
         by_n.setdefault(n, []).append([render(rng, shape, tr, 0) for _ in range(n)])

@@ -10,7 +10,8 @@ import random
 import numpy as np
 
 from k_llms_b200 import _native as K
-from tests.helpers import jsongpu_with_oracle
+from tests.helpers import (boundary_texts, cpython_doubles, jsongpu_with_oracle, near_halfway_texts, number_texts, pack_number_texts,
+                           repr_doubles)
 from tests.test_gpu_json import _expected, _random_nested_record, _random_record
 
 
@@ -342,40 +343,49 @@ def test_declines_what_it_does_not_model():
         assert got is None and st != 0, name
 
 
+def parse_doubles(texts, device=None):
+    """kc_debug_parse_doubles (device None: the host instantiation) or kc_debug_parse_doubles_device -> (values, ok flags)."""
+    lib = K.load()
+    blob, off = pack_number_texts(texts)
+    out, ok = np.zeros(len(texts)), np.zeros(len(texts), dtype=np.uint8)
+    if device is None:
+        K.check(lib.kc_debug_parse_doubles(blob.ctypes.data, off.ctypes.data, len(texts), out.ctypes.data, ok.ctypes.data))
+    else:
+        K.check(lib.kc_debug_parse_doubles_device(blob.ctypes.data, off.ctypes.data, len(texts), out.ctypes.data, ok.ctypes.data, device))
+    return out, ok
+
+
+def assert_parsed_like_cpython(texts, out, ok):
+    """Every accepted text parsed to the bits of float(json.loads(text))."""
+    exp = cpython_doubles(texts)
+    bad = np.nonzero(ok.astype(bool) & (out.view(np.uint64) != exp.view(np.uint64)))[0]
+    assert len(bad) == 0, [(texts[i], out[i], exp[i]) for i in bad[:10]]
+
+
 def test_exact_number_conversions_match_cpython():
     lib = K.load()
-    rng = random.Random(5)
-    texts = [repr(rng.random() * 1e4 + 1) for _ in range(20000)]
-    texts += [str(rng.randrange(-10 ** 19, 10 ** 19)) for _ in range(20000)]
-    texts += ["%.*f" % (rng.randrange(0, 12), rng.random() * 10 ** rng.randrange(-3, 9)) for _ in range(20000)]
-    texts += ["%.*e" % (rng.randrange(0, 18), rng.random() * 10.0 ** rng.randrange(-25, 25)) for _ in range(20000)]
-    texts += ["0.0", "-0.0", "1e0", "1E+5", "1e-5", "1234567890123456789", "0.30000000000000004", "9007199254740993", "4.35", "1e19",
-              "5e-20", "0.5000000000000000000000000", "9.999999999999999e22", "1e22"]
-    enc = [t.encode() for t in texts]
-    off = np.zeros(len(enc) + 1, dtype=np.int64)
-    np.cumsum([len(b) for b in enc], out=off[1:])
-    blob = np.frombuffer(b"".join(enc), dtype=np.uint8).copy()
-    out, ok = np.zeros(len(enc)), np.zeros(len(enc), dtype=np.uint8)
-    K.check(lib.kc_debug_parse_doubles(blob.ctypes.data, off.ctypes.data, len(enc), out.ctypes.data, ok.ctypes.data))
-    assert ok.sum() > 0.8 * len(enc)
-    for t, o, k in zip(texts, out, ok):
-        if k:
-            assert np.float64(o).tobytes() == np.float64(float(json.loads(t))).tobytes(), t
+    texts = number_texts()
+    out, ok = parse_doubles(texts)
+    assert ok.sum() > 0.8 * len(texts)
+    assert_parsed_like_cpython(texts, out, ok)
+    # both sides of rounding decisions (exact ties, the long division's sticky bit) and the edges of the accepted range
+    texts = near_halfway_texts()
+    out, ok = parse_doubles(texts)
+    assert ok.sum() > 0.8 * len(texts)
+    assert_parsed_like_cpython(texts, out, ok)
+    texts, decline = boundary_texts()
+    out, ok = parse_doubles(texts + decline)
+    assert not ok[len(texts):].any(), [t for t, k in zip(decline, ok[len(texts):]) if k]
+    assert_parsed_like_cpython(texts + decline, out, ok)
 
-    nrng = np.random.default_rng(1)
-    bits = nrng.integers(0, 2 ** 63, 40000, dtype=np.uint64).view(np.float64)
-    xs = np.concatenate([nrng.random(40000) * 1e4 + 1, np.floor(nrng.random(20000) * 1e6), bits[np.isfinite(bits)], -bits[:500],
-                         nrng.random(40000) * 10.0 ** nrng.integers(-30, 30, 40000), np.round(nrng.random(20000), 5),
-                         [2.0 ** k for k in range(-1074, 1024)], [10.0 ** k for k in range(-323, 309)],
-                         [0.0, -0.0, 1.0, 1e16, 1e15, 123456789012345680.0, 1e-5, 1e-4, 5e-324, 1.7976931348623157e308,
-                          2.2250738585072014e-308, 1e22, 1e23, float("inf"), float("-inf"), float("nan")]])
-    xs = np.ascontiguousarray(xs)
+    xs = repr_doubles()
     buf, lens = np.zeros((len(xs), 32), dtype=np.uint8), np.zeros(len(xs), dtype=np.int32)
     K.check(lib.kc_debug_float_reprs(xs.ctypes.data, len(xs), buf.ctypes.data, lens.ctypes.data))
     for i, x in enumerate(xs):
         assert bytes(buf[i, :lens[i]]).decode() == json.dumps(float(x)), repr(float(x))
 
     # and the products of tests/test_gpu_kernels.py::test_round5_random_products: pvf * support / present, near-half cases first
+    rng = random.Random(5)
     prng = np.random.default_rng(3)
     present = prng.integers(1, 65, 200000)
     support = np.minimum((prng.random(200000) * present).astype(np.int64) + 1, present)
