@@ -248,6 +248,18 @@ int kc_medoid_str(const uint8_t *d_chars, const int32_t *d_str_off, const int32_
 int kc_medoid_str_method(const uint8_t *d_chars, const int32_t *d_str_off, const int32_t *d_grp_off, int64_t n_groups,
                          int32_t max_group, int32_t method, int32_t *d_best_idx, double *d_best_avg, void *stream);
 
+/*
+ * K5 — numeric similarity medoid: the primitive branch of the reference's ASYNC dispatcher (async_consensus_as_primitive,
+ * consensus_utils.py:1638-1688), which has no numeric clustering.  Over the group's non-None cells: pairwise
+ * numerical_similarity (math.isclose(rel_tol=0.01) -> 1.0, else 1e-8), np.nanmean of each row in numpy's summation order,
+ * first argmax.
+ *   d_cells float64[G][n]  K2's encoding (n in 1..64): KC_F64_NONE_BITS / KC_F64_ABSENT_BITS (recognised by the high word) are
+ *                          not candidates; every other double is a present number (+-inf and other NaNs included)
+ *   d_best  int32[G]       position of the medoid among the group's non-None cells; -1 when there is none
+ *   d_best_avg float64[G]  its mean similarity (unrounded), bit-identical to numpy's; NaN when there are fewer than two cells
+ */
+int kc_numeric_medoid_f64(const double *d_cells, int64_t n_groups, int32_t n, int32_t *d_best, double *d_best_avg, void *stream);
+
 /* K4 with HOST buffers (H2D, one launch, D2H; synchronous): what the host planners call for a batch of string groups. */
 int kc_medoid_str_host(const uint8_t *h_chars, int64_t n_chars, const int32_t *h_str_off, const int32_t *h_grp_off, int64_t n_groups,
                        int32_t max_group, int32_t *h_best_idx, double *h_best_avg, int device);
@@ -347,11 +359,16 @@ void kc_free_strings(char **arr, int64_t count);
  *   h_text   all candidate texts back to back (ideally page-locked: kc_host_alloc)
  *   h_off    int64[n_records * n + 1]  candidate c of record r is h_text[h_off[r*n+c] .. h_off[r*n+c+1])  (record-major)
  *   flags    KC_JSON_DEVICE_ONLY: skip the host path (declined records keep status 1)
+ *            KC_JSON_NUMERIC_MEDOID: the reference's ASYNC dispatcher (async_consensus_values): a numeric field is decided by
+ *                     K5 (kc_numeric_medoid_f64) in K2's place, its value is the chosen candidate's original number and its
+ *                     likelihood round(pvf * avg, 5) (kc::medoid_confidence); a numeric field that also holds strings or bools
+ *                     is declined.  The host path decides numbers the sync way, so this flag implies KC_JSON_DEVICE_ONLY.
  *   *out     result handle: one text blob + per-record spans (kc_json_result_view), released with kc_json_result_free
  * status per record: 0 = consolidated on the device, 2 = consolidated by the host path, 1 = needs the Python path.
  * Texts are byte-identical to the reference's json.dumps output.  Re-entrant (pooled per-call streams and buffers).
  */
 #define KC_JSON_DEVICE_ONLY 1u
+#define KC_JSON_NUMERIC_MEDOID 2u
 typedef struct kc_json_result kc_json_result;
 typedef struct {
     int64_t n_records, n_device, n_host, n_python; /* where the records were consolidated */
@@ -381,6 +398,9 @@ void kc_json_result_free(kc_json_result *res);
  * kc_json_emit, so the CPU tests can put the oracle in K1 / K2's place.  Not a product path. */
 typedef struct kc_debug_jsongpu kc_debug_jsongpu;
 int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, kc_debug_jsongpu **out);
+/* the same with the flags of kc_consolidate_json_packed that change the phases (KC_JSON_NUMERIC_MEDOID) */
+int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, uint32_t flags,
+                                kc_debug_jsongpu **out);
 int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells, int64_t *n_vote_groups, const double **num_cells,
                             int64_t *n_num_groups, const uint8_t **status);
 int kc_debug_jsongpu_emit(kc_debug_jsongpu *h, const uint32_t *vote_meta, const double *num_value, const uint32_t *num_meta,
@@ -396,6 +416,9 @@ int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_met
 int kc_debug_jsongpu_medoid_inputs(const kc_debug_jsongpu *h, const uint8_t **chars, const int32_t **str_off, const int32_t **grp_off,
                                    int64_t *n_groups);
 int kc_debug_jsongpu_set_medoid(kc_debug_jsongpu *h, const int32_t *medoid_idx, const double *medoid_avg);
+/* KC_JSON_NUMERIC_MEDOID: K5's results for the numeric groups (kc_debug_jsongpu_inputs' numeric cells), set like _set_medoid;
+ * _emit's num_value / num_meta are then not read */
+int kc_debug_jsongpu_set_numeric_medoid(kc_debug_jsongpu *h, const int32_t *best, const double *best_avg);
 void kc_debug_jsongpu_free(kc_debug_jsongpu *h);
 int kc_debug_parse_doubles(const char *text, const int64_t *off, int64_t count, double *out, uint8_t *ok);
 int kc_debug_float_reprs(const double *xs, int64_t count, char *out /* [count][32] */, int32_t *lens);

@@ -55,6 +55,7 @@ _SIGNATURES = {
     "kc_medoid_str": (_int, [_vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp]),
     "kc_medoid_str_method": (_int, [_vp, _vp, _vp, _i64, _i32, _i32, _vp, _vp, _vp]),
     "kc_medoid_str_host": (_int, [_vp, _i64, _vp, _vp, _i64, _i32, _vp, _vp, _int]),
+    "kc_numeric_medoid_f64": (_int, [_vp, _i64, _i32, _vp, _vp, _vp]),
     "kc_levenshtein": (_int, [_str, _i32, _str, _i32]),
     "kc_consolidate_json": (_int, [_vp, _vp, _i64, _i32, _f64, _f64, _int, _i32, _vp, _vp, _vp]),
     "kc_free_strings": (None, [_vp, _i64]),
@@ -73,12 +74,14 @@ _SIGNATURES = {
     "kc_debug_alignsim": (_int, [_vp, _i32, _vp]),
     "kc_debug_alignsim_nodes": (_int, [_vp, _vp, _i32, _i32, _int, _vp]),
     "kc_debug_jsongpu_plan": (_int, [_vp, _vp, _i64, _i32, _pp]),
+    "kc_debug_jsongpu_plan_flags": (_int, [_vp, _vp, _i64, _i32, _u32, _pp]),
     "kc_debug_jsongpu_inputs": (_int, [_vp] * 6),
     "kc_debug_jsongpu_emit": (_int, [_vp, _vp, _vp, _vp] + [_pp] * 4),
     "kc_debug_jsongpu_group_records": (_int, [_vp, _pp]),
     "kc_debug_jsongpu_emit_weighted": (_int, [_vp, _vp, _vp, _vp, _vp] + [_pp] * 4),
     "kc_debug_jsongpu_medoid_inputs": (_int, [_vp] + [_pp] * 3 + [ctypes.POINTER(_i64)]),
     "kc_debug_jsongpu_set_medoid": (_int, [_vp, _vp, _vp]),
+    "kc_debug_jsongpu_set_numeric_medoid": (_int, [_vp, _vp, _vp]),
     "kc_debug_jsongpu_free": (None, [_vp]),
     "kc_debug_parse_doubles": (_int, [_vp, _vp, _i64, _vp, _vp]),
     "kc_debug_float_reprs": (_int, [_vp, _i64, _vp, _vp]),
@@ -284,6 +287,20 @@ def consensus_host(codes, none_code, vals, rel_eps=0.03, abs_eps=1e-6, device=0,
     return {"win_code": win, "vote_meta": vmeta, "value": value, "num_meta": nmeta, "device_ms": float(ms.value)}
 
 
+def numeric_medoid(cells, stream=None):
+    """K5 on device tensors: the async dispatcher's numeric medoid.  cells float64 [G, n] (K2's encoding, n <= 64) ->
+    (best int32 [G]: the medoid's position among the group's non-None cells, -1 for none; avg float64 [G]: its unrounded mean
+    similarity, NaN with fewer than two non-None cells)."""
+    torch = _require_cuda()
+    assert cells.is_cuda and cells.dtype == torch.float64 and cells.dim() == 2 and cells.is_contiguous()
+    G, n = cells.shape
+    best = torch.empty(G, dtype=torch.int32, device=cells.device)
+    avg = torch.empty(G, dtype=torch.float64, device=cells.device)
+    _bind(torch, cells)
+    check(load().kc_numeric_medoid_f64(cells.data_ptr(), G, n, best.data_ptr(), avg.data_ptr(), _stream_ptr(torch, stream)))
+    return best, avg
+
+
 SIM_METHODS = {"levenshtein": 0, "embeddings": 0, "jaccard": 1, "hamming": 2}  # "embeddings": pairs the planner sends here are Levenshtein pairs
 
 
@@ -454,6 +471,7 @@ class JsonStats(ctypes.Structure):
 
 
 JSON_DEVICE_ONLY = 1
+JSON_NUMERIC_MEDOID = 2  # the async dispatcher: numeric fields are similarity medoids (K5); implies JSON_DEVICE_ONLY
 
 
 def pack_texts(records, pinned: bool = True):

@@ -186,9 +186,10 @@ struct ChunkStage {  // per-chunk device-time split (CUDA events on the chunk's 
 };
 
 // One chunk on one worker: records [r0, r1) of the batch.  h_seq (NULL: count votes): the batch's candidate sums [R][n], the
-// vote leaves are likelihood-weighted (K3b over ragged records in K1's place).
-int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, int64_t r0, int64_t r1, int32_t n, double rel_eps,
-              double abs_eps, int sm_count, kc_json_result &res, ChunkStage &st) {
+// vote leaves are likelihood-weighted (K3b over ragged records in K1's place).  xmedoid (KC_JSON_NUMERIC_MEDOID): numeric fields
+// are similarity medoids (K5 in K2's place).
+int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, int64_t r0, int64_t r1, int32_t n,
+              double rel_eps, double abs_eps, int sm_count, kc_json_result &res, ChunkStage &st) {
     const int64_t Rc = r1 - r0;
     const int64_t b0 = h_off[r0 * n], b1 = h_off[r1 * n];
     const size_t bytes = (size_t)(b1 - b0);
@@ -239,6 +240,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     ch.ccount = w.ccount.as<uint32_t>();
     ch.len_c = w.len_c.as<int64_t>();
     ch.len_l = w.len_l.as<int64_t>();
+    ch.xmedoid = xmedoid;
 
     nvtxRangePushA("kc_json: H2D texts");
     KC_CUDA_I(cudaEventRecord(w.ev[0], s));
@@ -287,6 +289,8 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     ch.vmeta = w.vmeta.as<uint32_t>();
     ch.xvalue = w.xvalue.as<double>();
     ch.xmeta = w.xmeta.as<uint32_t>();
+    ch.xbest = w.xmeta.as<int32_t>();  // K5 writes its results where K2 would
+    ch.xavg = w.xvalue.as<double>();
     if (h_seq) {
         R_(w.vrec.reserve(std::max<size_t>(T, 1) * 4));
         R_(w.vweight.reserve(std::max<size_t>(T, 1) * 4));
@@ -343,7 +347,8 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
                                       w.vweight.as<float>(), s));
     else if (gv)
         R_(kc_vote_i8(ch.vcells, gv, n, nullptr, 1, w.win.as<int32_t>(), w.vmeta.as<uint32_t>(), s));
-    if (gx) R_(kc_numeric_f64(ch.xcells, gx, n, rel_eps, abs_eps, w.xvalue.as<double>(), w.xmeta.as<uint32_t>(), s));
+    if (gx && xmedoid) R_(kc_numeric_medoid_f64(ch.xcells, gx, n, w.xmeta.as<int32_t>(), w.xvalue.as<double>(), s));
+    else if (gx) R_(kc_numeric_f64(ch.xcells, gx, n, rel_eps, abs_eps, w.xvalue.as<double>(), w.xmeta.as<uint32_t>(), s));
     if (gm) R_(kc_medoid_str(ch.mchars, ch.mstr_off, ch.mgrp_off, gm, std::max(2, n), w.midx.as<int32_t>(), w.mavg.as<double>(), s));
     KC_CUDA_I(cudaEventRecord(w.ev[3], s));
     nvtxRangePop();
@@ -421,11 +426,11 @@ extern "C" {
 namespace {
 
 // kc_consolidate_json_packed, and with h_seq its likelihood-weighted variant (which hands no record to the host path: that
-// path votes by count)
+// path votes by count; nor does KC_JSON_NUMERIC_MEDOID: that path decides numbers the sync way)
 int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_seq, int64_t n_records, int32_t n, double rel_eps,
                        double abs_eps, int device, int32_t threads, uint32_t flags, kc_json_result **out) {
     if (!out) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: NULL out");
-    if (h_seq) flags |= KC_JSON_DEVICE_ONLY;
+    if (h_seq || (flags & KC_JSON_NUMERIC_MEDOID)) flags |= KC_JSON_DEVICE_ONLY;
     *out = nullptr;
     if (n < 2 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: n=%d outside [2,%d]", n, KC_MAX_CANDIDATES);
     if (n_records < 0 || (n_records && (!h_text || !h_off))) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: bad arguments");
@@ -496,7 +501,8 @@ int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_
         while (!rc) {
             const int k = next.fetch_add(1);
             if (k >= n_chunks) break;
-            rc = run_chunk(w, h_text, h_off, h_seq, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res, stages[(size_t)wi]);
+            rc = run_chunk(w, h_text, h_off, h_seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps,
+                           abs_eps, sm_count, *res, stages[(size_t)wi]);
         }
         if (rc) {
             cudaStreamSynchronize(w.stream);
@@ -657,6 +663,11 @@ struct kc_debug_jsongpu {
 };
 
 int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, kc_debug_jsongpu **out) {
+    return kc_debug_jsongpu_plan_flags(h_text, h_off, n_records, n, 0u, out);
+}
+
+int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, uint32_t flags,
+                                kc_debug_jsongpu **out) {
     if (!h_text || !h_off || !out || n < 2 || n > KC_MAX_CANDIDATES || n_records < 0) return KC_EINVAL;
     kc_debug_jsongpu *h = new kc_debug_jsongpu;
     const int64_t R = n_records;
@@ -692,6 +703,7 @@ int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_re
     ch.ccount = h->ccount.data();
     ch.len_c = h->len_c.data();
     ch.len_l = h->len_l.data();
+    ch.xmedoid = (flags & KC_JSON_NUMERIC_MEDOID) != 0;
     for (int32_t r = 0; r < R; ++r) kc::js::count_record(ch, r);
     for (int64_t r = 0; r < R; ++r) h->slot[(size_t)r + 1] = h->slot[(size_t)r] + h->fcount[(size_t)r];
     const size_t T = h->slot[(size_t)R];
@@ -754,6 +766,13 @@ int kc_debug_jsongpu_set_medoid(kc_debug_jsongpu *h, const int32_t *medoid_idx, 
     if (!h) return KC_EINVAL;
     h->ch.midx = medoid_idx;  // must stay alive until kc_debug_jsongpu_emit has returned
     h->ch.mavg = medoid_avg;
+    return KC_OK;
+}
+
+int kc_debug_jsongpu_set_numeric_medoid(kc_debug_jsongpu *h, const int32_t *best, const double *best_avg) {
+    if (!h) return KC_EINVAL;
+    h->ch.xbest = best;  // must stay alive until kc_debug_jsongpu_emit has returned
+    h->ch.xavg = best_avg;
     return KC_OK;
 }
 

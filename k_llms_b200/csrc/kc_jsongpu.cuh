@@ -72,6 +72,10 @@ struct Chunk {
     const uint32_t *vmeta;   // K1 (or K3b) result words
     const double *xvalue;    // K2 values
     const uint32_t *xmeta;   // K2 result words
+    // KC_JSON_NUMERIC_MEDOID (the reference's async dispatcher): numeric fields are similarity medoids, decided by K5 in K2's place
+    bool xmedoid;
+    const int32_t *xbest;    // K5 results: the medoid's position among the group's non-None cells,
+    const double *xavg;      //             its mean similarity
     uint32_t *piece_c, *piece_l;  // [slots] by (slot + rank): piece length, then (after the leader's pass) piece offset
     int64_t *len_c, *len_l;       // [R+1] record lengths -> (exclusive scan, in place) record offsets in the output blobs
     uint8_t *out_c, *out_l;       // output blobs: consensus texts, likelihoods texts
@@ -228,6 +232,12 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
                 }
         } else {
             kind = F_NUMERIC;  // strings / bools among the cells are "present, not a number" (cu:1105-1114)
+            if (ch.xmedoid)    // ... but the async medoid compares them by generic_similarity's own rules (0 and false are both falsy)
+                for (int32_t c = 0; c < n; ++c)
+                    if (row[c].kind == K_STR || row[c].kind == K_TRUE || row[c].kind == K_FALSE) {
+                        decline(ch, r, D_MIXED_TYPES);
+                        return;
+                    }
         }
         ch.fdesc[ch.slot[r] + j] = fdesc_pack(kind, last, rank, 0);
     }
@@ -404,6 +414,22 @@ KC_HD inline void encode_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t
 
 // ---------------------------------------------------------------- C0 / C1
 
+// one cell's original object as json.dumps prints it: ints keep their digits ("-0" is int 0), floats through float.__repr__
+KC_HD inline void put_original(const Chunk &ch, const Tok &t, Sink &content) {
+    if (t.kind == K_INT) {
+        if (t.vlen == 2 && ch.text[t.vstart] == '-' && ch.text[t.vstart + 1] == '0') content.put('0');
+        else content.put(ch.text + t.vstart, t.vlen);
+    } else if (t.kind == K_FLOAT) {
+        double v = 0.0;
+        to_double(ch.text + t.vstart, t.vlen, v);
+        float_repr(v, content);
+    } else if (t.kind == K_STR) {
+        content.json_string(ch.text + t.vstart, t.vlen, t.flags & TOK_ESCAPED);
+    } else {
+        content.lit(t.kind == K_TRUE ? "true" : (t.kind == K_FALSE ? "false" : "null"));
+    }
+}
+
 // value and confidence of one field, formatted into the two sinks (the epilogue emit_leaf of kc_json.cpp:
 // cu:971-982, cu:1085-1086, cu:1116, cu:1177-1219); the confidences are kc::confidence / kc::medoid_confidence
 KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &content, Sink &lik) {
@@ -420,24 +446,25 @@ KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &cont
         } else {
             content.json_string(ch.text + row[idx].vstart, row[idx].vlen, row[idx].flags & TOK_ESCAPED);  // first original whose sanitised form wins (cu:971)
         }
+    } else if (kind == F_NUMERIC && ch.xmedoid) {  // the async dispatcher's similarity medoid (cu:1638-1688, K5)
+        uint32_t live = 0;
+        for (int32_t c = 0; c < n; ++c) live += row[c].kind != K_NULL ? 1u : 0u;
+        const int64_t gi = (int64_t)ch.xbase[r] + g;
+        int32_t want = ch.xbest[gi];
+        conf = medoid_confidence(live, n, ch.xavg[gi]);
+        for (int32_t c = 0; c < n; ++c) {
+            if (row[c].kind == K_NULL) continue;
+            if (want-- == 0) {
+                put_original(ch, row[c], content);
+                break;
+            }
+        }
     } else if (kind == F_NUMERIC) {
         m = ch.xmeta[(int64_t)ch.xbase[r] + g];
         const uint32_t idx = KC_META_IDX(m), flags = KC_META_FLAGS(m);
         if (flags & KC_FLAG_HAS_VALUE) {
             if (flags & KC_FLAG_SINGLE) {  // the original object, confidence unrounded (cu:1085-1086)
-                const Tok &t = row[idx];
-                if (t.kind == K_INT) {
-                    if (t.vlen == 2 && ch.text[t.vstart] == '-' && ch.text[t.vstart + 1] == '0') content.put('0');
-                    else content.put(ch.text + t.vstart, t.vlen);
-                } else if (t.kind == K_FLOAT) {
-                    double v = 0.0;
-                    to_double(ch.text + t.vstart, t.vlen, v);
-                    float_repr(v, content);
-                } else if (t.kind == K_STR) {
-                    content.json_string(ch.text + t.vstart, t.vlen, t.flags & TOK_ESCAPED);
-                } else {
-                    content.lit(t.kind == K_TRUE ? "true" : (t.kind == K_FALSE ? "false" : "null"));
-                }
+                put_original(ch, row[idx], content);
             } else {
                 float_repr(ch.xvalue[(int64_t)ch.xbase[r] + g], content);
             }
@@ -467,7 +494,7 @@ KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &cont
     }
     // one call for both kinds keeps one inlined copy (two made write_kernel save convergence barriers); a vote group always
     // reaches the HAS_VALUE arm: a string group has a non-None cell, and a bool group turns None into False
-    if (kind == F_VOTE_STR || kind == F_VOTE_BOOL || kind == F_NUMERIC) conf = confidence(m, kind == F_NUMERIC, 1.0);
+    if (kind == F_VOTE_STR || kind == F_VOTE_BOOL || (kind == F_NUMERIC && !ch.xmedoid)) conf = confidence(m, kind == F_NUMERIC, 1.0);
     // likelihood-weighted calls: a vote leaf's likelihood is pvf (1 on this path) times K3b's weight share
     if (ch.vweight && (kind == F_VOTE_STR || kind == F_VOTE_BOOL)) conf = weighted_vote_confidence(1.0, ch.vweight[(int64_t)ch.vbase[r] + g]);
     float_repr(conf, lik);

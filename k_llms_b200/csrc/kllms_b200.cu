@@ -25,6 +25,7 @@
 #include "kc_extra.cuh"
 #include "kc_medoid.cuh"
 #include "kc_numeric.cuh"
+#include "kc_numeric_medoid.cuh"
 #include "kc_push.cuh"
 #include "kc_vote.cuh"
 
@@ -790,6 +791,23 @@ int kc_medoid_str_method(const uint8_t *d_chars, const int32_t *d_str_off, const
     if (rc) return rc;
     kernel<<<grid, WARPS * 32, smem, static_cast<cudaStream_t>(stream)>>>(d_chars, d_str_off, d_grp_off, n_groups, max_group,
                                                                          d_best_idx, d_best_avg, method);
+    KC_CUDA_I(cudaGetLastError());
+    return KC_OK;
+}
+
+int kc_numeric_medoid_f64(const double *d_cells, int64_t n_groups, int32_t n, int32_t *d_best, double *d_best_avg, void *stream) {
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_numeric_medoid_f64: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
+    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_numeric_medoid_f64: negative n_groups");
+    if (n_groups == 0) return KC_OK;
+    if (!d_cells || !d_best || !d_best_avg) return kc_fail(KC_EINVAL, "kc_numeric_medoid_f64: NULL buffer");
+    int team = 1;
+    while (team < n && team < 32) team *= 2;
+    const int64_t groups_per_block = (int64_t)kc::kNumMedoidWarps * (32 / team);
+    int grid = 0;
+    int rc = stride_grid((n_groups + groups_per_block - 1) / groups_per_block, grid);
+    if (rc) return rc;
+    kc::numeric_medoid_kernel<<<grid, kc::kNumMedoidWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(d_cells, n_groups, n, team, d_best,
+                                                                                                       d_best_avg);
     KC_CUDA_I(cudaGetLastError());
     return KC_OK;
 }

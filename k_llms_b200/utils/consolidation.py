@@ -126,11 +126,10 @@ def _native_settings(settings) -> bool:
             and settings.string_consensus_method == "centroid" and settings.min_support_ratio == 0.51)
 
 
-def _consensus_of_choices_native(choices, settings, embed, weighted: bool = False):
-    """The whole per-request path in native code (H1): the n `choice.message.content` texts in -> (consensus value,
-    likelihoods), i.e. parse + alignment pre-pass + vote / numeric / medoid kernels + decode — or None when the request needs
-    the Python path (non-default settings, fewer than two non-empty contents, anything H1 declines; no embeddings callable:
-    the reference raises ValueError for primitive fields then, cu:1445-1446, and so does the Python path)."""
+def _native_request(choices, settings, embed, weighted: bool):
+    """(candidate texts, their token logprobs or None) of a request the native JSON path may take, or None when it needs the
+    Python path (non-default settings, fewer than two or more than 64 non-empty contents; no embeddings callable: the reference
+    raises ValueError for primitive fields then, cu:1445-1446, and so does the Python path)."""
     from .. import _native
     # weighted: the token logprobs of the same candidates, checked before anything runs on the GPU
     lp = _pack_logprobs(_token_logprobs_of(choices)) if weighted else None
@@ -139,7 +138,36 @@ def _consensus_of_choices_native(choices, settings, embed, weighted: bool = Fals
     texts = [c.message.content for c in choices if c.message.content]  # the filter of _contents_of (reference consolidation.py:92)
     if len(texts) < 2 or len(texts) > _native.MAX_CANDIDATES or not _native_settings(settings):
         return None
-    out = _combiner.run(texts, settings.rel_eps, settings.abs_eps, lp)
+    return texts, lp
+
+
+def _consensus_of_choices_native(choices, settings, embed, weighted: bool = False):
+    """The whole per-request path in native code (H1): the n `choice.message.content` texts in -> (consensus value,
+    likelihoods), i.e. parse + alignment pre-pass + vote / numeric / medoid kernels + decode — or None when the request needs
+    the Python path (_native_request's rules, anything H1 declines)."""
+    req = _native_request(choices, settings, embed, weighted)
+    if req is None:
+        return None
+    return _native_value(_combiner.run(req[0], settings.rel_eps, settings.abs_eps, req[1]))
+
+
+async def _consensus_of_choices_native_async(choices, settings, embed, weighted: bool = False):
+    """The async twin of _consensus_of_choices_native: the device JSON path with the reference's ASYNC dispatcher
+    (JSON_NUMERIC_MEDOID: numeric fields are similarity medoids, K5).  None when the request needs the Python async route:
+    _native_request's rules, no CUDA device, or anything the device path declines (it hands nothing to the host path H1, which
+    decides numbers the sync way).  The event loop is not blocked while the GPU works."""
+    import torch
+    from .. import _native
+    if not torch.cuda.is_available():
+        return None
+    req = _native_request(choices, settings, embed, weighted)
+    if req is None:
+        return None
+    return _native_value(await _combiner.run_async(req[0], settings.rel_eps, settings.abs_eps, req[1], _native.JSON_NUMERIC_MEDOID))
+
+
+def _native_value(out):
+    """(consensus value, likelihoods) of one record's native result texts, or None."""
     if out is None:
         return None
     content_text, likelihoods_text = out
@@ -152,18 +180,19 @@ def _consensus_of_choices_native(choices, settings, embed, weighted: bool = Fals
     return value, json.loads(likelihoods_text)
 
 
-def _native_consolidate(records, rel_eps, abs_eps, device: int = 0, seq_logprobs=None, counts=None):
+def _native_consolidate(records, rel_eps, abs_eps, device: int = 0, seq_logprobs=None, counts=None, flags: int = 0):
     """records of n candidate texts -> [(content, likelihoods text) or None]: the device JSON path (H1g,
     kc_consolidate_json_packed: scan / key sort / typing / encode / K1 + K2 / emit on the GPU; re-entrant, pooled streams), which
     hands what it does not model to the host path (H1, kc_consolidate_json) inside the same call.  seq_logprobs (float32
-    [R*n], the candidates' sums): likelihood-weighted votes (kc_consolidate_json_packed_weighted; no host path).  counts
-    (optional dict): "device" += the records the device path consolidated."""
+    [R*n], the candidates' sums): likelihood-weighted votes (kc_consolidate_json_packed_weighted; no host path).  flags:
+    _native.JSON_NUMERIC_MEDOID for the async dispatcher (no host path either).  counts (optional dict): "device" += the records
+    the device path consolidated."""
     from .. import _native
     blob, off, n = _native.pack_texts(records, pinned=len(records) >= 256)  # page-locking only pays for batches
     if seq_logprobs is None:
-        res = _native.consolidate_json_packed(blob, off, n, rel_eps, abs_eps, device)
+        res = _native.consolidate_json_packed(blob, off, n, rel_eps, abs_eps, device, flags=flags)
     else:
-        res = _native.consolidate_json_packed_weighted(blob, off, n, seq_logprobs, rel_eps, abs_eps, device)
+        res = _native.consolidate_json_packed_weighted(blob, off, n, seq_logprobs, rel_eps, abs_eps, device, flags=flags)
     try:
         if counts is not None:
             counts["device"] = counts.get("device", 0) + int(res.stats.n_device)
@@ -177,13 +206,16 @@ class _Combiner:
     combining: the thread that holds the device runs its own request, then everything that queued up meanwhile as one
     kc_consolidate_json_packed call, and hands the results back).  An idle caller pays nothing (it takes the device and runs
     directly); under load the cost per request falls from one launch sequence each towards the batched rate
-    (tools/latency.py: tens of thousands of requests per second)."""
+    (tools/latency.py: tens of thousands of requests per second).  Coroutines queue through run_async, which never blocks the
+    event loop: the device is driven from a helper thread that completes the coroutines' futures.  Requests are combined per
+    (candidate count, eps, weighted, flags)."""
 
     def __init__(self):
         import threading
         self._device = threading.Lock()
         self._qlock = threading.Lock()
         self._queue: list = []
+        self._helper = None  # the one thread that drives the device for coroutines (created on first use)
 
     def _drain(self):
         while True:
@@ -192,9 +224,9 @@ class _Combiner:
             if not batch:
                 return
             groups: dict = {}
-            for item in batch:  # weighted requests apart from count votes
-                groups.setdefault((len(item["texts"]), item["eps"], item["lp"] is not None), []).append(item)
-            for (_n, eps, weighted), items in groups.items():
+            for item in batch:  # weighted requests apart from count votes, async dispatcher (flags) apart from sync
+                groups.setdefault((len(item["texts"]), item["eps"], item["lp"] is not None, item["flags"]), []).append(item)
+            for (_n, eps, weighted, flags), items in groups.items():
                 try:
                     seq = None
                     if weighted:  # one K3 launch for the whole combined call
@@ -205,32 +237,78 @@ class _Combiner:
                             offs.append(it["lp"][1][1:] + base)
                             base += int(it["lp"][1][-1])
                         seq = _logprob_sums(flat, np.concatenate(offs))
-                    outs = _native_consolidate([it["texts"] for it in items], eps[0], eps[1], seq_logprobs=seq)
+                    extra = {"flags": flags} if flags else {}  # the sync calls keep their signature
+                    outs = _native_consolidate([it["texts"] for it in items], eps[0], eps[1], seq_logprobs=seq, **extra)
                     for it, o in zip(items, outs):
                         it["out"] = o
                 except BaseException as exc:  # hand the failure to every waiter of the group
                     for it in items:
                         it["err"] = exc
                 for it in items:
-                    it["done"].set()
+                    it["notify"]()
 
-    def run(self, texts, rel_eps, abs_eps, lp=None):
-        """lp: (token logprobs, offsets) of the texts (_pack_logprobs) for likelihood-weighted votes, or None."""
-        import threading
-        item = {"texts": texts, "eps": (rel_eps, abs_eps), "lp": lp, "done": threading.Event(), "out": None, "err": None}
+    def _serve(self, held: bool = False):
+        """Drain while the device is free (held: the caller has already taken it).  After releasing it, look again: an item
+        queued while this thread held the device, whose caller found the device taken, is then served here or by the thread
+        that took the device since."""
+        while held or self._device.acquire(blocking=False):
+            held = False
+            try:
+                self._drain()
+            finally:
+                self._device.release()
+            with self._qlock:
+                if not self._queue:
+                    return
+
+    def _enqueue(self, texts, rel_eps, abs_eps, lp, flags, notify):
+        item = {"texts": texts, "eps": (rel_eps, abs_eps), "lp": lp, "flags": flags, "notify": notify, "out": None, "err": None}
         with self._qlock:
             self._queue.append(item)
-        while not item["done"].is_set():
-            if self._device.acquire(blocking=False):
-                try:
-                    self._drain()
-                finally:
-                    self._device.release()
-            else:
-                item["done"].wait(0.0005)
+        return item
+
+    @staticmethod
+    def _result(item):
         if item["err"] is not None:
             raise item["err"]
         return item["out"]
+
+    def run(self, texts, rel_eps, abs_eps, lp=None, flags: int = 0):
+        """lp: (token logprobs, offsets) of the texts (_pack_logprobs) for likelihood-weighted votes, or None; flags: those of
+        kc_consolidate_json_packed."""
+        import threading
+        done = threading.Event()
+        item = self._enqueue(texts, rel_eps, abs_eps, lp, flags, done.set)
+        while not done.is_set():
+            self._serve()
+            if not done.is_set():
+                done.wait(0.0005)
+        return self._result(item)
+
+    async def run_async(self, texts, rel_eps, abs_eps, lp=None, flags: int = 0):
+        """run() for a coroutine.  If the device is free, the helper thread drains the queue (this request and whatever queues up
+        meanwhile); else the thread holding the device serves it.  The coroutine waits on a future of its loop."""
+        loop = asyncio.get_running_loop()
+        fut = loop.create_future()
+
+        def wake():
+            if not fut.done():
+                fut.set_result(None)
+
+        def notify():
+            try:
+                loop.call_soon_threadsafe(wake)
+            except RuntimeError:  # the loop has been closed: nobody waits for the result
+                pass
+
+        item = self._enqueue(texts, rel_eps, abs_eps, lp, flags, notify)
+        if self._device.acquire(blocking=False):
+            if self._helper is None:  # one worker is enough: only the thread that took the device hands it work
+                from concurrent.futures import ThreadPoolExecutor
+                self._helper = ThreadPoolExecutor(max_workers=1, thread_name_prefix="kllms-combiner")
+            self._helper.submit(self._serve, True)
+        await fut
+        return self._result(item)
 
 
 _combiner = _Combiner()
@@ -277,6 +355,16 @@ def _consensus_of_choices_python(choices, settings, embed, client, weighted: boo
     """The Python planner's consensus of the choices (what the native path leaves to it), weighted or not."""
     contents, sums = _weighted_contents(choices) if weighted else (_contents_of(choices), None)
     return _consensus_sync(contents, settings, embed, client, sums)
+
+
+async def _consensus_of_choices_async(choices, settings, embed, client, weighted: bool):
+    """The async entry points' consensus of the choices: the device JSON path with the async dispatcher's numeric medoid when it
+    takes the request, else the Python async route (async_consensus_values: the reference's async semantics, votes on the GPU)."""
+    native = await _consensus_of_choices_native_async(choices, settings, embed, weighted)
+    if native is not None:
+        return native
+    contents, sums = _weighted_contents(choices) if weighted else (_contents_of(choices), None)
+    return await _consensus_async(contents, settings, embed, client, sums)
 
 
 def _assemble_plain(base: ChatCompletion, heads, consensus_content, likelihoods) -> KLLMsChatCompletion:
@@ -349,10 +437,8 @@ async def async_consolidate_chat_completions(
     if len(completion.choices) == 1:
         return KLLMsChatCompletion.model_validate(completion.model_dump())
     _check_candidates(len(completion.choices))
-    # the native JSON paths implement the SYNC semantics; the reference's async dispatcher differs on numeric fields
-    # (cu:1638-1688: no clustering), so the async entry points plan in Python (async_consensus_values) — votes still on the GPU
-    contents, sums = _weighted_contents(completion.choices) if weighted else (_contents_of(completion.choices), None)
-    content, likelihoods = await _consensus_async(contents, consensus_settings, async_get_openai_embeddings_from_text, client, sums)
+    content, likelihoods = await _consensus_of_choices_async(completion.choices, consensus_settings, async_get_openai_embeddings_from_text,
+                                                             client, weighted)
     return _assemble_plain(completion, list(completion.choices), content, likelihoods)
 
 
@@ -417,8 +503,8 @@ async def async_consolidate_parsed_chat_completions(
     if len(completion.choices) == 1:
         return KLLMsParsedChatCompletion.model_validate(completion.model_dump())
     _check_candidates(len(completion.choices))
-    contents, sums = _weighted_contents(completion.choices) if weighted else (_contents_of(completion.choices), None)
-    content, likelihoods = await _consensus_async(contents, consensus_settings, async_get_openai_embeddings_from_text, client, sums)
+    content, likelihoods = await _consensus_of_choices_async(completion.choices, consensus_settings, async_get_openai_embeddings_from_text,
+                                                             client, weighted)
     return _assemble_parsed(completion, content, likelihoods, response_format, keep_usage=False)
 
 
