@@ -363,12 +363,17 @@ void kc_free_strings(char **arr, int64_t count);
  *                     K5 (kc_numeric_medoid_f64) in K2's place, its value is the chosen candidate's original number and its
  *                     likelihood round(pvf * avg, 5) (kc::medoid_confidence); a numeric field that also holds strings or bools
  *                     is declined.  The host path decides numbers the sync way, so this flag implies KC_JSON_DEVICE_ONLY.
+ *            KC_JSON_KEY_UNION: records whose candidates differ in shape (keys in another order, missing or extra keys, a null or
+ *                     missing sub-object where another candidate holds an object) stay on the device: the key-union round
+ *                     consolidates them as the reference's pre-pass aligns them (missing -> None, None -> an object of Nones).
+ *                     Without it they are declined as before.  The client functions set it.
  *   *out     result handle: one text blob + per-record spans (kc_json_result_view), released with kc_json_result_free
  * status per record: 0 = consolidated on the device, 2 = consolidated by the host path, 1 = needs the Python path.
  * Texts are byte-identical to the reference's json.dumps output.  Re-entrant (pooled per-call streams and buffers).
  */
 #define KC_JSON_DEVICE_ONLY 1u
 #define KC_JSON_NUMERIC_MEDOID 2u
+#define KC_JSON_KEY_UNION 4u
 typedef struct kc_json_result kc_json_result;
 typedef struct {
     int64_t n_records, n_device, n_host, n_python; /* where the records were consolidated */
@@ -398,7 +403,7 @@ void kc_json_result_free(kc_json_result *res);
  * kc_json_emit, so the CPU tests can put the oracle in K1 / K2's place.  Not a product path. */
 typedef struct kc_debug_jsongpu kc_debug_jsongpu;
 int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, kc_debug_jsongpu **out);
-/* the same with the flags of kc_consolidate_json_packed that change the phases (KC_JSON_NUMERIC_MEDOID) */
+/* the same with the flags of kc_consolidate_json_packed that change the phases (KC_JSON_NUMERIC_MEDOID, KC_JSON_KEY_UNION) */
 int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, uint32_t flags,
                                 kc_debug_jsongpu **out);
 int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells, int64_t *n_vote_groups, const double **num_cells,

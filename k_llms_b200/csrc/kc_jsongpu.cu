@@ -45,6 +45,22 @@ struct DBuf {  // grow-only device buffer
         cap = need;
         return KC_OK;
     }
+    // reserve() that keeps the first `keep` bytes (copied on stream s; the stream is synchronised before the old buffer is freed)
+    int grow(size_t need, size_t keep, cudaStream_t s) {
+        if (p && need <= cap) return KC_OK;
+        void *old = p;
+        const size_t old_cap = cap;
+        p = nullptr;
+        cap = 0;
+        if (const int rc = reserve(need)) {
+            cudaFree(old);
+            return rc;
+        }
+        if (old && keep) KC_CUDA_I(cudaMemcpyAsync(p, old, std::min(keep, old_cap), cudaMemcpyDeviceToDevice, s));
+        KC_CUDA_I(cudaStreamSynchronize(s));
+        if (old) cudaFree(old);
+        return KC_OK;
+    }
     template <typename T>
     T *as() const { return static_cast<T *>(p); }
 };
@@ -75,7 +91,8 @@ struct Worker {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[7] = {};
     DBuf text, off, fcount, slot, status, vbase, xbase, counters, toks, fdesc, piece_c, piece_l, vcells, xcells, win, vmeta, xvalue, xmeta,
-        len_c, len_l, out_c, out_l, scan_tmp, mcount, scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, gpos, seq, vrec, vweight;
+        len_c, len_l, out_c, out_l, scan_tmp, mcount, scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, gpos, seq, vrec, vweight,
+        pend, plist, ucand, ubase, usize, utok, unode, umap;
     PBuf h_small;  // totals and counters (pinned so the small D2H copies are asynchronous)
     PBuf h_scan;   // the scanned record offsets and the statuses of a chunk
     bool busy = false;
@@ -185,10 +202,92 @@ struct ChunkStage {  // per-chunk device-time split (CUDA events on the chunk's 
     float h2d = 0, plan = 0, kernels = 0, emit = 0, d2h = 0;
 };
 
+// The union round of a chunk whose A1 sent P records to it (kc_jsongpu.cuh, U1-U3): U1 counts the candidates' tokens and
+// reserves scratch, U2 builds the union trees and reserves union rows behind the first round's T slots, U3 writes the tables
+// and runs A1's phases on them.  Two read-backs size the scratch and the rows; the arrays A1 has already written grow with
+// their contents kept.  On return T counts the union rows too, and h_cnt[0..2] the chunk's groups.
+int union_round(Worker &w, Chunk &ch, int64_t P, size_t &T, int team, int grid, bool weighted, unsigned long long *h_cnt) {
+    cudaStream_t s = w.stream;
+    const int32_t n = ch.n;
+    int rc;
+#define R_(call)          \
+    do {                  \
+        rc = (call);      \
+        if (rc) return rc; \
+    } while (0)
+    R_(w.ucand.reserve((size_t)P * n * 4));
+    R_(w.ubase.reserve((size_t)P * 4));
+    R_(w.usize.reserve((size_t)P * 4));
+    ch.ucand = w.ucand.as<uint32_t>();
+    ch.ubase = w.ubase.as<uint32_t>();
+    ch.usize = w.usize.as<uint32_t>();
+    ch.uslot = (uint32_t)T;
+    kc::js::union_count_kernel<<<grid, 128, 0, s>>>(ch, team, (int32_t)P);
+    KC_CUDA_I(cudaGetLastError());
+    KC_CUDA_I(cudaMemcpyAsync(h_cnt, ch.counters, 48, cudaMemcpyDeviceToHost, s));
+    KC_CUDA_I(cudaStreamSynchronize(s));
+    const size_t S = std::max<size_t>(h_cnt[4], 1);  // scratch entries: tokens of the candidates, plus a root per record
+    if (S >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: %zu union scratch entries in one chunk", S);
+    R_(w.utok.reserve(S * sizeof(Tok)));
+    R_(w.unode.reserve(S * sizeof(kc::js::UNode)));
+    R_(w.umap.reserve(S * 4));
+    ch.utok = w.utok.as<Tok>();
+    ch.unode = w.unode.as<kc::js::UNode>();
+    ch.umap = w.umap.as<int32_t>();
+    kc::js::union_build_kernel<<<grid, 128, 0, s>>>(ch, team, (int32_t)P);
+    KC_CUDA_I(cudaGetLastError());
+    KC_CUDA_I(cudaMemcpyAsync(h_cnt, ch.counters, 48, cudaMemcpyDeviceToHost, s));
+    KC_CUDA_I(cudaStreamSynchronize(s));
+    const size_t U = h_cnt[5];
+    if (U) {
+        const size_t T1 = T + U, Tn = T * (size_t)n, T1n = T1 * (size_t)n;
+        if (T1 >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: %zu field slots in one chunk", T1);
+        R_(w.toks.grow(T1n * sizeof(Tok), Tn * sizeof(Tok), s));
+        R_(w.fdesc.grow(T1 * 4, T * 4, s));
+        R_(w.gpos.grow(T1 * 4, T * 4, s));
+        R_(w.piece_c.grow(T1 * 4, T * 4, s));
+        R_(w.piece_l.grow(T1 * 4, T * 4, s));
+        R_(w.vcells.grow(T1n, Tn, s));
+        R_(w.xcells.grow(T1n * 8, Tn * 8, s));
+        R_(w.win.reserve(T1 * 4));
+        R_(w.vmeta.reserve(T1 * 4));
+        R_(w.xvalue.reserve(T1 * 8));
+        R_(w.xmeta.reserve(T1 * 4));
+        ch.toks = w.toks.as<Tok>();
+        ch.fdesc = w.fdesc.as<uint32_t>();
+        ch.gpos = w.gpos.as<uint32_t>();
+        ch.piece_c = w.piece_c.as<uint32_t>();
+        ch.piece_l = w.piece_l.as<uint32_t>();
+        ch.vcells = w.vcells.as<int8_t>();
+        ch.xcells = w.xcells.as<double>();
+        ch.vmeta = w.vmeta.as<uint32_t>();
+        ch.xvalue = w.xvalue.as<double>();
+        ch.xmeta = w.xmeta.as<uint32_t>();
+        ch.xbest = w.xmeta.as<int32_t>();
+        ch.xavg = w.xvalue.as<double>();
+        if (weighted) {
+            R_(w.vrec.grow(T1 * 4, T * 4, s));
+            R_(w.vweight.reserve(T1 * 4));
+            ch.vrec = w.vrec.as<int32_t>();
+            ch.vweight = w.vweight.as<float>();
+        }
+        // the union records' rows of the cell matrices get the same defined contents as the first round's
+        KC_CUDA_I(cudaMemsetAsync(ch.vcells + Tn, 0xFF, T1n - Tn, s));
+        KC_CUDA_I(cudaMemsetAsync(ch.xcells + Tn, 0, (T1n - Tn) * 8, s));
+        T = T1;
+    }
+    kc::js::union_plan_kernel<<<grid, 128, 0, s>>>(ch, team, (int32_t)P);
+    KC_CUDA_I(cudaGetLastError());
+    KC_CUDA_I(cudaMemcpyAsync(h_cnt, ch.counters, 48, cudaMemcpyDeviceToHost, s));
+    KC_CUDA_I(cudaStreamSynchronize(s));
+#undef R_
+    return KC_OK;
+}
+
 // One chunk on one worker: records [r0, r1) of the batch.  h_seq (NULL: count votes): the batch's candidate sums [R][n], the
 // vote leaves are likelihood-weighted (K3b over ragged records in K1's place).  xmedoid (KC_JSON_NUMERIC_MEDOID): numeric fields
 // are similarity medoids (K5 in K2's place).
-int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, int64_t r0, int64_t r1, int32_t n,
+int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, bool key_union, int64_t r0, int64_t r1, int32_t n,
               double rel_eps, double abs_eps, int sm_count, kc_json_result &res, ChunkStage &st) {
     const int64_t Rc = r1 - r0;
     const int64_t b0 = h_off[r0 * n], b1 = h_off[r1 * n];
@@ -207,15 +306,17 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     R_(w.slot.reserve((size_t)(Rc + 1) * 4));
     R_(w.status.reserve((size_t)Rc));
     R_(w.nest.reserve((size_t)Rc));
+    R_(w.pend.reserve((size_t)Rc));
+    R_(w.plist.reserve((size_t)Rc * 4));
     R_(w.vbase.reserve((size_t)Rc * 4));
     R_(w.xbase.reserve((size_t)Rc * 4));
-    R_(w.counters.reserve(32));
+    R_(w.counters.reserve(48));
     R_(w.mcount.reserve((size_t)(Rc + 1) * 4));
     R_(w.scount.reserve((size_t)(Rc + 1) * 4));
     R_(w.ccount.reserve((size_t)(Rc + 1) * 4));
     R_(w.len_c.reserve((size_t)(Rc + 1) * 8));
     R_(w.len_l.reserve((size_t)(Rc + 1) * 8));
-    R_(w.h_small.reserve(64));
+    R_(w.h_small.reserve(64));  // the slot total, then the six counters
     R_(w.h_scan.reserve((size_t)(Rc + 1) * 16 + (size_t)Rc));
     if (h_seq) R_(w.seq.reserve((size_t)std::max<int64_t>(Rc * n, 1) * 4));
     size_t tmp_bytes = 0, tmp_bytes32 = 0;
@@ -232,6 +333,8 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     ch.slot = w.slot.as<uint32_t>();
     ch.status = w.status.as<uint8_t>();
     ch.nest = w.nest.as<uint8_t>();
+    ch.pend = w.pend.as<uint8_t>();
+    ch.plist = w.plist.as<int32_t>();
     ch.vbase = w.vbase.as<uint32_t>();
     ch.xbase = w.xbase.as<uint32_t>();
     ch.counters = w.counters.as<unsigned long long>();
@@ -241,6 +344,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     ch.len_c = w.len_c.as<int64_t>();
     ch.len_l = w.len_l.as<int64_t>();
     ch.xmedoid = xmedoid;
+    ch.key_union = key_union;
 
     nvtxRangePushA("kc_json: H2D texts");
     KC_CUDA_I(cudaEventRecord(w.ev[0], s));
@@ -266,8 +370,8 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     uint32_t *h_total = w.h_small.as<uint32_t>();
     KC_CUDA_I(cudaMemcpyAsync(h_total, ch.slot + Rc, 4, cudaMemcpyDeviceToHost, s));
     KC_CUDA_I(cudaStreamSynchronize(s));
-    const size_t T = *h_total;  // field slots of the chunk
-    const size_t Tn = T * (size_t)n;
+    size_t T = *h_total;  // field slots of the chunk (after a union round: its rows too)
+    size_t Tn = T * (size_t)n;
     R_(w.toks.reserve(std::max<size_t>(Tn, 1) * sizeof(Tok)));
     R_(w.fdesc.reserve(std::max<size_t>(T, 1) * 4));
     R_(w.gpos.reserve(std::max<size_t>(T, 1) * 4));
@@ -297,7 +401,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
         ch.vrec = w.vrec.as<int32_t>();
         ch.vweight = w.vweight.as<float>();
     }
-    KC_CUDA_I(cudaMemsetAsync(w.counters.p, 0, 24, s));
+    KC_CUDA_I(cudaMemsetAsync(w.counters.p, 0, 48, s));
     // records declined before slots_phase own no medoid groups
     KC_CUDA_I(cudaMemsetAsync(w.mcount.p, 0, (size_t)(Rc + 1) * 4, s));
     KC_CUDA_I(cudaMemsetAsync(w.scount.p, 0, (size_t)(Rc + 1) * 4, s));
@@ -311,8 +415,12 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
         kc::js::plan_kernel<<<grid_for(rounds * 32), 128, 0, s>>>(ch, team);
         KC_CUDA_I(cudaGetLastError());
         unsigned long long *h_cnt = w.h_small.as<unsigned long long>() + 1;
-        KC_CUDA_I(cudaMemcpyAsync(h_cnt, w.counters.p, 24, cudaMemcpyDeviceToHost, s));
+        KC_CUDA_I(cudaMemcpyAsync(h_cnt, w.counters.p, 32, cudaMemcpyDeviceToHost, s));
         KC_CUDA_I(cudaStreamSynchronize(s));
+        if (const int64_t P = (int64_t)h_cnt[3]) {  // records whose candidates differ in shape
+            R_(union_round(w, ch, P, T, team, grid_for((P + tpw - 1) / tpw * 32), h_seq != nullptr, h_cnt));
+            Tn = T * (size_t)n;
+        }
         gv = (int64_t)h_cnt[0];
         gx = (int64_t)h_cnt[1];
         gm = (int64_t)h_cnt[2];
@@ -501,7 +609,7 @@ int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_
         while (!rc) {
             const int k = next.fetch_add(1);
             if (k >= n_chunks) break;
-            rc = run_chunk(w, h_text, h_off, h_seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps,
+            rc = run_chunk(w, h_text, h_off, h_seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, (flags & KC_JSON_KEY_UNION) != 0, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps,
                            abs_eps, sm_count, *res, stages[(size_t)wi]);
         }
         if (rc) {
@@ -648,9 +756,13 @@ struct kc_debug_jsongpu {
     int32_t n = 0;
     int64_t R = 0;
     std::vector<uint32_t> fcount, slot, fdesc, gpos, vbase, xbase, piece_c, piece_l;
-    std::vector<uint8_t> status, nest;
+    std::vector<uint8_t> status, nest, pend;
     std::vector<Tok> toks;
-    unsigned long long counters[3] = {0, 0, 0};
+    unsigned long long counters[6] = {0, 0, 0, 0, 0, 0};
+    std::vector<int32_t> plist, umap;
+    std::vector<uint32_t> ucand, ubase, usize;
+    std::vector<Tok> utok;
+    std::vector<kc::js::UNode> unode;
     std::vector<uint32_t> mcount, scount, ccount;
     std::vector<uint8_t> mchars;
     std::vector<int32_t> mstr_off, mgrp_off;
@@ -679,6 +791,8 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     h->slot.assign((size_t)R + 1, 0);
     h->status.assign((size_t)R, 0);
     h->nest.assign((size_t)R, 0);
+    h->pend.assign((size_t)R, 0);
+    h->plist.assign((size_t)R + 1, -1);
     h->vbase.assign((size_t)R, 0);
     h->xbase.assign((size_t)R, 0);
     h->len_c.assign((size_t)R + 1, 0);
@@ -695,6 +809,8 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     ch.slot = h->slot.data();
     ch.status = h->status.data();
     ch.nest = h->nest.data();
+    ch.pend = h->pend.data();
+    ch.plist = h->plist.data();
     ch.vbase = h->vbase.data();
     ch.xbase = h->xbase.data();
     ch.counters = h->counters;
@@ -704,6 +820,7 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     ch.len_c = h->len_c.data();
     ch.len_l = h->len_l.data();
     ch.xmedoid = (flags & KC_JSON_NUMERIC_MEDOID) != 0;
+    ch.key_union = (flags & KC_JSON_KEY_UNION) != 0;
     for (int32_t r = 0; r < R; ++r) kc::js::count_record(ch, r);
     for (int64_t r = 0; r < R; ++r) h->slot[(size_t)r + 1] = h->slot[(size_t)r] + h->fcount[(size_t)r];
     const size_t T = h->slot[(size_t)R];
@@ -728,8 +845,58 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
         for (int lane = 0; lane < team; ++lane) kc::js::parse_phase(ch, r, lane, team);
         for (int lane = 0; lane < team; ++lane) kc::js::type_phase(ch, r, lane, team);
         for (int lane = 0; lane < team; ++lane) kc::js::order_phase(ch, r, lane, team);
-        kc::js::slots_phase(ch, r);
+        kc::js::slots_phase(ch, r, true);
         for (int lane = 0; lane < team; ++lane) kc::js::encode_phase(ch, r, lane, team);
+    }
+    if (const int64_t P = (int64_t)h->counters[3]) {  // the union round, as run_chunk / union_round run it
+        h->ucand.assign((size_t)(P * n), 0);
+        h->ubase.assign((size_t)P, 0);
+        h->usize.assign((size_t)P, 0);
+        ch.ucand = h->ucand.data();
+        ch.ubase = h->ubase.data();
+        ch.usize = h->usize.data();
+        ch.uslot = (uint32_t)T;
+        for (int32_t p = 0; p < P; ++p) {
+            for (int lane = 0; lane < team; ++lane) kc::js::union_count_phase(ch, p, lane, team);
+            kc::js::union_reserve(ch, p);
+        }
+        const size_t S = std::max<size_t>(h->counters[4], 1);
+        h->utok.assign(S, Tok{});
+        h->unode.assign(S, kc::js::UNode{});
+        h->umap.assign(S, -1);
+        ch.utok = h->utok.data();
+        ch.unode = h->unode.data();
+        ch.umap = h->umap.data();
+        for (int32_t p = 0; p < P; ++p) {
+            for (int lane = 0; lane < team; ++lane) kc::js::union_scan_phase(ch, p, lane, team);
+            kc::js::union_build(ch, p);
+        }
+        const size_t T1 = T + (size_t)h->counters[5];
+        h->toks.resize(std::max<size_t>(T1 * n, 1), Tok{});
+        h->fdesc.resize(std::max<size_t>(T1, 1), 0);
+        h->gpos.resize(std::max<size_t>(T1, 1), 0);
+        h->piece_c.resize(std::max<size_t>(T1, 1), 0);
+        h->piece_l.resize(std::max<size_t>(T1, 1), 0);
+        h->vcells.resize(std::max<size_t>(T1 * n, 16), (int8_t)-1);
+        h->vrec.resize(std::max<size_t>(T1, 1), -1);
+        h->xcells.resize(std::max<size_t>(T1 * n, 2), 0.0);
+        ch.toks = h->toks.data();
+        ch.fdesc = h->fdesc.data();
+        ch.gpos = h->gpos.data();
+        ch.piece_c = h->piece_c.data();
+        ch.piece_l = h->piece_l.data();
+        ch.vcells = h->vcells.data();
+        ch.vrec = h->vrec.data();
+        ch.xcells = h->xcells.data();
+        for (int32_t p = 0; p < P; ++p) {
+            const int32_t r = h->plist[(size_t)p];
+            for (int lane = 0; lane < team; ++lane) kc::js::union_write_phase(ch, p, lane, team);
+            if (h->status[(size_t)r] == kc::js::D_UNION) h->status[(size_t)r] = 0;
+            for (int lane = 0; lane < team; ++lane) kc::js::type_phase(ch, r, lane, team);
+            for (int lane = 0; lane < team; ++lane) kc::js::order_phase(ch, r, lane, team);
+            kc::js::slots_phase(ch, r, false);
+            for (int lane = 0; lane < team; ++lane) kc::js::encode_phase(ch, r, lane, team);
+        }
     }
     for (std::vector<uint32_t> *cnt : {&h->mcount, &h->scount, &h->ccount}) {  // exclusive scans, in place
         uint32_t acc = 0;

@@ -16,6 +16,14 @@
 //         order   nested records: the token's position in output order (depth-first, keys sorted at every level)
 //         slots   the team leader numbers the record's vote / numeric groups and reserves rows in the batch's cell matrices
 //         encode  lane j: sanitised-equality classes -> int8 local codes (K1 cells), exact decimal -> float64 (K2 cells)
+//   U1-U3 only under KC_JSON_KEY_UNION and when A1 found records whose candidates differ in SHAPE (keys in another order,
+//         missing or extra keys, None or nothing where another candidate holds a sub-object): the key-union round, a team per
+//         such record (without the flag A1 declines them)
+//     U1  union_count_kernel   lane c counts candidate c's tokens; the leader reserves scratch        (read-back: scratch size)
+//     U2  union_build_kernel   lane c scans candidate c into scratch; the leader builds the union tree (one node per key path,
+//                              duplicate keys and object-against-value declined) and reserves its rows  (read-back: union rows)
+//     U3  union_plan_kernel    lane c writes column c of the [union rows x n] table (synthetic K_NULL / K_OPEN..K_CLOSE where
+//                              candidate c lacks the key or holds None), then type / order / slots / encode run on it as in A1
 //   A2  medoid_kernel   only when the chunk has multi-word string fields (three exclusive scans of the per-record counts first):
 //                       lane j writes its field's normalised strings and their offsets in K4's CSR form
 //   K1  kc_vote_i8, K2  kc_numeric_f64, K4  kc_medoid_str on the cell matrices / string groups — the kernels of the columnar path
@@ -23,8 +31,9 @@
 //                       leader turns them into piece offsets and record lengths          (then two exclusive scans: offsets)
 //   C1  write_kernel    lane j writes `"key": value` / `"key": confidence` at its offset of the two output blobs
 //
-// A record the device path does not model exactly (\u escapes, escapes in keys, non-ASCII, nested values or lists, candidates with different
-// keys, multi-word strings outside K4's contract, numbers outside the exact-conversion range, ...) gets a non-zero status and is
+// A record the device path does not model exactly (\u escapes, escapes in keys, non-ASCII, lists, empty objects, an object in one
+// candidate against a value in another, candidates of different shapes without KC_JSON_KEY_UNION, multi-word strings outside
+// K4's contract, numbers outside the exact-conversion range, ...) gets a non-zero status and is
 // consolidated by the host path (kc_consolidate_json) instead: the device path never guesses.
 //
 // The phases are plain __host__ __device__ functions of (chunk, record, lane, team size) that communicate through global
@@ -37,6 +46,23 @@ namespace kc {
 namespace js {
 
 constexpr int32_t kMaxFields = 1024;  // per record; the key ranking is quadratic in it
+
+// status of a record between A1 and the union round (U1-U3): its candidates differ in shape.  Internal: the union round turns
+// it into 0 or a D_* code before anything reads the statuses back.
+constexpr uint8_t D_UNION = 0xFF;
+
+// A node of a record's key-union tree (union round): one key path.  Indices are relative to the record's scratch region;
+// node 0 is the top-level object.
+struct UNode {
+    uint32_t kstart;           // key span of the first candidate that has the key
+    uint16_t klen;
+    uint8_t depth;
+    uint8_t obj;               // an object in some candidate
+    uint8_t scalar;            // a non-null scalar in some candidate
+    int32_t parent, child, last, next;  // tree links, -1 = none; members in order of first appearance
+    int32_t lastc;             // the last candidate that has the key (a second hit from the same one is a duplicate key)
+    uint32_t row, close;       // its row in the union table; an object's K_CLOSE row (the root: the node count in `row`)
+};
 
 // field descriptor word: kind:3 | last of its siblings in key order:1 | rank among its siblings:12 | group index within the record:16
 KC_HD inline uint32_t fdesc_pack(uint32_t kind, uint32_t last, uint32_t rank, uint32_t gidx) { return kind | (last << 3) | (rank << 4) | (gidx << 16); }
@@ -79,10 +105,31 @@ struct Chunk {
     uint32_t *piece_c, *piece_l;  // [slots] by (slot + rank): piece length, then (after the leader's pass) piece offset
     int64_t *len_c, *len_l;       // [R+1] record lengths -> (exclusive scan, in place) record offsets in the output blobs
     uint8_t *out_c, *out_l;       // output blobs: consensus texts, likelihoods texts
+    // the union round: records whose candidates differ in shape (key order, missing keys, null sub-objects), rebuilt as
+    // [union rows x n] tables behind the first round's slots; counters [3] records, [4] scratch entries, [5] union rows
+    uint8_t *pend;      // [R]   A1: a candidate's token count or a row's key / depth / structure differs from candidate 0's
+    int32_t *plist;     // [R]   the records sent to the union round (chunk-local)
+    uint32_t *ucand;    // [P*n] U1: candidate c's token count -> its first entry in the record's scratch region
+    uint32_t *ubase;    // [P]   the record's scratch region
+    uint32_t *usize;    // [P]   its size
+    Tok *utok;          // [scratch] the candidates' tokens, back to back
+    UNode *unode;       // [scratch] the union tree
+    int32_t *umap;      // [scratch] token -> node (-1: a K_CLOSE)
+    uint32_t uslot;     // the first round's slot total: union rows are numbered from here
+    bool key_union;     // KC_JSON_KEY_UNION: such records go to the union round; without it A1 declines them as the reason says
 };
 
 KC_HD inline uint8_t load_status(const Chunk &ch, int32_t r) { return *(volatile const uint8_t *)(ch.status + r); }
 KC_HD inline void decline(const Chunk &ch, int32_t r, int32_t why) { *(volatile uint8_t *)(ch.status + r) = (uint8_t)why; }
+// the candidates differ in shape (`why`: how A1 sees it): with KC_JSON_KEY_UNION the union round decides the record
+// (D_KEYS_DIFFER keeps the later phases off it until then), else it is declined
+KC_HD inline void differ(const Chunk &ch, int32_t r, int32_t why) {
+    if (ch.key_union) {
+        *(volatile uint8_t *)(ch.pend + r) = 1;
+        why = D_KEYS_DIFFER;
+    }
+    decline(ch, r, why);
+}
 
 // ---------------------------------------------------------------- A0
 
@@ -93,6 +140,7 @@ KC_HD inline void count_record(const Chunk &ch, int32_t r) {
     if (e - b < ((int64_t)1 << 31)) f = scan_object(ch.text + (b - ch.off[0]), (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, &nested);
     ch.fcount[r] = f > 0 ? (uint32_t)f : 0u;
     ch.nest[r] = nested ? 1 : 0;
+    ch.pend[r] = 0;
     ch.status[r] = f > 0 ? (uint8_t)D_OK : (uint8_t)(-f);
 }
 
@@ -107,8 +155,8 @@ KC_HD inline void parse_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t 
         int32_t f = -D_TOO_LONG;
         if (e - b < ((int64_t)1 << 31) && (b - base0) + (e - b) < ((int64_t)1 << 32))
             f = scan_object(ch.text + (b - base0), (uint32_t)(e - b), (uint32_t)(b - base0), ch.toks + (int64_t)ch.slot[r] * ch.n + c, ch.n, F);
-        if (f < 0) decline(ch, r, f == -D_TOO_MANY_FIELDS ? D_KEYS_DIFFER : -f);
-        else if (f != F) decline(ch, r, D_KEYS_DIFFER);
+        if (f == -D_TOO_MANY_FIELDS || (f >= 0 && f != F)) differ(ch, r, D_KEYS_DIFFER);  // more or fewer tokens than candidate 0
+        else if (f < 0) decline(ch, r, -f);
     }
 }
 
@@ -133,12 +181,13 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
         const Tok *row = rt + (int64_t)j * n;
         const uint32_t k0 = row[0].kind, d = tok_depth(row[0]);
         // the same SHAPE in every candidate: the same key at position j, nested objects open and close at the same positions
-        // (else the key union / missing -> None / None -> dict of Nones logic of the pre-pass is the host path's, cu:516-548)
+        // (else, with KC_JSON_KEY_UNION, the union round applies the pre-pass's key union / missing -> None / None -> dict of
+        // Nones, cu:516-548; it also tells an object against a non-null value, D_NESTED, from a row that is only out of step)
         int32_t ref = j;  // the token whose key orders this one among its siblings: itself, or a K_CLOSE's K_OPEN
         if (k0 == K_CLOSE) {
             for (int32_t c = 1; c < n; ++c)
                 if (row[c].kind != K_CLOSE || tok_depth(row[c]) != d) {
-                    decline(ch, r, D_KEYS_DIFFER);
+                    differ(ch, r, D_KEYS_DIFFER);
                     return;
                 }
             ref = j - 1;  // its K_OPEN: the nearest token to the left at the same depth (everything between them is deeper)
@@ -149,11 +198,11 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
         if (k0 != K_CLOSE) {
             for (int32_t c = 1; c < n; ++c) {
                 if ((row[c].kind == K_OPEN) != (k0 == K_OPEN) || row[c].kind == K_CLOSE) {  // an object here, a scalar / None there
-                    decline(ch, r, D_NESTED);
+                    differ(ch, r, D_NESTED);
                     return;
                 }
                 if (tok_depth(row[c]) != d || row[c].klen != klen || key_compare(ch.text + row[c].kstart, klen, key, klen) != 0) {
-                    decline(ch, r, D_KEYS_DIFFER);
+                    differ(ch, r, D_KEYS_DIFFER);
                     return;
                 }
             }
@@ -289,9 +338,20 @@ KC_HD inline uint32_t out_pos(const Chunk &ch, int32_t r, int32_t j) {
     return ch.nest[r] ? ch.gpos[ch.slot[r] + j] : fdesc_rank(ch.fdesc[ch.slot[r] + j]);
 }
 
-// team leader only: number the groups, reserve rows of the cell matrices (chunk-wide counters)
-KC_HD inline void slots_phase(const Chunk &ch, int32_t r) {
-    if (load_status(ch, r)) return;
+// team leader only: number the groups, reserve rows of the cell matrices (chunk-wide counters).  First round: a record whose
+// candidates differ in shape goes to the union round, whatever else A1 found (the union round scans and checks it afresh).
+KC_HD inline void slots_phase(const Chunk &ch, int32_t r, bool first_round) {
+    if (load_status(ch, r)) {
+        if (first_round && ch.pend[r]) {
+            decline(ch, r, D_UNION);
+#ifdef __CUDA_ARCH__
+            ch.plist[atomicAdd(ch.counters + 3, 1ull)] = r;
+#else
+            ch.plist[ch.counters[3]++] = r;
+#endif
+        }
+        return;
+    }
     const int32_t F = (int32_t)ch.fcount[r];
     uint32_t *fd = ch.fdesc + ch.slot[r];
     uint32_t nv = 0, nx = 0, nm = 0, ns = 0, nc = 0;
@@ -408,6 +468,199 @@ KC_HD inline void encode_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t
                 }
                 cells[c] = v;
             }
+        }
+    }
+}
+
+// ---------------------------------------------------------------- U1 - U3: the key-union round
+//
+// Record p of the round is plist[p].  After the pre-pass (cu:516-548) a missing key is an explicit None and a None (or missing)
+// sub-object is an object of Nones at every level, so a record whose candidates differ in shape becomes a table of one shape:
+// one row per key path of the union (depth-first, members in order of first appearance), a synthetic K_NULL where a candidate
+// lacks the leaf, a synthetic K_OPEN / K_NULL... / K_CLOSE subtree where it lacks the object or holds None.  A1's type / order /
+// slots / encode phases then run on that table unchanged.
+
+KC_HD inline bool candidate_span(const Chunk &ch, int32_t r, int32_t c, int64_t &b, int64_t &len) {
+    const int64_t base0 = ch.off[0];
+    b = ch.off[(int64_t)r * ch.n + c] - base0;
+    len = ch.off[(int64_t)r * ch.n + c + 1] - base0 - b;
+    return len < ((int64_t)1 << 31) && b + len < ((int64_t)1 << 32);
+}
+
+// U1: lane c counts candidate c's tokens (scanning it afresh finds every scan-level reason to decline the record)
+KC_HD inline void union_count_phase(const Chunk &ch, int32_t p, int32_t lane, int32_t team) {
+    const int32_t r = ch.plist[p];
+    for (int32_t c = lane; c < ch.n; c += team) {
+        int64_t b, len;
+        int32_t f = -D_TOO_LONG;
+        if (candidate_span(ch, r, c, b, len)) f = scan_object(ch.text + b, (uint32_t)len, 0, nullptr, 0, kMaxFields);
+        if (f < 0) decline(ch, r, f == -D_TOO_MANY_FIELDS ? D_KEYS_DIFFER : -f);  // one candidate alone is over the union's limit
+        ch.ucand[(int64_t)p * ch.n + c] = f > 0 ? (uint32_t)f : 0u;
+    }
+}
+
+// U1, team leader: counts -> the candidates' first entries in the record's scratch region (entry 0: the root node), reserved
+// from the chunk-wide counter
+KC_HD inline void union_reserve(const Chunk &ch, int32_t p) {
+    uint32_t *cand = ch.ucand + (int64_t)p * ch.n;
+    uint32_t s = 1;
+    for (int32_t c = 0; c < ch.n; ++c) {
+        const uint32_t f = cand[c];
+        cand[c] = s;
+        s += f;
+    }
+    if (load_status(ch, ch.plist[p]) != D_UNION) s = 0;
+    ch.usize[p] = s;
+#ifdef __CUDA_ARCH__
+    ch.ubase[p] = (uint32_t)atomicAdd(ch.counters + 4, (unsigned long long)s);
+#else
+    ch.ubase[p] = (uint32_t)ch.counters[4];
+    ch.counters[4] += s;
+#endif
+}
+
+// U2: lane c scans candidate c into the scratch region
+KC_HD inline void union_scan_phase(const Chunk &ch, int32_t p, int32_t lane, int32_t team) {
+    const int32_t r = ch.plist[p];
+    if (load_status(ch, r) != D_UNION) return;
+    for (int32_t c = lane; c < ch.n; c += team) {
+        int64_t b, len;
+        candidate_span(ch, r, c, b, len);  // U1 checked it
+        scan_object(ch.text + b, (uint32_t)len, (uint32_t)b, ch.utok + ch.ubase[p] + ch.ucand[(int64_t)p * ch.n + c], 1, kMaxFields);
+    }
+}
+
+KC_HD inline bool same_key(const Chunk &ch, const UNode &u, const Tok &t) {
+    return u.klen == t.klen && key_compare(ch.text + u.kstart, u.klen, ch.text + t.kstart, t.klen) == 0;
+}
+
+// U2, team leader: the union tree, candidate by candidate.  A token's node is probed at the same position of the previous
+// candidate, then after the node of its previous sibling, before the parent's members are searched: a reordered or one-key-
+// short record costs about one more pass over its tokens.  Then the rows (depth-first) and the record's union slots.
+KC_HD inline void union_build(const Chunk &ch, int32_t p) {
+    const int32_t r = ch.plist[p], n = ch.n;
+    if (load_status(ch, r) != D_UNION) return;
+    const uint32_t base = ch.ubase[p], total = ch.usize[p];
+    const uint32_t *cand = ch.ucand + (int64_t)p * n;
+    const Tok *tk = ch.utok + base;
+    UNode *nd = ch.unode + base;
+    int32_t *map = ch.umap + base;
+    nd[0] = UNode{0, 0, 0, 1, 0, -1, -1, -1, -1, -1, 0, 0};
+    int32_t nn = 1;
+    for (int32_t c = 0; c < n; ++c) {
+        int32_t par[kMaxNesting + 2], sib[kMaxNesting + 2];  // per depth: the parent node, the node of the previous member
+        par[0] = 0;
+        sib[0] = -1;
+        const uint32_t b = cand[c], e = c + 1 < n ? cand[c + 1] : total, pb = c ? cand[c - 1] : 0u;
+        for (uint32_t i = b; i < e; ++i) {
+            const Tok &t = tk[i];
+            map[i] = -1;
+            if (t.kind == K_CLOSE) continue;
+            const uint32_t d = tok_depth(t);
+            const int32_t P = par[d];
+            int32_t u = -1;
+            if (c > 0 && pb + (i - b) < b) {
+                const int32_t v = map[pb + (i - b)];
+                if (v > 0 && nd[v].parent == P && same_key(ch, nd[v], t)) u = v;
+            }
+            if (u < 0 && sib[d] > 0) {
+                const int32_t v = nd[sib[d]].next;
+                if (v > 0 && same_key(ch, nd[v], t)) u = v;
+            }
+            for (int32_t v = u < 0 ? nd[P].child : -1; v > 0; v = nd[v].next)
+                if (same_key(ch, nd[v], t)) {
+                    u = v;
+                    break;
+                }
+            if (u < 0) {
+                u = nn++;
+                nd[u] = UNode{t.kstart, t.klen, (uint8_t)d, 0, 0, P, -1, -1, -1, -1, 0, 0};
+                if (nd[P].last >= 0) nd[nd[P].last].next = u;
+                else nd[P].child = u;
+                nd[P].last = u;
+            } else if (nd[u].lastc == c) {  // dict semantics would keep the last one: host path
+                decline(ch, r, D_DUP_KEY);
+                return;
+            }
+            nd[u].lastc = c;
+            map[i] = u;
+            if (t.kind == K_OPEN) {
+                nd[u].obj = 1;
+                par[d + 1] = u;
+                sib[d + 1] = -1;
+            } else if (t.kind != K_NULL) {
+                nd[u].scalar = 1;
+            }
+            if (nd[u].obj && nd[u].scalar) {  // an object against a non-null value: the pre-pass leaves the values alone (cu:507-512)
+                decline(ch, r, D_NESTED);
+                return;
+            }
+            sib[d] = u;
+        }
+    }
+    uint32_t rows = 0;
+    uint8_t nested = 0;
+    for (int32_t u = nd[0].child; u > 0;) {  // depth-first: an object's K_OPEN row, its members, its K_CLOSE row
+        nd[u].row = rows++;
+        nested |= nd[u].obj;
+        if (nd[u].obj) {  // every object has a member: the scanner declines empty ones
+            u = nd[u].child;
+            continue;
+        }
+        while (u > 0 && nd[u].next < 0) {
+            u = nd[u].parent;
+            if (u > 0) nd[u].close = rows++;
+        }
+        if (u > 0) u = nd[u].next;
+    }
+    if (rows > (uint32_t)kMaxFields) {
+        decline(ch, r, D_KEYS_DIFFER);
+        return;
+    }
+    nd[0].row = (uint32_t)nn;
+    ch.fcount[r] = rows;
+    ch.nest[r] = nested;
+#ifdef __CUDA_ARCH__
+    ch.slot[r] = ch.uslot + (uint32_t)atomicAdd(ch.counters + 5, (unsigned long long)rows);
+#else
+    ch.slot[r] = ch.uslot + (uint32_t)ch.counters[5];
+    ch.counters[5] += rows;
+#endif
+}
+
+// U3: lane c writes column c of the [rows x n] table: synthetic tokens under every node (keyed like the node, so row 0 carries
+// the key even where candidate 0 lacks it), then the candidate's own tokens over them (not its None where the node is an object)
+KC_HD inline void union_write_phase(const Chunk &ch, int32_t p, int32_t lane, int32_t team) {
+    const int32_t r = ch.plist[p], n = ch.n;
+    if (load_status(ch, r) != D_UNION) return;
+    const uint32_t base = ch.ubase[p];
+    const uint32_t *cand = ch.ucand + (int64_t)p * n;
+    const Tok *tk = ch.utok + base;
+    const UNode *nd = ch.unode + base;
+    const int32_t nn = (int32_t)nd[0].row;
+    const int32_t *map = ch.umap + base;
+    Tok *tab = ch.toks + (int64_t)ch.slot[r] * n;
+    for (int32_t c = lane; c < n; c += team) {
+        for (int32_t u = 1; u < nn; ++u) {
+            Tok s;
+            s.vstart = nd[u].kstart;
+            s.vlen = 0;
+            s.kstart = nd[u].kstart;
+            s.klen = nd[u].klen;
+            s.kind = nd[u].obj ? K_OPEN : K_NULL;
+            s.flags = (uint8_t)(nd[u].depth << 4);
+            tab[(int64_t)nd[u].row * n + c] = s;
+            if (nd[u].obj) {
+                s.kind = K_CLOSE;
+                s.klen = 0;
+                tab[(int64_t)nd[u].close * n + c] = s;
+            }
+        }
+        const uint32_t e = c + 1 < n ? cand[c + 1] : ch.usize[p];
+        for (uint32_t i = cand[c]; i < e; ++i) {
+            const int32_t u = map[i];
+            if (u < 0 || (nd[u].obj && tk[i].kind != K_OPEN)) continue;
+            tab[(int64_t)nd[u].row * n + c] = tk[i];
         }
     }
 }
@@ -609,7 +862,58 @@ __global__ void __launch_bounds__(128) plan_kernel(const Chunk ch, int32_t team)
         __syncwarp();
         if (live) order_phase(ch, r, lane, team);  // nested records only; reads the ranks its team wrote
         __syncwarp();
-        if (live && lane == 0) slots_phase(ch, r);
+        if (live && lane == 0) slots_phase(ch, r, true);
+        __syncwarp();
+        if (live) encode_phase(ch, r, lane, team);
+        __syncwarp();
+    }
+}
+
+// The union round: team t of a warp owns the round's record p = warp_index * teams_per_warp + t, as in plan_kernel.
+__global__ void __launch_bounds__(128) union_count_kernel(const Chunk ch, int32_t team, int32_t P) {
+    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
+    const int32_t lane = lane_w % team, t = lane_w / team;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t w = warp; w < ((int64_t)P + tpw - 1) / tpw; w += n_warps) {
+        const int64_t p = w * tpw + t;
+        if (p < P) union_count_phase(ch, (int32_t)p, lane, team);
+        __syncwarp();
+        if (p < P && lane == 0) union_reserve(ch, (int32_t)p);
+        __syncwarp();
+    }
+}
+
+__global__ void __launch_bounds__(128) union_build_kernel(const Chunk ch, int32_t team, int32_t P) {
+    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
+    const int32_t lane = lane_w % team, t = lane_w / team;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t w = warp; w < ((int64_t)P + tpw - 1) / tpw; w += n_warps) {
+        const int64_t p = w * tpw + t;
+        if (p < P) union_scan_phase(ch, (int32_t)p, lane, team);
+        __syncwarp();
+        if (p < P && lane == 0) union_build(ch, (int32_t)p);
+        __syncwarp();
+    }
+}
+
+// the table, then A1's phases on it (the leader clears the status between the two)
+__global__ void __launch_bounds__(128) union_plan_kernel(const Chunk ch, int32_t team, int32_t P) {
+    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
+    const int32_t lane = lane_w % team, t = lane_w / team;
+    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+    for (int64_t w = warp; w < ((int64_t)P + tpw - 1) / tpw; w += n_warps) {
+        const int64_t p = w * tpw + t;
+        const bool live = p < P;
+        const int32_t r = live ? ch.plist[p] : 0;
+        if (live) union_write_phase(ch, (int32_t)p, lane, team);
+        __syncwarp();
+        if (live && lane == 0 && load_status(ch, r) == D_UNION) decline(ch, r, D_OK);
+        __syncwarp();
+        if (live) type_phase(ch, r, lane, team);
+        __syncwarp();
+        if (live) order_phase(ch, r, lane, team);
+        __syncwarp();
+        if (live && lane == 0) slots_phase(ch, r, false);
         __syncwarp();
         if (live) encode_phase(ch, r, lane, team);
         __syncwarp();

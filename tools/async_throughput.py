@@ -1,7 +1,8 @@
 """The async entry points on the device (KC_JSON_NUMERIC_MEDOID) against the Python async route, and K5 against K2.
 
 1. requests/s and p50 / p99 latency of async_consolidate_parsed_chat_completions at 1, 16 and 256 concurrent requests on one event
-   loop, on S32 texts (SURVEY.md section 8d) at n = 3 and 16: the native route (device JSON path, requests combined per device call)
+   loop, on S32 texts (SURVEY.md section 8d) or (--workload invoice_optional) invoice texts whose candidates reorder, drop and add
+   keys (tools/jsonpacked_throughput.py), at n = 3 and 16: the native route (device JSON path, requests combined per device call)
    against the Python async route (_consensus_async) on the same contents.
 2. kernel time of K5 (kc_numeric_medoid_f64) against K2 (kc_numeric_f64) on the same S32 numeric cells, 1 M records x 8 fields,
    at n = 4, 16, 32, 64 (CUDA events, median of 20 launches).
@@ -27,13 +28,17 @@ async def _no_embeddings(texts):
     raise RuntimeError("no embeddings service in this measurement")
 
 
-def s32_completions(count, n, seed):
+def s32_completions(count, n, seed, workload="s32"):
     from openai.types.chat import ParsedChatCompletion
-    blob, off = K.s32_texts_packed(count, n, seed, pinned=False)
-    raw = bytes(blob[:int(off[-1])])
+    if workload == "invoice_optional":
+        from tools.jsonpacked_throughput import invoice_texts
+        records = invoice_texts(count, n, seed, optional=True)
+    else:
+        blob, off = K.s32_texts_packed(count, n, seed, pinned=False)
+        raw = bytes(blob[:int(off[-1])])
+        records = [[raw[off[r * n + c]:off[r * n + c + 1]].decode("ascii") for c in range(n)] for r in range(count)]
     out = []
-    for r in range(count):
-        texts = [raw[off[r * n + c]:off[r * n + c + 1]].decode("ascii") for c in range(n)]
+    for texts in records:
         out.append(ParsedChatCompletion.model_validate({
             "id": "x", "object": "chat.completion", "created": 0, "model": "m",
             "choices": [{"index": i, "finish_reason": "stop", "message": {"role": "assistant", "content": t}} for i, t in enumerate(texts)]}))
@@ -55,15 +60,15 @@ async def _run(completions, concurrency):
     return time.perf_counter() - t0, lat
 
 
-def requests_rows(card):
+def requests_rows(card, workload="s32"):
     native_route = C._consensus_of_choices_native_async
 
     async def python_only(*a, **k):
         return None
     for n in (3, 16):
-        comps = s32_completions(2048, n, 20261016 + n)
+        comps = s32_completions(2048, n, 20261016 + n, workload)
         for conc in (1, 16, 256):
-            row = {"what": "async_requests", "n": n, "concurrency": conc, "gpu": card}
+            row = {"what": "async_requests", "workload": workload, "n": n, "concurrency": conc, "gpu": card}
             for route in ("python", "native", "python", "native"):  # alternated twice; the faster run of each is reported
                 C._consensus_of_choices_native_async = native_route if route == "native" else python_only
                 count = len(comps) if route == "native" else 256
@@ -103,10 +108,16 @@ def kernel_rows(card):
 
 
 def main():
+    import argparse
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--workload", choices=["s32", "invoice_optional"], default="s32", help="the request rows' candidate texts")
+    ap.add_argument("--requests-only", action="store_true", help="skip the K5 / K2 kernel rows")
+    args = ap.parse_args()
     torch.cuda.set_device(0)
     card = gpu_card()
-    kernel_rows(card)
-    requests_rows(card)
+    if not args.requests_only:
+        kernel_rows(card)
+    requests_rows(card, args.workload)
 
 
 if __name__ == "__main__":

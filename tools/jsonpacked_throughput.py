@@ -10,10 +10,16 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from k_llms_b200 import _native as K  # noqa: E402
 
 
-def invoice_texts(records, n, seed, nested=False):
+# the optional-keys workloads: each candidate independently reorders its keys (at every level), drops one, adds an extra one,
+# and (nested) sets a sub-object to None or leaves it out, with these probabilities
+P_REORDER, P_DROP, P_EXTRA, P_NULL_SUB, P_MISSING_SUB = 0.5, 0.2, 0.2, 0.1, 0.05
+
+
+def invoice_texts(records, n, seed, nested=False, optional=False):
     """An extraction-like schema with FREE-TEXT fields (multi-word strings -> similarity medoid, K4) next to enums, bools and
     numbers: 4 phrases, 3 enums, 2 bools, 3 numbers per record; every candidate copies the record's truth with probability 0.8
-    per field, otherwise a variant (case / punctuation / one word changed / another value), None with probability 0.05."""
+    per field, otherwise a variant (case / punctuation / one word changed / another value), None with probability 0.05.
+    optional: the candidates differ in shape as well (P_* above): the device path's key-union round."""
     import random
     rng = random.Random(seed)
     vendors = ["Acme Industrial Supply Co", "Globex Logistics and Freight", "Initech Software Services Ltd", "Umbrella Medical Devices Inc"]
@@ -59,16 +65,32 @@ def invoice_texts(records, n, seed, nested=False):
                      "payment": {"terms": d["terms"], "status": d["status"], "signed": d["signed"]},
                      "amounts": {"total": d["total"], "tax": d["tax"], "taxable": d["taxable"]},
                      "kind": d["kind"], "note": d["note"], "items": d["items"]}
+            if optional:
+                d = _optional(rng, d, top=True)
             cands.append(json.dumps(d))
         out.append(cands)
     return out
 
 
+def _optional(rng, d, top=False):
+    items = [(k, _optional(rng, v) if isinstance(v, dict) else v) for k, v in d.items()]
+    items = [(k, None if isinstance(v, dict) and rng.random() < P_NULL_SUB else v) for k, v in items
+             if not (isinstance(v, dict) and rng.random() < P_MISSING_SUB)]
+    if len(items) > 1 and rng.random() < P_DROP:
+        del items[rng.randrange(len(items))]
+    if top and rng.random() < P_EXTRA:
+        items.append(("po_number", rng.choice(["PO-1001", "PO-1002", None])))
+    if rng.random() < P_REORDER:
+        rng.shuffle(items)
+    return dict(items)
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["s32", "invoice", "invoice_nested"], default="s32",
+    ap.add_argument("--workload", choices=["s32", "invoice", "invoice_nested", "invoice_optional", "invoice_nested_optional"], default="s32",
                     help="s32: the bench schema (enum / bool / number fields); invoice: 12 fields, 4 of them free text (medoid, K4); "
-                         "invoice_nested: the same fields in nested objects (depth 3)")
+                         "invoice_nested: the same fields in nested objects (depth 3); *_optional: candidates that reorder, drop and add "
+                         "keys and (nested) hold None or nothing for sub-objects")
     ap.add_argument("--records", type=int, default=262144)
     ap.add_argument("--n", type=int, default=16)
     ap.add_argument("--reps", type=int, default=4)
@@ -78,7 +100,8 @@ def main():
     args = ap.parse_args()
     t0 = time.perf_counter()
     if args.workload != "s32":
-        blob, off, _n = K.pack_texts(invoice_texts(args.records, args.n, 11, nested=args.workload == "invoice_nested"), pinned=not args.pageable)
+        blob, off, _n = K.pack_texts(invoice_texts(args.records, args.n, 11, nested="nested" in args.workload, optional="optional" in args.workload),
+                                     pinned=not args.pageable)
     else:
         blob, off = K.s32_texts_packed(args.records, args.n, 11, pinned=not args.pageable)
     gen_s = time.perf_counter() - t0
@@ -88,7 +111,7 @@ def main():
             walls, stats = [], None
             for i in range(args.reps + 1):
                 t0 = time.perf_counter()
-                res = K.consolidate_json_packed(blob, off, args.n)
+                res = K.consolidate_json_packed(blob, off, args.n, flags=K.JSON_KEY_UNION)  # as the client functions call it
                 dt = time.perf_counter() - t0
                 stats = res.stats.as_dict()
                 first = res.content(0)
@@ -99,7 +122,8 @@ def main():
             print(json.dumps({"workload": args.workload, "records": args.records, "n": args.n, "chunk_mb": int(chunk), "streams": int(streams),
                               "pinned_input": not args.pageable, "json_GB": round(stats["input_bytes"] / 1e9, 3),
                               "best_s": round(best, 4), "mean_s": round(sum(walls) / len(walls), 4),
-                              "records_per_s": round(args.records / best), "json_GBps": round(stats["input_bytes"] / best / 1e9, 2),
+                              "records_per_s": round(args.records / best), "n_device": stats["n_device"], "n_host": stats["n_host"],
+                              "n_python": stats["n_python"], "json_GBps": round(stats["input_bytes"] / best / 1e9, 2),
                               "stats": {k: (round(v, 2) if isinstance(v, float) else v) for k, v in stats.items()},
                               "generate_s": round(gen_s, 1), "example": first[:80]}), flush=True)
 
