@@ -15,6 +15,7 @@
 #include <mutex>
 #include <string>
 #include <thread>
+#include <type_traits>
 #include <vector>
 
 #include <cub/device/device_scan.cuh>
@@ -28,6 +29,11 @@ namespace {
 
 using kc::js::Chunk;
 using kc::js::Tok;
+
+#define R_(call)                              \
+    do {                                      \
+        if (const int rc_ = (call)) return rc_; \
+    } while (0)
 
 struct DBuf {  // grow-only device buffer
     void *p = nullptr;
@@ -47,6 +53,7 @@ struct DBuf {  // grow-only device buffer
     }
     // reserve() that keeps the first `keep` bytes (copied on stream s; the stream is synchronised before the old buffer is freed)
     int grow(size_t need, size_t keep, cudaStream_t s) {
+        if (!keep) return reserve(need);
         if (p && need <= cap) return KC_OK;
         void *old = p;
         const size_t old_cap = cap;
@@ -56,7 +63,7 @@ struct DBuf {  // grow-only device buffer
             cudaFree(old);
             return rc;
         }
-        if (old && keep) KC_CUDA_I(cudaMemcpyAsync(p, old, std::min(keep, old_cap), cudaMemcpyDeviceToDevice, s));
+        if (old) KC_CUDA_I(cudaMemcpyAsync(p, old, std::min(keep, old_cap), cudaMemcpyDeviceToDevice, s));
         KC_CUDA_I(cudaStreamSynchronize(s));
         if (old) cudaFree(old);
         return KC_OK;
@@ -85,14 +92,38 @@ struct PBuf {  // grow-only pinned host buffer
     T *as() const { return static_cast<T *>(p); }
 };
 
+constexpr int kSlotArrays = 8;
+
+// The chunk's slot-sized arrays, each named once: its buffer index, its elements per field slot, its minimum length and the
+// byte its new elements are filled with.  alloc(k, ptr, len, keep, fill, on_device) sizes buffer k for len elements keeping the
+// first `keep`, binds ptr to it and fills the rest: the host twin fills every array, the device only those marked on_device
+// (the cell matrices: a record declined while encoding leaves its rows untouched, and K1 / K2 read them; every other element
+// is written before it is read).  vrec: the vote groups' records, for weighted calls.
+template <class Alloc>
+int slot_arrays(const Alloc &alloc, Chunk &ch, size_t T, size_t keep, bool vrec) {
+    const size_t n = (size_t)ch.n;
+    auto a = [&](int k, auto *&ptr, size_t per, size_t min, int fill, bool on_device) {
+        return alloc(k, ptr, std::max(T * per, min), keep * per, fill, on_device);
+    };
+    R_(a(0, ch.toks, n, 1, 0, false));
+    R_(a(1, ch.fdesc, 1, 1, 0, false));
+    R_(a(2, ch.gpos, 1, 1, 0, false));
+    R_(a(3, ch.piece_c, 1, 1, 0, false));
+    R_(a(4, ch.piece_l, 1, 1, 0, false));
+    R_(a(5, ch.vcells, n, 16, 0xFF, true));  // KC_CODE_NONE
+    R_(a(6, ch.xcells, n, 2, 0, true));
+    if (vrec) R_(a(7, ch.vrec, 1, 1, 0xFF, false));  // -1
+    return KC_OK;
+}
+
 // Everything one in-flight chunk needs on the device.  Workers are pooled per device and reused across calls.
 struct Worker {
     int device = -1;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[7] = {};
-    DBuf text, off, fcount, slot, status, vbase, xbase, counters, toks, fdesc, piece_c, piece_l, vcells, xcells, win, vmeta, xvalue, xmeta,
-        len_c, len_l, out_c, out_l, scan_tmp, mcount, scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, gpos, seq, vrec, vweight,
-        pend, plist, ucand, ubase, usize, utok, unode, umap;
+    DBuf text, off, fcount, slot, status, vbase, xbase, counters, win, vmeta, xvalue, xmeta, len_c, len_l, out_c, out_l, scan_tmp, mcount,
+        scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, seq, vweight, pend, plist, ucand, ubase, usize, utok, unode, umap;
+    DBuf slot_buf[kSlotArrays];  // slot_arrays
     PBuf h_small;  // totals and counters (pinned so the small D2H copies are asynchronous)
     PBuf h_scan;   // the scanned record offsets and the statuses of a chunk
     bool busy = false;
@@ -184,6 +215,44 @@ int team_size(int n) {
     return t;
 }
 
+// the device slot arrays for T slots (the first `keep` kept), and the result arrays of K1 (or K3b), K2 (or K5) beside them
+int size_slots(Worker &w, Chunk &ch, size_t T, size_t keep, bool weighted) {
+    cudaStream_t s = w.stream;
+    auto dev = [&](int k, auto *&ptr, size_t len, size_t keep_len, int fill, bool on_device) -> int {
+        using E = std::remove_reference_t<decltype(*ptr)>;
+        R_(w.slot_buf[k].grow(len * sizeof(E), keep_len * sizeof(E), s));
+        ptr = w.slot_buf[k].as<E>();
+        if (on_device) KC_CUDA_I(cudaMemsetAsync(ptr + keep_len, fill, (len - keep_len) * sizeof(E), s));
+        return KC_OK;
+    };
+    R_(slot_arrays(dev, ch, T, keep, weighted));
+    const size_t T1 = std::max<size_t>(T, 1);
+    R_(w.win.reserve(T1 * 4));
+    R_(w.vmeta.reserve(T1 * 4));
+    R_(w.xvalue.reserve(T1 * 8));
+    R_(w.xmeta.reserve(T1 * 4));
+    ch.vmeta = w.vmeta.as<uint32_t>();
+    ch.xvalue = w.xvalue.as<double>();
+    ch.xmeta = w.xmeta.as<uint32_t>();
+    ch.xbest = w.xmeta.as<int32_t>();  // K5 writes its results where K2 would
+    ch.xavg = w.xvalue.as<double>();
+    if (weighted) {
+        R_(w.vweight.reserve(T1 * 4));
+        ch.vweight = w.vweight.as<float>();
+    }
+    return KC_OK;
+}
+
+template <typename T>
+void exclusive_scan(std::vector<T> &v) {  // in place, as cub::DeviceScan::ExclusiveSum
+    T acc = 0;
+    for (T &x : v) {
+        const T c = x;
+        x = acc;
+        acc += c;
+    }
+}
+
 }  // namespace
 
 struct kc_json_result {
@@ -209,12 +278,6 @@ struct ChunkStage {  // per-chunk device-time split (CUDA events on the chunk's 
 int union_round(Worker &w, Chunk &ch, int64_t P, size_t &T, int team, int grid, bool weighted, unsigned long long *h_cnt) {
     cudaStream_t s = w.stream;
     const int32_t n = ch.n;
-    int rc;
-#define R_(call)          \
-    do {                  \
-        rc = (call);      \
-        if (rc) return rc; \
-    } while (0)
     R_(w.ucand.reserve((size_t)P * n * 4));
     R_(w.ubase.reserve((size_t)P * 4));
     R_(w.usize.reserve((size_t)P * 4));
@@ -240,47 +303,15 @@ int union_round(Worker &w, Chunk &ch, int64_t P, size_t &T, int team, int grid, 
     KC_CUDA_I(cudaStreamSynchronize(s));
     const size_t U = h_cnt[5];
     if (U) {
-        const size_t T1 = T + U, Tn = T * (size_t)n, T1n = T1 * (size_t)n;
+        const size_t T1 = T + U;
         if (T1 >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: %zu field slots in one chunk", T1);
-        R_(w.toks.grow(T1n * sizeof(Tok), Tn * sizeof(Tok), s));
-        R_(w.fdesc.grow(T1 * 4, T * 4, s));
-        R_(w.gpos.grow(T1 * 4, T * 4, s));
-        R_(w.piece_c.grow(T1 * 4, T * 4, s));
-        R_(w.piece_l.grow(T1 * 4, T * 4, s));
-        R_(w.vcells.grow(T1n, Tn, s));
-        R_(w.xcells.grow(T1n * 8, Tn * 8, s));
-        R_(w.win.reserve(T1 * 4));
-        R_(w.vmeta.reserve(T1 * 4));
-        R_(w.xvalue.reserve(T1 * 8));
-        R_(w.xmeta.reserve(T1 * 4));
-        ch.toks = w.toks.as<Tok>();
-        ch.fdesc = w.fdesc.as<uint32_t>();
-        ch.gpos = w.gpos.as<uint32_t>();
-        ch.piece_c = w.piece_c.as<uint32_t>();
-        ch.piece_l = w.piece_l.as<uint32_t>();
-        ch.vcells = w.vcells.as<int8_t>();
-        ch.xcells = w.xcells.as<double>();
-        ch.vmeta = w.vmeta.as<uint32_t>();
-        ch.xvalue = w.xvalue.as<double>();
-        ch.xmeta = w.xmeta.as<uint32_t>();
-        ch.xbest = w.xmeta.as<int32_t>();
-        ch.xavg = w.xvalue.as<double>();
-        if (weighted) {
-            R_(w.vrec.grow(T1 * 4, T * 4, s));
-            R_(w.vweight.reserve(T1 * 4));
-            ch.vrec = w.vrec.as<int32_t>();
-            ch.vweight = w.vweight.as<float>();
-        }
-        // the union records' rows of the cell matrices get the same defined contents as the first round's
-        KC_CUDA_I(cudaMemsetAsync(ch.vcells + Tn, 0xFF, T1n - Tn, s));
-        KC_CUDA_I(cudaMemsetAsync(ch.xcells + Tn, 0, (T1n - Tn) * 8, s));
+        R_(size_slots(w, ch, T1, T, weighted));
         T = T1;
     }
     kc::js::union_plan_kernel<<<grid, 128, 0, s>>>(ch, team, (int32_t)P);
     KC_CUDA_I(cudaGetLastError());
     KC_CUDA_I(cudaMemcpyAsync(h_cnt, ch.counters, 48, cudaMemcpyDeviceToHost, s));
     KC_CUDA_I(cudaStreamSynchronize(s));
-#undef R_
     return KC_OK;
 }
 
@@ -294,12 +325,6 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     const size_t bytes = (size_t)(b1 - b0);
     if (bytes >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: chunk of %zu bytes", bytes);
     cudaStream_t s = w.stream;
-    int rc;
-#define R_(call)          \
-    do {                  \
-        rc = (call);      \
-        if (rc) return rc; \
-    } while (0)
     R_(w.text.reserve(bytes + 16));
     R_(w.off.reserve((size_t)(Rc * n + 1) * 8));
     R_(w.fcount.reserve((size_t)(Rc + 1) * 4));
@@ -361,6 +386,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
         const int64_t blocks = (threads_needed + 127) / 128;
         return (int)std::max<int64_t>(1, std::min<int64_t>(blocks, (int64_t)sm_count * 16));
     };
+    auto team_grid = [&](int64_t units) { return grid_for((units + tpw - 1) / tpw * 32); };  // a warp per tpw units
     // A0: fields per record, then their exclusive scan (entry Rc of fcount is 0, so slot[Rc] is the total)
     KC_CUDA_I(cudaMemsetAsync(ch.fcount + Rc, 0, 4, s));
     kc::js::count_kernel<<<grid_for(Rc), 128, 0, s>>>(ch);
@@ -371,56 +397,21 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     KC_CUDA_I(cudaMemcpyAsync(h_total, ch.slot + Rc, 4, cudaMemcpyDeviceToHost, s));
     KC_CUDA_I(cudaStreamSynchronize(s));
     size_t T = *h_total;  // field slots of the chunk (after a union round: its rows too)
-    size_t Tn = T * (size_t)n;
-    R_(w.toks.reserve(std::max<size_t>(Tn, 1) * sizeof(Tok)));
-    R_(w.fdesc.reserve(std::max<size_t>(T, 1) * 4));
-    R_(w.gpos.reserve(std::max<size_t>(T, 1) * 4));
-    R_(w.piece_c.reserve(std::max<size_t>(T, 1) * 4));
-    R_(w.piece_l.reserve(std::max<size_t>(T, 1) * 4));
-    R_(w.vcells.reserve(std::max<size_t>(Tn, 16)));
-    R_(w.xcells.reserve(std::max<size_t>(Tn, 2) * 8));
-    R_(w.win.reserve(std::max<size_t>(T, 1) * 4));
-    R_(w.vmeta.reserve(std::max<size_t>(T, 1) * 4));
-    R_(w.xvalue.reserve(std::max<size_t>(T, 1) * 8));
-    R_(w.xmeta.reserve(std::max<size_t>(T, 1) * 4));
-    ch.toks = w.toks.as<Tok>();
-    ch.fdesc = w.fdesc.as<uint32_t>();
-    ch.gpos = w.gpos.as<uint32_t>();
-    ch.piece_c = w.piece_c.as<uint32_t>();
-    ch.piece_l = w.piece_l.as<uint32_t>();
-    ch.vcells = w.vcells.as<int8_t>();
-    ch.xcells = w.xcells.as<double>();
-    ch.vmeta = w.vmeta.as<uint32_t>();
-    ch.xvalue = w.xvalue.as<double>();
-    ch.xmeta = w.xmeta.as<uint32_t>();
-    ch.xbest = w.xmeta.as<int32_t>();  // K5 writes its results where K2 would
-    ch.xavg = w.xvalue.as<double>();
-    if (h_seq) {
-        R_(w.vrec.reserve(std::max<size_t>(T, 1) * 4));
-        R_(w.vweight.reserve(std::max<size_t>(T, 1) * 4));
-        ch.vrec = w.vrec.as<int32_t>();
-        ch.vweight = w.vweight.as<float>();
-    }
+    R_(size_slots(w, ch, T, 0, h_seq != nullptr));
     KC_CUDA_I(cudaMemsetAsync(w.counters.p, 0, 48, s));
     // records declined before slots_phase own no medoid groups
     KC_CUDA_I(cudaMemsetAsync(w.mcount.p, 0, (size_t)(Rc + 1) * 4, s));
     KC_CUDA_I(cudaMemsetAsync(w.scount.p, 0, (size_t)(Rc + 1) * 4, s));
     KC_CUDA_I(cudaMemsetAsync(w.ccount.p, 0, (size_t)(Rc + 1) * 4, s));
-    // rows reserved by a record that is declined while encoding stay untouched: give them defined contents
-    KC_CUDA_I(cudaMemsetAsync(w.vcells.p, 0xFF, std::max<size_t>(Tn, 16), s));
-    KC_CUDA_I(cudaMemsetAsync(w.xcells.p, 0, std::max<size_t>(Tn, 2) * 8, s));
     int64_t gv = 0, gx = 0, gm = 0;
     if (T) {
-        const int64_t rounds = (Rc + tpw - 1) / tpw;
-        kc::js::plan_kernel<<<grid_for(rounds * 32), 128, 0, s>>>(ch, team);
+        kc::js::plan_kernel<<<team_grid(Rc), 128, 0, s>>>(ch, team);
         KC_CUDA_I(cudaGetLastError());
         unsigned long long *h_cnt = w.h_small.as<unsigned long long>() + 1;
         KC_CUDA_I(cudaMemcpyAsync(h_cnt, w.counters.p, 32, cudaMemcpyDeviceToHost, s));
         KC_CUDA_I(cudaStreamSynchronize(s));
-        if (const int64_t P = (int64_t)h_cnt[3]) {  // records whose candidates differ in shape
-            R_(union_round(w, ch, P, T, team, grid_for((P + tpw - 1) / tpw * 32), h_seq != nullptr, h_cnt));
-            Tn = T * (size_t)n;
-        }
+        if (const int64_t P = (int64_t)h_cnt[3])  // records whose candidates differ in shape
+            R_(union_round(w, ch, P, T, team, team_grid(P), h_seq != nullptr, h_cnt));
         gv = (int64_t)h_cnt[0];
         gx = (int64_t)h_cnt[1];
         gm = (int64_t)h_cnt[2];
@@ -429,7 +420,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
         // A2: multi-word string fields -> K4's CSR input.  Sizes by upper bound (no read-back): the normalised characters are a
         // subset of the chunk's text, a group has at most n strings, a record at most fcount groups.
         R_(w.mchars.reserve(bytes + 16));
-        R_(w.mstr_off.reserve((Tn + 2) * 4));
+        R_(w.mstr_off.reserve((T * (size_t)n + 2) * 4));
         R_(w.mgrp_off.reserve((T + 2) * 4));
         R_(w.midx.reserve((T + 1) * 4));
         R_(w.mavg.reserve((T + 1) * 8));
@@ -442,8 +433,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
             tb = w.scan_tmp.cap;
             KC_CUDA_I(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, tb, (const uint32_t *)cnt, cnt, (int)(Rc + 1), s));
         }
-        const int64_t rounds = (Rc + tpw - 1) / tpw;
-        kc::js::medoid_kernel<<<grid_for(rounds * 32), 128, 0, s>>>(ch, team);
+        kc::js::medoid_kernel<<<team_grid(Rc), 128, 0, s>>>(ch, team);
         KC_CUDA_I(cudaGetLastError());
     }
     KC_CUDA_I(cudaEventRecord(w.ev[2], s));
@@ -464,11 +454,8 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     // C0: piece lengths and record lengths, then record offsets in the two output blobs
     KC_CUDA_I(cudaMemsetAsync(ch.len_c + Rc, 0, 8, s));
     KC_CUDA_I(cudaMemsetAsync(ch.len_l + Rc, 0, 8, s));
-    {
-        const int64_t rounds = (Rc + tpw - 1) / tpw;
-        kc::js::len_kernel<<<grid_for(rounds * 32), 128, 0, s>>>(ch, team);
-        KC_CUDA_I(cudaGetLastError());
-    }
+    kc::js::len_kernel<<<team_grid(Rc), 128, 0, s>>>(ch, team);
+    KC_CUDA_I(cudaGetLastError());
     tb = w.scan_tmp.cap;
     KC_CUDA_I(cub::DeviceScan::ExclusiveSum(w.scan_tmp.p, tb, (const int64_t *)ch.len_c, ch.len_c, (int)(Rc + 1), s));
     tb = w.scan_tmp.cap;
@@ -485,8 +472,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     ch.out_c = w.out_c.as<uint8_t>();
     ch.out_l = w.out_l.as<uint8_t>();
     if (out_c_bytes) {
-        const int64_t rounds = (Rc + tpw - 1) / tpw;
-        kc::js::write_kernel<<<grid_for(rounds * 32), 128, 0, s>>>(ch, team);
+        kc::js::write_kernel<<<team_grid(Rc), 128, 0, s>>>(ch, team);
         KC_CUDA_I(cudaGetLastError());
     }
     KC_CUDA_I(cudaEventRecord(w.ev[4], s));
@@ -523,7 +509,6 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     cudaEventElapsedTime(&ms, w.ev[2], w.ev[3]); st.kernels += ms;
     cudaEventElapsedTime(&ms, w.ev[3], w.ev[4]); st.emit += ms;
     cudaEventElapsedTime(&ms, w.ev[4], w.ev[5]); st.d2h += ms;
-#undef R_
     return KC_OK;
 }
 
@@ -755,9 +740,9 @@ struct kc_debug_jsongpu {
     std::vector<uint8_t> text;
     int32_t n = 0;
     int64_t R = 0;
-    std::vector<uint32_t> fcount, slot, fdesc, gpos, vbase, xbase, piece_c, piece_l;
+    std::vector<uint32_t> fcount, slot, vbase, xbase;
     std::vector<uint8_t> status, nest, pend;
-    std::vector<Tok> toks;
+    std::vector<uint8_t> slot_mem[kSlotArrays];  // slot_arrays (operator new aligns them for any type, Tok's 16 bytes included)
     unsigned long long counters[6] = {0, 0, 0, 0, 0, 0};
     std::vector<int32_t> plist, umap;
     std::vector<uint32_t> ucand, ubase, usize;
@@ -766,9 +751,6 @@ struct kc_debug_jsongpu {
     std::vector<uint32_t> mcount, scount, ccount;
     std::vector<uint8_t> mchars;
     std::vector<int32_t> mstr_off, mgrp_off;
-    std::vector<int8_t> vcells;
-    std::vector<int32_t> vrec;
-    std::vector<double> xcells;
     std::vector<int64_t> len_c, len_l;
     std::vector<uint8_t> out_c, out_l;
     Chunk ch{};
@@ -824,30 +806,15 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     for (int32_t r = 0; r < R; ++r) kc::js::count_record(ch, r);
     for (int64_t r = 0; r < R; ++r) h->slot[(size_t)r + 1] = h->slot[(size_t)r] + h->fcount[(size_t)r];
     const size_t T = h->slot[(size_t)R];
-    h->toks.assign(std::max<size_t>(T * n, 1), Tok{});
-    h->fdesc.assign(std::max<size_t>(T, 1), 0);
-    h->gpos.assign(std::max<size_t>(T, 1), 0);
-    h->piece_c.assign(std::max<size_t>(T, 1), 0);
-    h->piece_l.assign(std::max<size_t>(T, 1), 0);
-    h->vcells.assign(std::max<size_t>(T * n, 16), (int8_t)-1);
-    h->vrec.assign(std::max<size_t>(T, 1), -1);
-    h->xcells.assign(std::max<size_t>(T * n, 2), 0.0);
-    ch.toks = h->toks.data();
-    ch.fdesc = h->fdesc.data();
-    ch.gpos = h->gpos.data();
-    ch.piece_c = h->piece_c.data();
-    ch.piece_l = h->piece_l.data();
-    ch.vcells = h->vcells.data();
-    ch.vrec = h->vrec.data();
-    ch.xcells = h->xcells.data();
-    const int team = team_size(n);
-    for (int32_t r = 0; r < R; ++r) {
-        for (int lane = 0; lane < team; ++lane) kc::js::parse_phase(ch, r, lane, team);
-        for (int lane = 0; lane < team; ++lane) kc::js::type_phase(ch, r, lane, team);
-        for (int lane = 0; lane < team; ++lane) kc::js::order_phase(ch, r, lane, team);
-        kc::js::slots_phase(ch, r, true);
-        for (int lane = 0; lane < team; ++lane) kc::js::encode_phase(ch, r, lane, team);
-    }
+    auto host = [&](int k, auto *&ptr, size_t len, size_t, int fill, bool) -> int {
+        using E = std::remove_reference_t<decltype(*ptr)>;
+        h->slot_mem[k].resize(len * sizeof(E), (uint8_t)fill);  // keeps what is there, fills the rest
+        ptr = reinterpret_cast<E *>(h->slot_mem[k].data());
+        return KC_OK;
+    };
+    slot_arrays(host, ch, T, 0, true);
+    const kc::js::HostTeam team{team_size(n)};
+    for (int32_t r = 0; r < R; ++r) kc::js::plan_step(ch, r, team);
     if (const int64_t P = (int64_t)h->counters[3]) {  // the union round, as run_chunk / union_round run it
         h->ucand.assign((size_t)(P * n), 0);
         h->ubase.assign((size_t)P, 0);
@@ -856,10 +823,7 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
         ch.ubase = h->ubase.data();
         ch.usize = h->usize.data();
         ch.uslot = (uint32_t)T;
-        for (int32_t p = 0; p < P; ++p) {
-            for (int lane = 0; lane < team; ++lane) kc::js::union_count_phase(ch, p, lane, team);
-            kc::js::union_reserve(ch, p);
-        }
+        for (int32_t p = 0; p < P; ++p) kc::js::union_count_step(ch, p, team);
         const size_t S = std::max<size_t>(h->counters[4], 1);
         h->utok.assign(S, Tok{});
         h->unode.assign(S, kc::js::UNode{});
@@ -867,53 +831,18 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
         ch.utok = h->utok.data();
         ch.unode = h->unode.data();
         ch.umap = h->umap.data();
-        for (int32_t p = 0; p < P; ++p) {
-            for (int lane = 0; lane < team; ++lane) kc::js::union_scan_phase(ch, p, lane, team);
-            kc::js::union_build(ch, p);
-        }
-        const size_t T1 = T + (size_t)h->counters[5];
-        h->toks.resize(std::max<size_t>(T1 * n, 1), Tok{});
-        h->fdesc.resize(std::max<size_t>(T1, 1), 0);
-        h->gpos.resize(std::max<size_t>(T1, 1), 0);
-        h->piece_c.resize(std::max<size_t>(T1, 1), 0);
-        h->piece_l.resize(std::max<size_t>(T1, 1), 0);
-        h->vcells.resize(std::max<size_t>(T1 * n, 16), (int8_t)-1);
-        h->vrec.resize(std::max<size_t>(T1, 1), -1);
-        h->xcells.resize(std::max<size_t>(T1 * n, 2), 0.0);
-        ch.toks = h->toks.data();
-        ch.fdesc = h->fdesc.data();
-        ch.gpos = h->gpos.data();
-        ch.piece_c = h->piece_c.data();
-        ch.piece_l = h->piece_l.data();
-        ch.vcells = h->vcells.data();
-        ch.vrec = h->vrec.data();
-        ch.xcells = h->xcells.data();
-        for (int32_t p = 0; p < P; ++p) {
-            const int32_t r = h->plist[(size_t)p];
-            for (int lane = 0; lane < team; ++lane) kc::js::union_write_phase(ch, p, lane, team);
-            if (h->status[(size_t)r] == kc::js::D_UNION) h->status[(size_t)r] = 0;
-            for (int lane = 0; lane < team; ++lane) kc::js::type_phase(ch, r, lane, team);
-            for (int lane = 0; lane < team; ++lane) kc::js::order_phase(ch, r, lane, team);
-            kc::js::slots_phase(ch, r, false);
-            for (int lane = 0; lane < team; ++lane) kc::js::encode_phase(ch, r, lane, team);
-        }
+        for (int32_t p = 0; p < P; ++p) kc::js::union_build_step(ch, p, team);
+        slot_arrays(host, ch, T + (size_t)h->counters[5], T, true);
+        for (int32_t p = 0; p < P; ++p) kc::js::union_plan_step(ch, p, team);
     }
-    for (std::vector<uint32_t> *cnt : {&h->mcount, &h->scount, &h->ccount}) {  // exclusive scans, in place
-        uint32_t acc = 0;
-        for (auto &x : *cnt) {
-            const uint32_t v = x;
-            x = acc;
-            acc += v;
-        }
-    }
+    for (std::vector<uint32_t> *cnt : {&h->mcount, &h->scount, &h->ccount}) exclusive_scan(*cnt);
     h->mchars.assign((size_t)h->ccount[(size_t)R] + 1, 0);
     h->mstr_off.assign((size_t)h->scount[(size_t)R] + 1, 0);
     h->mgrp_off.assign((size_t)h->mcount[(size_t)R] + 1, 0);
     ch.mchars = h->mchars.data();
     ch.mstr_off = h->mstr_off.data();
     ch.mgrp_off = h->mgrp_off.data();
-    for (int32_t r = 0; r < R; ++r)
-        for (int lane = 0; lane < team; ++lane) kc::js::medoid_phase(ch, r, lane, team);
+    for (int32_t r = 0; r < R; ++r) kc::js::medoid_step(ch, r, team);
     *out = h;
     return KC_OK;
 }
@@ -946,9 +875,9 @@ int kc_debug_jsongpu_set_numeric_medoid(kc_debug_jsongpu *h, const int32_t *best
 int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells, int64_t *n_vote_groups, const double **num_cells,
                             int64_t *n_num_groups, const uint8_t **status) {
     if (!h) return KC_EINVAL;
-    if (vote_cells) *vote_cells = h->vcells.data();
+    if (vote_cells) *vote_cells = h->ch.vcells;
     if (n_vote_groups) *n_vote_groups = (int64_t)h->counters[0];
-    if (num_cells) *num_cells = h->xcells.data();
+    if (num_cells) *num_cells = h->ch.xcells;
     if (n_num_groups) *n_num_groups = (int64_t)h->counters[1];
     if (status) *status = h->status.data();
     return KC_OK;
@@ -961,7 +890,7 @@ int kc_debug_jsongpu_emit(kc_debug_jsongpu *h, const uint32_t *vote_meta, const 
 
 int kc_debug_jsongpu_group_records(const kc_debug_jsongpu *h, const int32_t **group_record) {
     if (!h) return KC_EINVAL;
-    if (group_record) *group_record = h->vrec.data();
+    if (group_record) *group_record = h->ch.vrec;
     return KC_OK;
 }
 
@@ -975,25 +904,16 @@ int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_met
     ch.xvalue = num_value;
     ch.xmeta = num_meta;
     const int64_t R = h->R;
-    const int team = team_size(h->n);
-    for (int32_t r = 0; r < R; ++r) {
-        for (int lane = 0; lane < team; ++lane) kc::js::len_phase(ch, r, lane, team);
-        kc::js::offsets_phase(ch, r);
-    }
-    int64_t ac = 0, al = 0;
-    for (int64_t r = 0; r <= R; ++r) {  // exclusive scans, in place
-        const int64_t c = r < R ? h->len_c[(size_t)r] : 0, l = r < R ? h->len_l[(size_t)r] : 0;
-        h->len_c[(size_t)r] = ac;
-        h->len_l[(size_t)r] = al;
-        ac += c;
-        al += l;
-    }
+    const kc::js::HostTeam team{team_size(h->n)};
+    for (int32_t r = 0; r < R; ++r) kc::js::len_step(ch, r, team);
+    exclusive_scan(h->len_c);
+    exclusive_scan(h->len_l);
+    const int64_t ac = h->len_c[(size_t)R], al = h->len_l[(size_t)R];
     h->out_c.assign((size_t)std::max<int64_t>(ac, 1), 0);
     h->out_l.assign((size_t)std::max<int64_t>(al, 1), 0);
     ch.out_c = h->out_c.data();
     ch.out_l = h->out_l.data();
-    for (int32_t r = 0; r < R; ++r)
-        for (int lane = 0; lane < team; ++lane) kc::js::write_phase(ch, r, lane, team);
+    for (int32_t r = 0; r < R; ++r) kc::js::write_step(ch, r, team);
     if (content) *content = (const char *)h->out_c.data();
     if (content_off) *content_off = h->len_c.data();
     if (likelihoods) *likelihoods = (const char *)h->out_l.data();

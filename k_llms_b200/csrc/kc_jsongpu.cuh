@@ -37,7 +37,9 @@
 // consolidated by the host path (kc_consolidate_json) instead: the device path never guesses.
 //
 // The phases are plain __host__ __device__ functions of (chunk, record, lane, team size) that communicate through global
-// arrays only — no warp intrinsics — so the CPU tests run the SAME code on the host, lane by lane (kc_debug_jsongpu_*).
+// arrays only — no warp intrinsics.  Each kernel's schedule of phases is one step function over a team type (the steps at the
+// end of this file): the kernels run it with a team of lanes, the host twin (kc_debug_jsongpu_*) with a loop over the lanes,
+// so the CPU tests run the SAME phases in the SAME order as the kernels.
 #pragma once
 
 #include "kc_jsoncore.cuh"
@@ -837,6 +839,105 @@ KC_HD inline void write_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t 
     }
 }
 
+// ---------------------------------------------------------------- steps: each kernel's schedule of phases
+//
+// A step runs the phases of one unit of work (a record; in the union round, record plist[p]) on a team, in the kernel's order.
+// On the device a team is `size` lanes of one warp: a phase runs on the lanes of a live team, then the whole warp meets at
+// __syncwarp() (which also orders the team's global-memory traffic between phases).  A dead team (no unit left this round)
+// still reaches every __syncwarp() of the live teams of its warp.  On the host a team is a loop over its lanes.
+
+struct DeviceTeam {
+    int32_t lane, size;
+    bool live;
+    KC_HD void sync() const {
+#ifdef __CUDA_ARCH__
+        __syncwarp();
+#endif
+    }
+    template <class F>
+    KC_HD void each(const F &f) const {
+        if (live) f(lane);
+        sync();
+    }
+    template <class F>
+    KC_HD void leader(const F &f) const {
+        if (live && lane == 0) f();
+        sync();
+    }
+    // a kernel's only phase: no lane reads what another one wrote, so the lanes need not meet
+    template <class F>
+    KC_HD void each_nosync(const F &f) const {
+        if (live) f(lane);
+    }
+};
+
+struct HostTeam {
+    int32_t size;
+    static constexpr bool live = true;
+    template <class F>
+    KC_HD void each(const F &f) const {
+        for (int32_t lane = 0; lane < size; ++lane) f(lane);
+    }
+    template <class F>
+    KC_HD void leader(const F &f) const { f(); }
+    template <class F>
+    KC_HD void each_nosync(const F &f) const { each(f); }
+};
+
+// A1 after the parse, and U3 after the table: type / order / slots / encode
+template <class Team>
+KC_HD void table_phases(const Chunk &ch, int32_t r, const Team &tm, bool first_round) {
+    tm.each([&](int32_t lane) { type_phase(ch, r, lane, tm.size); });
+    tm.each([&](int32_t lane) { order_phase(ch, r, lane, tm.size); });  // nested records only; reads the ranks its team wrote
+    tm.leader([&] { slots_phase(ch, r, first_round); });
+    tm.each([&](int32_t lane) { encode_phase(ch, r, lane, tm.size); });
+}
+
+template <class Team>
+KC_HD void plan_step(const Chunk &ch, int32_t r, const Team &tm) {
+    tm.each([&](int32_t lane) { parse_phase(ch, r, lane, tm.size); });
+    table_phases(ch, r, tm, true);
+}
+
+template <class Team>
+KC_HD void union_count_step(const Chunk &ch, int32_t p, const Team &tm) {
+    tm.each([&](int32_t lane) { union_count_phase(ch, p, lane, tm.size); });
+    tm.leader([&] { union_reserve(ch, p); });
+}
+
+template <class Team>
+KC_HD void union_build_step(const Chunk &ch, int32_t p, const Team &tm) {
+    tm.each([&](int32_t lane) { union_scan_phase(ch, p, lane, tm.size); });
+    tm.leader([&] { union_build(ch, p); });
+}
+
+// the table, then A1's phases on it (the leader clears the status between the two)
+template <class Team>
+KC_HD void union_plan_step(const Chunk &ch, int32_t p, const Team &tm) {
+    const int32_t r = tm.live ? ch.plist[p] : 0;
+    tm.each([&](int32_t lane) { union_write_phase(ch, p, lane, tm.size); });
+    tm.leader([&] {
+        if (load_status(ch, r) == D_UNION) decline(ch, r, D_OK);
+    });
+    table_phases(ch, r, tm, false);
+}
+
+template <class Team>
+KC_HD void medoid_step(const Chunk &ch, int32_t r, const Team &tm) {
+    tm.each_nosync([&](int32_t lane) { medoid_phase(ch, r, lane, tm.size); });
+}
+
+template <class Team>
+KC_HD void len_step(const Chunk &ch, int32_t r, const Team &tm) {
+    tm.each([&](int32_t lane) { len_phase(ch, r, lane, tm.size); });
+    tm.leader([&] { offsets_phase(ch, r); });
+}
+
+template <class Team>
+KC_HD void write_step(const Chunk &ch, int32_t r, const Team &tm) {
+    tm.each_nosync([&](int32_t lane) { write_phase(ch, r, lane, tm.size); });
+}
+
 // ---------------------------------------------------------------- kernels
 
 #ifdef __CUDACC__
@@ -845,117 +946,46 @@ __global__ void __launch_bounds__(128) count_kernel(const Chunk ch) {
     for (int32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < ch.R; r += gridDim.x * blockDim.x) count_record(ch, r);
 }
 
-// Team t of a warp owns record (warp_index * teams_per_warp + t) of every grid-stride round; all lanes of the warp walk the
-// same phases and meet at __syncwarp() (which also orders the team's global-memory traffic between phases).
-__global__ void __launch_bounds__(128) plan_kernel(const Chunk ch, int32_t team) {
+// Team t of a warp owns unit (warp_index * teams_per_warp + t) of every grid-stride round; all lanes of the warp walk the
+// same rounds, so they meet at the same __syncwarp()s.
+template <class Step>
+__device__ __forceinline__ void team_loop(int32_t team, int64_t units, const Step &step) {
     const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
     const int32_t lane = lane_w % team, t = lane_w / team;
     const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int64_t rounds = ((int64_t)ch.R + tpw - 1) / tpw;
+    const int64_t rounds = (units + tpw - 1) / tpw;
     for (int64_t w = warp; w < rounds; w += n_warps) {
-        const int64_t r64 = w * tpw + t;
-        const bool live = r64 < ch.R;
-        const int32_t r = (int32_t)r64;
-        if (live) parse_phase(ch, r, lane, team);
-        __syncwarp();
-        if (live) type_phase(ch, r, lane, team);
-        __syncwarp();
-        if (live) order_phase(ch, r, lane, team);  // nested records only; reads the ranks its team wrote
-        __syncwarp();
-        if (live && lane == 0) slots_phase(ch, r, true);
-        __syncwarp();
-        if (live) encode_phase(ch, r, lane, team);
-        __syncwarp();
+        const int64_t u = w * tpw + t;
+        step((int32_t)u, DeviceTeam{lane, team, u < units});
     }
 }
 
-// The union round: team t of a warp owns the round's record p = warp_index * teams_per_warp + t, as in plan_kernel.
+__global__ void __launch_bounds__(128) plan_kernel(const Chunk ch, int32_t team) {
+    team_loop(team, ch.R, [&](int32_t r, const DeviceTeam &tm) { plan_step(ch, r, tm); });
+}
+
 __global__ void __launch_bounds__(128) union_count_kernel(const Chunk ch, int32_t team, int32_t P) {
-    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
-    const int32_t lane = lane_w % team, t = lane_w / team;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t w = warp; w < ((int64_t)P + tpw - 1) / tpw; w += n_warps) {
-        const int64_t p = w * tpw + t;
-        if (p < P) union_count_phase(ch, (int32_t)p, lane, team);
-        __syncwarp();
-        if (p < P && lane == 0) union_reserve(ch, (int32_t)p);
-        __syncwarp();
-    }
+    team_loop(team, P, [&](int32_t p, const DeviceTeam &tm) { union_count_step(ch, p, tm); });
 }
 
 __global__ void __launch_bounds__(128) union_build_kernel(const Chunk ch, int32_t team, int32_t P) {
-    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
-    const int32_t lane = lane_w % team, t = lane_w / team;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t w = warp; w < ((int64_t)P + tpw - 1) / tpw; w += n_warps) {
-        const int64_t p = w * tpw + t;
-        if (p < P) union_scan_phase(ch, (int32_t)p, lane, team);
-        __syncwarp();
-        if (p < P && lane == 0) union_build(ch, (int32_t)p);
-        __syncwarp();
-    }
+    team_loop(team, P, [&](int32_t p, const DeviceTeam &tm) { union_build_step(ch, p, tm); });
 }
 
-// the table, then A1's phases on it (the leader clears the status between the two)
 __global__ void __launch_bounds__(128) union_plan_kernel(const Chunk ch, int32_t team, int32_t P) {
-    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
-    const int32_t lane = lane_w % team, t = lane_w / team;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    for (int64_t w = warp; w < ((int64_t)P + tpw - 1) / tpw; w += n_warps) {
-        const int64_t p = w * tpw + t;
-        const bool live = p < P;
-        const int32_t r = live ? ch.plist[p] : 0;
-        if (live) union_write_phase(ch, (int32_t)p, lane, team);
-        __syncwarp();
-        if (live && lane == 0 && load_status(ch, r) == D_UNION) decline(ch, r, D_OK);
-        __syncwarp();
-        if (live) type_phase(ch, r, lane, team);
-        __syncwarp();
-        if (live) order_phase(ch, r, lane, team);
-        __syncwarp();
-        if (live && lane == 0) slots_phase(ch, r, false);
-        __syncwarp();
-        if (live) encode_phase(ch, r, lane, team);
-        __syncwarp();
-    }
+    team_loop(team, P, [&](int32_t p, const DeviceTeam &tm) { union_plan_step(ch, p, tm); });
 }
 
 __global__ void __launch_bounds__(128) medoid_kernel(const Chunk ch, int32_t team) {
-    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
-    const int32_t lane = lane_w % team, t = lane_w / team;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int64_t rounds = ((int64_t)ch.R + tpw - 1) / tpw;
-    for (int64_t w = warp; w < rounds; w += n_warps) {
-        const int64_t r64 = w * tpw + t;
-        if (r64 < ch.R) medoid_phase(ch, (int32_t)r64, lane, team);
-    }
+    team_loop(team, ch.R, [&](int32_t r, const DeviceTeam &tm) { medoid_step(ch, r, tm); });
 }
 
 __global__ void __launch_bounds__(128) len_kernel(const Chunk ch, int32_t team) {
-    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
-    const int32_t lane = lane_w % team, t = lane_w / team;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int64_t rounds = ((int64_t)ch.R + tpw - 1) / tpw;
-    for (int64_t w = warp; w < rounds; w += n_warps) {
-        const int64_t r64 = w * tpw + t;
-        const bool live = r64 < ch.R;
-        const int32_t r = (int32_t)r64;
-        if (live) len_phase(ch, r, lane, team);
-        __syncwarp();
-        if (live && lane == 0) offsets_phase(ch, r);
-        __syncwarp();
-    }
+    team_loop(team, ch.R, [&](int32_t r, const DeviceTeam &tm) { len_step(ch, r, tm); });
 }
 
 __global__ void __launch_bounds__(128) write_kernel(const Chunk ch, int32_t team) {
-    const int32_t lane_w = threadIdx.x & 31, tpw = 32 / team;
-    const int32_t lane = lane_w % team, t = lane_w / team;
-    const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, n_warps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-    const int64_t rounds = ((int64_t)ch.R + tpw - 1) / tpw;
-    for (int64_t w = warp; w < rounds; w += n_warps) {
-        const int64_t r64 = w * tpw + t;
-        if (r64 < ch.R) write_phase(ch, (int32_t)r64, lane, team);
-    }
+    team_loop(team, ch.R, [&](int32_t r, const DeviceTeam &tm) { write_step(ch, r, tm); });
 }
 
 #endif  // __CUDACC__

@@ -1,14 +1,14 @@
 """Test helpers of the async dispatcher on the device JSON path (KC_JSON_NUMERIC_MEDOID): K5's oracle (numpy's own nanmean / argmax
-on the reference's similarity matrix), the device phases instantiated on the host with the oracles in the kernels' place, and the
-cell encoding of golden value groups."""
+on the reference's similarity matrix), a stand-in for the async entry's device call (the device phases on the host with the
+oracles in the kernels' place), and the cell encoding of golden value groups."""
 from __future__ import annotations
 
-import ctypes as c
 import json
 
 import numpy as np
 
 from oracle import columnar as OC
+from tests.helpers import jsongpu_with_oracle
 
 GOLDEN = "tests/golden/async_numeric.json"
 
@@ -66,60 +66,12 @@ def numeric_medoid(cells: np.ndarray, block: int = 2048):
     return best, avg
 
 
-def jsongpu_async_with_oracle(records, seq=None):
-    """The device JSON path's phases under KC_JSON_NUMERIC_MEDOID, run on the host: kc_debug_jsongpu_plan_flags -> the C oracle
-    in K1 (or K3b, seq float32 [R*n] given) and K4's place, numeric_medoid in K5's -> kc_debug_jsongpu_emit(_weighted).  Returns (pairs, status):
-    pairs[r] = (content, likelihoods) or None where the device path declines the record (status[r] = its reason code)."""
-    from k_llms_b200 import _native as K
-    lib = K.load()
-    R = len(records)
-    if R == 0:
-        return [], []
-    blob, off, n = K.pack_texts(records, pinned=False)
-    h = c.c_void_p()
-    K.check(lib.kc_debug_jsongpu_plan_flags(blob.ctypes.data, off.ctypes.data, R, n, K.JSON_NUMERIC_MEDOID, c.byref(h)))
-    try:
-        vc, nc, st, gr = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_void_p()
-        gv, gx = c.c_int64(), c.c_int64()
-        K.check(lib.kc_debug_jsongpu_inputs(h, c.byref(vc), c.byref(gv), c.byref(nc), c.byref(gx), c.byref(st)))
-        K.check(lib.kc_debug_jsongpu_group_records(h, c.byref(gr)))
-        vmeta, vweight = np.zeros(max(gv.value, 1), dtype=np.uint32), np.zeros(max(gv.value, 1), dtype=np.float32)
-        if gv.value:
-            codes = np.ctypeslib.as_array(c.cast(vc, c.POINTER(c.c_int8)), shape=(gv.value, n)).astype(np.int32)
-            if seq is None:
-                _, vmeta = OC.vote(codes, None)
-            else:
-                rec = np.ctypeslib.as_array(c.cast(gr, c.POINTER(c.c_int32)), shape=(gv.value,)).copy()
-                _, vmeta, vweight = OC.weighted_vote(codes[:, None, :], np.asarray(seq, dtype=np.float32).reshape(R, n)[rec])
-        best, avg = np.zeros(max(gx.value, 1), dtype=np.int32), np.zeros(max(gx.value, 1), dtype=np.float64)
-        if gx.value:  # the oracle in K5's place
-            best, avg = numeric_medoid(np.ctypeslib.as_array(c.cast(nc, c.POINTER(c.c_double)), shape=(gx.value, n)).copy())
-        K.check(lib.kc_debug_jsongpu_set_numeric_medoid(h, best.ctypes.data, avg.ctypes.data))
-        mc, so, go, gm = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_int64()
-        K.check(lib.kc_debug_jsongpu_medoid_inputs(h, c.byref(mc), c.byref(so), c.byref(go), c.byref(gm)))
-        midx, mavg = np.zeros(max(gm.value, 1), dtype=np.int32), np.zeros(max(gm.value, 1), dtype=np.float64)
-        if gm.value:
-            OC.lib().ko_medoid_str(mc, so, go, gm.value, midx.ctypes.data, mavg.ctypes.data)
-        K.check(lib.kc_debug_jsongpu_set_medoid(h, midx.ctypes.data, mavg.ctypes.data))
-        pc, po, pl, plo = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_void_p()
-        K.check(lib.kc_debug_jsongpu_emit_weighted(h, vmeta.ctypes.data, vweight.ctypes.data if seq is not None else None, None, None,
-                                                   c.byref(pc), c.byref(po), c.byref(pl), c.byref(plo)))
-        status = np.ctypeslib.as_array(c.cast(st, c.POINTER(c.c_uint8)), shape=(R,)).copy()
-        co = np.ctypeslib.as_array(c.cast(po, c.POINTER(c.c_int64)), shape=(R + 1,))
-        lo = np.ctypeslib.as_array(c.cast(plo, c.POINTER(c.c_int64)), shape=(R + 1,))
-        pairs = [None if status[r] else (c.string_at(pc.value + int(co[r]), int(co[r + 1] - co[r])).decode("ascii"),
-                                         c.string_at(pl.value + int(lo[r]), int(lo[r + 1] - lo[r])).decode("ascii")) for r in range(R)]
-        return pairs, list(status)
-    finally:
-        lib.kc_debug_jsongpu_free(h)
-
-
 def oracle_native_consolidate(records, rel_eps, abs_eps, device=0, seq_logprobs=None, counts=None, flags=0):
     """consolidation._native_consolidate for the async dispatcher (flags = JSON_NUMERIC_MEDOID) with the device path's phases on
     the host and the oracle in the kernels' place."""
     from k_llms_b200 import _native as K
     assert flags == K.JSON_NUMERIC_MEDOID
-    pairs, _ = jsongpu_async_with_oracle(records, seq_logprobs)
+    pairs, _ = jsongpu_with_oracle(records, seq_logprobs, flags=flags)
     if counts is not None:
         counts["device"] = counts.get("device", 0) + sum(p is not None for p in pairs)
     return pairs

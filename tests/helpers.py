@@ -343,53 +343,61 @@ def consolidate_json_with_oracle(records):
         lib.kc_json_free(h)
 
 
-def jsongpu_with_oracle(records):
-    """The DEVICE JSON path's phases (kc_jsongpu.cuh) instantiated on the host: kc_debug_jsongpu_plan -> the C ORACLE in the
-    place of K1 / K2 / K4 -> kc_debug_jsongpu_emit.  Returns (pairs, status): pairs[r] = (content, likelihoods) or None where the
-    device path declines the record (status[r] = its reason code)."""
+def jsongpu_with_oracle(records, seq=None, flags=0):
+    """The DEVICE JSON path's phases (kc_jsongpu.cuh) instantiated on the host: kc_debug_jsongpu_plan_flags -> the oracles in the
+    kernels' places -> kc_debug_jsongpu_emit_weighted.  K1: the C oracle's vote, or with seq (float32 [R*n] candidate sums) its
+    likelihood-weighted vote over the group records (K3b); K2: the C oracle, or with JSON_NUMERIC_MEDOID in flags numpy's medoid
+    (K5, tests.async_native_oracle.numeric_medoid); K4: the C oracle.  Returns (pairs, status): pairs[r] = (content,
+    likelihoods) or None where the device path declines the record (status[r] = its reason code)."""
     import ctypes as c
     from k_llms_b200 import _native as K
     from oracle import columnar as OC
+    from tests.async_native_oracle import numeric_medoid
     lib = K.load()
     R = len(records)
     if R == 0:
         return [], []
     blob, off, n = K.pack_texts(records, pinned=False)
     h = c.c_void_p()
-    K.check(lib.kc_debug_jsongpu_plan(blob.ctypes.data, off.ctypes.data, R, n, c.byref(h)))
+    K.check(lib.kc_debug_jsongpu_plan_flags(blob.ctypes.data, off.ctypes.data, R, n, flags, c.byref(h)))
     try:
-        vc, nc, st = c.c_void_p(), c.c_void_p(), c.c_void_p()
+        vc, nc, st, gr = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_void_p()
         gv, gx = c.c_int64(), c.c_int64()
         K.check(lib.kc_debug_jsongpu_inputs(h, c.byref(vc), c.byref(gv), c.byref(nc), c.byref(gx), c.byref(st)))
-        status = np.ctypeslib.as_array(c.cast(st, c.POINTER(c.c_uint8)), shape=(R,)).copy()
-        vmeta = np.zeros(max(gv.value, 1), dtype=np.uint32)
-        nvalue, nmeta = np.zeros(max(gx.value, 1), dtype=np.float64), np.zeros(max(gx.value, 1), dtype=np.uint32)
+        vmeta, vweight = np.zeros(max(gv.value, 1), dtype=np.uint32), np.zeros(max(gv.value, 1), dtype=np.float32)
         if gv.value:
             codes = np.ctypeslib.as_array(c.cast(vc, c.POINTER(c.c_int8)), shape=(gv.value, n)).astype(np.int32)
-            _, vmeta = OC.vote(codes, None)
+            if seq is None:
+                _, vmeta = OC.vote(codes, None)
+            else:
+                K.check(lib.kc_debug_jsongpu_group_records(h, c.byref(gr)))
+                rec = np.ctypeslib.as_array(c.cast(gr, c.POINTER(c.c_int32)), shape=(gv.value,)).copy()
+                assert (rec >= 0).all() and (rec < R).all()
+                _, vmeta, vweight = OC.weighted_vote(codes[:, None, :], np.asarray(seq, dtype=np.float32).reshape(R, n)[rec])
+        nvalue, nmeta = np.zeros(max(gx.value, 1), dtype=np.float64), np.zeros(max(gx.value, 1), dtype=np.uint32)
+        best, avg = np.zeros(max(gx.value, 1), dtype=np.int32), np.zeros(max(gx.value, 1), dtype=np.float64)
         if gx.value:
-            vals = np.ctypeslib.as_array(c.cast(nc, c.POINTER(c.c_double)), shape=(gx.value, n)).copy()
-            nvalue, nmeta = OC.numeric(vals)
+            cells = np.ctypeslib.as_array(c.cast(nc, c.POINTER(c.c_double)), shape=(gx.value, n)).copy()
+            if flags & K.JSON_NUMERIC_MEDOID:
+                best, avg = numeric_medoid(cells)
+            else:
+                nvalue, nmeta = OC.numeric(cells)
+        K.check(lib.kc_debug_jsongpu_set_numeric_medoid(h, best.ctypes.data, avg.ctypes.data))
         mc, so, go, gm = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_int64()
         K.check(lib.kc_debug_jsongpu_medoid_inputs(h, c.byref(mc), c.byref(so), c.byref(go), c.byref(gm)))
         midx, mavg = np.zeros(max(gm.value, 1), dtype=np.int32), np.zeros(max(gm.value, 1), dtype=np.float64)
-        if gm.value:   # the C oracle in K4's place
+        if gm.value:
             OC.lib().ko_medoid_str(mc, so, go, gm.value, midx.ctypes.data, mavg.ctypes.data)
         K.check(lib.kc_debug_jsongpu_set_medoid(h, midx.ctypes.data, mavg.ctypes.data))
         pc, po, pl, plo = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_void_p()
-        K.check(lib.kc_debug_jsongpu_emit(h, vmeta.ctypes.data, nvalue.ctypes.data, nmeta.ctypes.data, c.byref(pc), c.byref(po),
-                                          c.byref(pl), c.byref(plo)))
-        # a record can still be declined while encoding (number range): re-read the statuses
+        K.check(lib.kc_debug_jsongpu_emit_weighted(h, vmeta.ctypes.data, None if seq is None else vweight.ctypes.data, nvalue.ctypes.data,
+                                                   nmeta.ctypes.data, c.byref(pc), c.byref(po), c.byref(pl), c.byref(plo)))
+        # a record can still be declined while encoding (number range): read the statuses after emit
         status = np.ctypeslib.as_array(c.cast(st, c.POINTER(c.c_uint8)), shape=(R,)).copy()
         co = np.ctypeslib.as_array(c.cast(po, c.POINTER(c.c_int64)), shape=(R + 1,))
         lo = np.ctypeslib.as_array(c.cast(plo, c.POINTER(c.c_int64)), shape=(R + 1,))
-        pairs = []
-        for r in range(R):
-            if status[r]:
-                pairs.append(None)
-            else:
-                pairs.append((c.string_at(pc.value + int(co[r]), int(co[r + 1] - co[r])).decode("ascii"),
-                              c.string_at(pl.value + int(lo[r]), int(lo[r + 1] - lo[r])).decode("ascii")))
-        return pairs, list(status)
+        pairs = [None if status[r] else (c.string_at(pc.value + int(co[r]), int(co[r + 1] - co[r])).decode("ascii"),
+                                         c.string_at(pl.value + int(lo[r]), int(lo[r + 1] - lo[r])).decode("ascii")) for r in range(R)]
+        return pairs, [int(s) for s in status]
     finally:
         lib.kc_debug_jsongpu_free(h)

@@ -17,8 +17,8 @@ from k_llms_b200 import columnar
 from k_llms_b200.utils import consensus_utils as CU
 from k_llms_b200.utils import consolidation as C
 from oracle import columnar as OC
-from tests.async_native_oracle import cells_of, golden_cases, jsongpu_async_with_oracle, numeric_medoid, oracle_native_consolidate
-from tests.helpers import oracle_run
+from tests.async_native_oracle import cells_of, golden_cases, numeric_medoid, oracle_native_consolidate
+from tests.helpers import jsongpu_with_oracle, oracle_run
 
 
 async def _raising(texts):
@@ -109,7 +109,7 @@ def test_device_phases_match_golden_texts():
     assert len(cases) > 40
     accepted = 0
     for case in cases:
-        (got,), (st,) = jsongpu_async_with_oracle([case["texts"]])
+        (got,), (st,) = jsongpu_with_oracle([case["texts"]], flags=K.JSON_NUMERIC_MEDOID)
         if got is not None:
             accepted += 1
             assert got == (case["content"], case["likelihoods"]), (case, got)
@@ -132,7 +132,7 @@ def test_device_phases_match_python_async_route(oracle_kernels):
     from tests.test_json_fuzz import _records
     accepted = declined = 0
     for _n, recs in _records(600, 4242, ns=(2, 3, 5, 8, 16)).items():
-        pairs, status = jsongpu_async_with_oracle(recs)
+        pairs, status = jsongpu_with_oracle(recs, flags=K.JSON_NUMERIC_MEDOID)
         for texts, got, st in zip(recs, pairs, status):
             if got is None:
                 declined += 1
@@ -146,7 +146,7 @@ def test_mixed_numeric_fields_are_declined():
     records = [[json.dumps({"v": 0}), json.dumps({"v": False}), json.dumps({"v": 1})],
                [json.dumps({"v": 1}), json.dumps({"v": "1"}), json.dumps({"v": 1})],
                [json.dumps({"v": 1}), json.dumps({"v": None}), json.dumps({"v": 2})]]
-    pairs, status = jsongpu_async_with_oracle(records)
+    pairs, status = jsongpu_with_oracle(records, flags=K.JSON_NUMERIC_MEDOID)
     assert pairs[0] is None and pairs[1] is None and status[0] == status[1] == 11  # D_MIXED_TYPES
     assert pairs[2] is not None
 

@@ -12,7 +12,8 @@ from k_llms_b200 import _native as K
 from k_llms_b200.utils import consensus_utils as CU
 from k_llms_b200.utils import consolidation as C
 from oracle import columnar as OC
-from tests.async_native_oracle import cells_of, golden_cases, jsongpu_async_with_oracle, numeric_medoid
+from tests.async_native_oracle import cells_of, golden_cases, numeric_medoid
+from tests.helpers import jsongpu_with_oracle
 from tests.test_async_native_host_logic import _completion, random_numeric_groups
 
 pytestmark = pytest.mark.gpu
@@ -102,7 +103,7 @@ def _fuzz_records(n, count, seed):
 def test_device_path_matches_its_host_phases(n, weighted, monkeypatch):
     recs = _fuzz_records(n, 300, 777 + n)
     seq = (-np.random.default_rng(n).exponential(3.0, len(recs) * n)).astype(np.float32) if weighted else None
-    exp_pairs, exp_status = jsongpu_async_with_oracle(recs, seq)
+    exp_pairs, exp_status = jsongpu_with_oracle(recs, seq, flags=K.JSON_NUMERIC_MEDOID)
     for chunk_mb in (None, 1):
         pairs, status, why = _packed(recs, seq, chunk_mb, monkeypatch)
         assert [s != 0 for s in status] == [s != 0 for s in exp_status]

@@ -22,7 +22,7 @@ from tests.helpers import boundary_texts, general_and_mutated_records, jsongpu_w
 from tests.test_gpu_json import _expected
 from tests.test_json_fuzz import _records
 from tests.test_jsongpu_host_logic import assert_parsed_like_cpython, parse_doubles
-from tests.test_weighted_host_logic import _seq, jsongpu_weighted_with_oracle
+from tests.test_weighted_host_logic import _seq
 
 pytestmark = pytest.mark.gpu
 
@@ -147,7 +147,7 @@ def test_json_fuzz_on_the_device(monkeypatch, weighted):
         n = len(recs[0])
         seq = np.concatenate([_seq(rng, n) for _ in recs]).astype(np.float32) if weighted else None
         got, status, why, _ = _run_packed(recs, seq=seq)
-        host, host_status = jsongpu_weighted_with_oracle(recs, seq) if weighted else jsongpu_with_oracle(recs)
+        host, host_status = jsongpu_with_oracle(recs, seq) if weighted else jsongpu_with_oracle(recs)
         assert [p is None for p in got] == [s != 0 for s in host_status], label
         assert (why[status != 0] != 0).all(), label
         accepted = 0

@@ -18,7 +18,6 @@ from tests.test_async_native_host_logic import _completion
 from tests.test_gpu_json import _expected
 from tests.test_jsongpu_host_logic import _shaped_record, s32_texts
 from tests.test_jsongpu_union_host_logic import ACCEPTED, DECLINED, union_record, union_records
-from tests.union_oracle import jsongpu_union_with_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -36,7 +35,7 @@ def _run(records, flags=0, seq=None, key_union=True):
 
 def test_union_records_count_vote():
     for n, recs in union_records(101, 1400).items():
-        exp, exp_status = jsongpu_union_with_oracle(recs)
+        exp, exp_status = jsongpu_with_oracle(recs, flags=K.JSON_KEY_UNION)
         host = K.consolidate_json(recs)
         for flags in (0, K.JSON_DEVICE_ONLY):
             pairs, status, why, stats = _run(recs, flags)
@@ -55,12 +54,12 @@ def test_union_records_weighted_and_async_medoid():
     rng = np.random.default_rng(3)
     for n, recs in union_records(202, 600, ns=(2, 3, 5, 8, 16, 33, 64)).items():
         seq = (-rng.exponential(4.0, len(recs) * n)).astype(np.float32)
-        exp, _ = jsongpu_union_with_oracle(recs, seq)
+        exp, _ = jsongpu_with_oracle(recs, seq, flags=K.JSON_KEY_UNION)
         pairs, status, _, stats = _run(recs, seq=seq)
         assert status == [0] * len(recs) and stats["n_device"] == len(recs)
         assert pairs == exp, n
         for s in (None, seq):
-            exp, exp_status = jsongpu_union_with_oracle(recs, s, numeric_medoid=True)
+            exp, exp_status = jsongpu_with_oracle(recs, s, flags=K.JSON_KEY_UNION | K.JSON_NUMERIC_MEDOID)
             pairs, status, why, stats = _run(recs, K.JSON_NUMERIC_MEDOID, s)
             assert why == [int(x) for x in exp_status] and not any(status) and stats["n_device"] == len(recs), n
             assert pairs == exp, n
@@ -85,7 +84,7 @@ def test_mixed_chunks(monkeypatch):
     plain = s32_texts(4000, 8, 5)
     only = [union_record(rng, 8) for _ in range(3000)]
     recs = mixed + plain + only
-    exp, exp_status = jsongpu_union_with_oracle(recs)
+    exp, exp_status = jsongpu_with_oracle(recs, flags=K.JSON_KEY_UNION)
     monkeypatch.setenv("KC_JSON_CHUNK_MB", "64")
     big = _run(recs, K.JSON_DEVICE_ONLY)
     monkeypatch.setenv("KC_JSON_CHUNK_MB", "1")

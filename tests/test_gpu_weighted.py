@@ -9,8 +9,8 @@ import pytest
 from oracle import columnar as OC
 from oracle import consensus_py as O
 from tests import weighted_oracle as W
-from tests.helpers import same
-from tests.test_weighted_host_logic import _completion, _flat_records, _seq, _wrapped, jsongpu_weighted_with_oracle, random_record
+from tests.helpers import jsongpu_with_oracle, same
+from tests.test_weighted_host_logic import _completion, _flat_records, _seq, _wrapped, random_record
 
 pytestmark = pytest.mark.gpu
 EMBED = lambda texts: [[0.0] for _ in texts]  # noqa: E731
@@ -170,7 +170,7 @@ def test_weighted_device_json_path_matches_host_phases(n):
     rng = np.random.default_rng(700 + n)
     records = _flat_records(rng, 2000, n)
     seq = np.concatenate([_seq(rng, n) for _ in records]).astype(np.float32)
-    exp, status = jsongpu_weighted_with_oracle(records, seq)
+    exp, status = jsongpu_with_oracle(records, seq)
     blob, off, _ = K.pack_texts(records)
     res = K.consolidate_json_packed_weighted(blob, off, n, seq)
     try:

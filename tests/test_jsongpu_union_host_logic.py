@@ -10,13 +10,13 @@ import random
 import numpy as np
 import pytest
 
+from k_llms_b200._native import JSON_KEY_UNION, JSON_NUMERIC_MEDOID
 from oracle import consensus_py as O
 from tests import weighted_oracle as W
 from tests.helpers import jsongpu_with_oracle
 from tests.test_async_native_host_logic import oracle_kernels, python_async  # noqa: F401  (a fixture)
 from tests.test_gpu_json import _expected
 from tests.test_weighted_host_logic import EMBED
-from tests.union_oracle import jsongpu_union_with_oracle
 
 KEYS = ["zeta", "Alpha", "b", "a", "aa", "k1", "k10", "k2", "Z", "id", "name", "addr"]
 # short phrases only: two strings over 50 characters are the embeddings service's, which every path declines
@@ -110,7 +110,7 @@ def _differ_in_shape(texts):
 def test_union_records_on_the_device_path():
     on_union = 0
     for _n, recs in union_records(101, 1400).items():
-        pairs, status = jsongpu_union_with_oracle(recs)
+        pairs, status = jsongpu_with_oracle(recs, flags=JSON_KEY_UNION)
         for texts, got, st in zip(recs, pairs, status):
             assert st == 0, (texts, st)
             on_union += _differ_in_shape(texts)
@@ -120,7 +120,7 @@ def test_union_records_on_the_device_path():
 
 def test_union_records_under_the_async_medoid(oracle_kernels):  # noqa: F811
     for _n, recs in union_records(202, 500, ns=(2, 3, 5, 8, 16)).items():
-        pairs, status = jsongpu_union_with_oracle(recs, numeric_medoid=True)
+        pairs, status = jsongpu_with_oracle(recs, flags=JSON_KEY_UNION | JSON_NUMERIC_MEDOID)
         for texts, got, st in zip(recs, pairs, status):
             assert st == 0, (texts, st)
             assert got == python_async(texts), texts
@@ -132,7 +132,7 @@ def test_union_records_weighted():
         n = len(recs[0])
         seq = (-rng.exponential(4.0, len(recs) * n)).astype(np.float32)
         seq[:n] = -1.5  # equal sums: the count winner
-        pairs, status = jsongpu_union_with_oracle(recs, seq)
+        pairs, status = jsongpu_with_oracle(recs, seq, flags=JSON_KEY_UNION)
         for r, (texts, got, st) in enumerate(zip(recs, pairs, status)):
             assert st == 0, (texts, st)
             contents = [json.loads(t) for t in texts]
@@ -147,9 +147,9 @@ def test_same_shape_records_are_untouched_and_mixed_batches_agree():
     recs = []
     for i in range(300):
         recs.append(_shaped_record(rng, 5) if i % 3 else union_record(rng, 5))
-    pairs, status = jsongpu_union_with_oracle(recs)
+    pairs, status = jsongpu_with_oracle(recs, flags=JSON_KEY_UNION)
     for texts, got, st in zip(recs, pairs, status):
-        alone, st1 = jsongpu_union_with_oracle([texts])
+        alone, st1 = jsongpu_with_oracle([texts], flags=JSON_KEY_UNION)
         assert (got, st) == (alone[0], st1[0]), texts
         if got is not None:
             assert got == _expected(texts)
@@ -192,14 +192,14 @@ DECLINED = {  # name: (texts, D_* code)
 @pytest.mark.parametrize("name", list(ACCEPTED))
 def test_union_edge_accepted(name):
     texts = ACCEPTED[name]
-    (got,), (st,) = jsongpu_union_with_oracle([texts])
+    (got,), (st,) = jsongpu_with_oracle([texts], flags=JSON_KEY_UNION)
     assert st == 0 and got == _expected(texts), (name, st, got)
 
 
 @pytest.mark.parametrize("name", list(DECLINED))
 def test_union_edge_declined(name):
     texts, why = DECLINED[name]
-    (got,), (st,) = jsongpu_union_with_oracle([texts])
+    (got,), (st,) = jsongpu_with_oracle([texts], flags=JSON_KEY_UNION)
     assert got is None and st == why, (name, st)
 
 
@@ -231,7 +231,7 @@ def test_declines_what_it_does_not_model_after_the_union():
         "trailing junk": ['{"a": 1} x', '{"a": 1}'],
         "empty content": ['{"a": 1}', ''],
     }
-    pairs, status = jsongpu_union_with_oracle(list(cases.values()))
+    pairs, status = jsongpu_with_oracle(list(cases.values()), flags=JSON_KEY_UNION)
     for (name, _), got, st in zip(cases.items(), pairs, status):
         assert got is None and 0 < st < 0xFF, (name, st)
 
@@ -240,7 +240,7 @@ def test_without_the_flag_nothing_changes():
     """The same records without KC_JSON_KEY_UNION: the records whose candidates differ in shape are declined with the reasons A1
     gave before the union round existed, and every other record comes out as it does with the flag."""
     recs = [t for _n, group in union_records(404, 300, ns=(3,)).items() for t in group]
-    with_flag, st_flag = jsongpu_union_with_oracle(recs)
+    with_flag, st_flag = jsongpu_with_oracle(recs, flags=JSON_KEY_UNION)
     without, st = jsongpu_with_oracle(recs)
     declined = 0
     for texts, a, b, s_flag, s in zip(recs, with_flag, without, st_flag, st):

@@ -10,7 +10,7 @@ import pytest
 from oracle import columnar as OC
 from oracle import consensus_py as O
 from tests import weighted_oracle as W
-from tests.helpers import same
+from tests.helpers import jsongpu_with_oracle, same
 
 EMBED = lambda texts: [[0.0] for _ in texts]  # noqa: E731
 
@@ -99,57 +99,9 @@ def _oracle_run(plan, device=None):
     return out
 
 
-def jsongpu_weighted_with_oracle(records, seq):
-    """The WEIGHTED device JSON path's phases instantiated on the host (kc_debug_jsongpu_plan -> group records -> the C oracle's
-    K3b in kc_weighted_vote_groups_i8's place, K2 / K4 oracles -> kc_debug_jsongpu_emit_weighted).  seq float32 [R*n].
-    Returns (pairs, status) like tests.helpers.jsongpu_with_oracle."""
-    import ctypes as c
-    from k_llms_b200 import _native as K
-    lib = K.load()
-    R = len(records)
-    if R == 0:
-        return [], []
-    blob, off, n = K.pack_texts(records, pinned=False)
-    seq = np.asarray(seq, dtype=np.float32).reshape(R, n)
-    h = c.c_void_p()
-    K.check(lib.kc_debug_jsongpu_plan(blob.ctypes.data, off.ctypes.data, R, n, c.byref(h)))
-    try:
-        vc, nc, st, gr = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_void_p()
-        gv, gx = c.c_int64(), c.c_int64()
-        K.check(lib.kc_debug_jsongpu_inputs(h, c.byref(vc), c.byref(gv), c.byref(nc), c.byref(gx), c.byref(st)))
-        K.check(lib.kc_debug_jsongpu_group_records(h, c.byref(gr)))
-        vmeta, vweight = np.zeros(max(gv.value, 1), dtype=np.uint32), np.zeros(max(gv.value, 1), dtype=np.float32)
-        nvalue, nmeta = np.zeros(max(gx.value, 1), dtype=np.float64), np.zeros(max(gx.value, 1), dtype=np.uint32)
-        if gv.value:
-            codes = np.ctypeslib.as_array(c.cast(vc, c.POINTER(c.c_int8)), shape=(gv.value, n)).astype(np.int32)
-            rec = np.ctypeslib.as_array(c.cast(gr, c.POINTER(c.c_int32)), shape=(gv.value,)).copy()
-            assert (rec >= 0).all() and (rec < R).all()
-            _, vmeta, vweight = OC.weighted_vote(codes[:, None, :], seq[rec])
-        if gx.value:
-            nvalue, nmeta = OC.numeric(np.ctypeslib.as_array(c.cast(nc, c.POINTER(c.c_double)), shape=(gx.value, n)).copy())
-        mc, so, go, gm = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_int64()
-        K.check(lib.kc_debug_jsongpu_medoid_inputs(h, c.byref(mc), c.byref(so), c.byref(go), c.byref(gm)))
-        midx, mavg = np.zeros(max(gm.value, 1), dtype=np.int32), np.zeros(max(gm.value, 1), dtype=np.float64)
-        if gm.value:
-            OC.lib().ko_medoid_str(mc, so, go, gm.value, midx.ctypes.data, mavg.ctypes.data)
-        K.check(lib.kc_debug_jsongpu_set_medoid(h, midx.ctypes.data, mavg.ctypes.data))
-        pc, po, pl, plo = c.c_void_p(), c.c_void_p(), c.c_void_p(), c.c_void_p()
-        K.check(lib.kc_debug_jsongpu_emit_weighted(h, vmeta.ctypes.data, vweight.ctypes.data, nvalue.ctypes.data, nmeta.ctypes.data,
-                                                   c.byref(pc), c.byref(po), c.byref(pl), c.byref(plo)))
-        status = np.ctypeslib.as_array(c.cast(st, c.POINTER(c.c_uint8)), shape=(R,)).copy()
-        co = np.ctypeslib.as_array(c.cast(po, c.POINTER(c.c_int64)), shape=(R + 1,))
-        lo = np.ctypeslib.as_array(c.cast(plo, c.POINTER(c.c_int64)), shape=(R + 1,))
-        pairs = [None if status[r] else (c.string_at(pc.value + int(co[r]), int(co[r + 1] - co[r])).decode("ascii"),
-                                         c.string_at(pl.value + int(lo[r]), int(lo[r + 1] - lo[r])).decode("ascii")) for r in range(R)]
-        return pairs, list(status)
-    finally:
-        lib.kc_debug_jsongpu_free(h)
-
-
-def _oracle_native_consolidate(records, rel_eps, abs_eps, device=0, seq_logprobs=None, counts=None):
+def _oracle_native_consolidate(records, rel_eps, abs_eps, device=0, seq_logprobs=None, counts=None, flags=0):
     """consolidation._native_consolidate with the device JSON path's phases on the host and the oracle in the kernels' place."""
-    from tests.helpers import jsongpu_with_oracle
-    pairs, _ = jsongpu_with_oracle(records) if seq_logprobs is None else jsongpu_weighted_with_oracle(records, seq_logprobs)
+    pairs, _ = jsongpu_with_oracle(records, seq_logprobs, flags=flags)
     if counts is not None:
         counts["device"] = counts.get("device", 0) + sum(p is not None for p in pairs)
     return pairs
@@ -436,13 +388,12 @@ def _flat_records(rng, R, n):
 def test_weighted_device_phases_match_planner(oracle_kernels, n):
     """kc_consolidate_json_packed_weighted's phases on the host (oracle in K3b's place) against the weighted Python planner,
     byte for byte; the records it declines are exactly the ones the count-vote device path declines."""
-    from tests.helpers import jsongpu_with_oracle
     from k_llms_b200.utils.consensus_utils import ConsensusSettings
     from k_llms_b200.utils.consolidation import _aligned_sync, _format_consensus_content, _safe_parse_content
     rng = np.random.default_rng(400 + n)
     records = _flat_records(rng, 300, n)
     seq = np.concatenate([_seq(rng, n) for _ in records]).astype(np.float32)
-    pairs, status = jsongpu_weighted_with_oracle(records, seq)
+    pairs, status = jsongpu_with_oracle(records, seq)
     _, status_count = jsongpu_with_oracle(records)
     assert [s != 0 for s in status] == [s != 0 for s in status_count]
     assert sum(p is not None for p in pairs) > 150
