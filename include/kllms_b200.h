@@ -367,6 +367,14 @@ void kc_free_strings(char **arr, int64_t count);
  *                     missing sub-object where another candidate holds an object) stay on the device: the key-union round
  *                     consolidates them as the reference's pre-pass aligns them (missing -> None, None -> an object of Nones).
  *                     Without it they are declined as before.  The client functions set it.
+ *            KC_JSON_LISTS: records with list fields stay on the device through a list round inside the same call.  The first
+ *                     round marks a record in which some candidate holds a list and no candidate is declined for another reason;
+ *                     the alignment pre-pass H2 (kc_align_json_batch, host threads) aligns the marked records; the device
+ *                     consolidates the aligned texts with list nodes (`"key": [...]`, elements in aligned order) in an aligned
+ *                     round on the same streams and chunking, and their results take the records' places.  A record H2
+ *                     declines keeps status 1 with why = 15 (D_ALIGN); what the aligned round declines follows the route of any
+ *                     declined record (the host path, with the original texts).  Without it a list declines the record as before
+ *                     (why = 4, D_NESTED).  The client functions set it.
  *   *out     result handle: one text blob + per-record spans (kc_json_result_view), released with kc_json_result_free
  * status per record: 0 = consolidated on the device, 2 = consolidated by the host path, 1 = needs the Python path.
  * Texts are byte-identical to the reference's json.dumps output.  Re-entrant (pooled per-call streams and buffers).
@@ -374,6 +382,7 @@ void kc_free_strings(char **arr, int64_t count);
 #define KC_JSON_DEVICE_ONLY 1u
 #define KC_JSON_NUMERIC_MEDOID 2u
 #define KC_JSON_KEY_UNION 4u
+#define KC_JSON_LISTS 8u
 typedef struct kc_json_result kc_json_result;
 typedef struct {
     int64_t n_records, n_device, n_host, n_python; /* where the records were consolidated */
@@ -403,7 +412,9 @@ void kc_json_result_free(kc_json_result *res);
  * kc_json_emit, so the CPU tests can put the oracle in K1 / K2's place.  Not a product path. */
 typedef struct kc_debug_jsongpu kc_debug_jsongpu;
 int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, kc_debug_jsongpu **out);
-/* the same with the flags of kc_consolidate_json_packed that change the phases (KC_JSON_NUMERIC_MEDOID, KC_JSON_KEY_UNION) */
+/* the same with the flags of kc_consolidate_json_packed that change the phases (KC_JSON_NUMERIC_MEDOID, KC_JSON_KEY_UNION,
+ * KC_JSON_LISTS: the list round's alignment runs on the host inside the plan, the aligned round's groups follow the first
+ * round's in the input hooks, and the emit puts their texts and statuses at the call's records) */
 int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, uint32_t flags,
                                 kc_debug_jsongpu **out);
 int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells, int64_t *n_vote_groups, const double **num_cells,

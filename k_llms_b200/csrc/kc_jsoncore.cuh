@@ -23,16 +23,20 @@ namespace js {
 typedef unsigned __int128 u128;
 
 // value kinds of a token (JSON scalar types; nested values and non-standard tokens make the scanner decline)
-// K_OPEN / K_CLOSE: a nested object's `"key": {` and its `}` — structure tokens between which the object's members follow
-enum : uint8_t { K_NULL = 0, K_TRUE = 1, K_FALSE = 2, K_INT = 3, K_FLOAT = 4, K_STR = 5, K_OPEN = 6, K_CLOSE = 7 };
+// K_OPEN / K_CLOSE: a nested object's `"key": {` and its `}` — structure tokens between which the object's members follow;
+// K_LOPEN / K_LCLOSE: a list's `"key": [` and its `]` (only when the scanner is asked for list nodes), its elements between them
+enum : uint8_t { K_NULL = 0, K_TRUE = 1, K_FALSE = 2, K_INT = 3, K_FLOAT = 4, K_STR = 5, K_OPEN = 6, K_CLOSE = 7, K_LOPEN = 8, K_LCLOSE = 9 };
+KC_HD inline bool is_open(uint32_t k) { return k == K_OPEN || k == K_LOPEN; }
+KC_HD inline bool is_close(uint32_t k) { return k == K_CLOSE || k == K_LCLOSE; }
 // which kernel decides a field (plan_leaf in kc_json.cpp; consensus_utils.py:1405-1411 vote, :1443-1453 numeric)
 // F_MEDOID: a string field that is not enum-like (some value has >= 3 words): the similarity medoid, K4 (:1221-1237)
-enum : uint8_t { F_ALLNULL = 0, F_VOTE_STR = 1, F_VOTE_BOOL = 2, F_NUMERIC = 3, F_MEDOID = 4, F_OPEN = 5, F_CLOSE = 6 };
-constexpr int32_t kMaxNesting = 8;  // nested objects below the top level; the depth lives in the token's flags (4 bits)
+enum : uint8_t { F_ALLNULL = 0, F_VOTE_STR = 1, F_VOTE_BOOL = 2, F_NUMERIC = 3, F_MEDOID = 4, F_OPEN = 5, F_CLOSE = 6, F_LOPEN = 7, F_LCLOSE = 8 };
+constexpr int32_t kMaxNesting = 8;  // nested objects and lists below the top level; the depth lives in the token's flags (4 bits)
 
 // One (field, candidate) cell of a record: views into the chunk's text.  Strings: the raw inner span (no quotes); raw == value
-// unless TOK_ESCAPED (keys: always, the scanner declines escapes in keys).  flags: bit 0 TOK_MULTIWORD, bit 1 TOK_ESCAPED, bits 4-7
-// the nesting depth of the member.  K_OPEN carries the key of the nested object, K_CLOSE no key.  TOK_MULTIWORD: the string has >= 3 whitespace-separated words (not enum-like, cu:1405).
+// unless TOK_ESCAPED (keys: always, the scanner declines escapes in keys).  flags: bit 0 TOK_MULTIWORD, bit 1 TOK_ESCAPED, bit 2
+// TOK_ELEM, bits 4-7 the nesting depth of the member.  K_OPEN / K_LOPEN carry the key of the nested value, K_CLOSE / K_LCLOSE no
+// key.  TOK_MULTIWORD: the string has >= 3 whitespace-separated words (not enum-like, cu:1405).  TOK_ELEM: a list element (no key).
 struct alignas(16) Tok {
     uint32_t vstart, vlen;  // value span, relative to the chunk's first byte
     uint32_t kstart;        // key span (inner)
@@ -43,12 +47,14 @@ struct alignas(16) Tok {
 constexpr uint8_t TOK_MULTIWORD = 1;
 KC_HD inline uint32_t tok_depth(const Tok &t) { return (uint32_t)t.flags >> 4; }  // 0 = a member of the top-level object
 constexpr uint8_t TOK_ESCAPED = 2;  // the span holds two-character escapes (\" \\ \/ \b \f \n \r \t), never \uXXXX
+constexpr uint8_t TOK_ELEM = 4;
 
-// why a record left the device path (diagnostics only; every non-zero code means "host path")
+// why a record left the device path (diagnostics only; every non-zero code means "host path").  D_ALIGN: the alignment
+// pre-pass of the list round declined the record (a pair of long strings for the embeddings service, non-ASCII text).
 enum : int32_t {
     D_OK = 0, D_NOT_OBJECT = 1, D_SYNTAX = 2, D_ESCAPE_OR_NON_ASCII = 3, D_NESTED = 4, D_NONSTANDARD_NUMBER = 5, D_TOO_MANY_FIELDS = 6,
     D_KEYS_DIFFER = 7, D_DUP_KEY = 8, D_SPECIAL_KEY = 9, D_MULTIWORD = 10, D_MIXED_TYPES = 11, D_NUMBER_RANGE = 12, D_EMPTY = 13,
-    D_TOO_LONG = 14,
+    D_TOO_LONG = 14, D_ALIGN = 15,
 };
 
 KC_HD inline bool is_json_ws(uint8_t c) { return c == ' ' || c == '\t' || c == '\n' || c == '\r'; }
@@ -79,8 +85,11 @@ KC_HD inline double bits_f64(uint64_t b) {
 // toks[j * stride] when toks != nullptr (spans are stored relative to `rel`: s == chunk + rel); a nested object is its K_OPEN
 // token, its members' tokens, its K_CLOSE token.  Returns the token count (>= 1) or -D_* — the scanner never guesses: whatever
 // it does not model exactly (\u escapes, non-ASCII, lists, NaN/Infinity, free text that the reference wraps as {"text": ...},
-// an empty object) is left to the host path.  *nested (optional): whether the object holds a nested object.
-KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, Tok *toks, int32_t stride, int32_t cap, bool *nested = nullptr) {
+// an empty object) is left to the host path.  *nested (optional): whether the object holds a nested object (or a list).
+// lists: `[` opens a list node (K_LOPEN, its elements keyless TOK_ELEM tokens one level deeper, K_LCLOSE) instead of declining
+// the record with D_NESTED; *has_list (optional): whether the text holds a list.
+KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, Tok *toks, int32_t stride, int32_t cap, bool *nested = nullptr,
+                                 bool lists = false, bool *has_list = nullptr) {
     uint32_t p = 0;
     while (p < len && is_json_ws(s[p])) ++p;
     if (p >= len) return -D_EMPTY;
@@ -90,32 +99,40 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
     if (p < len && s[p] == '}') return -D_EMPTY;  // {}: consensus of empty dicts — rare, host path
     int32_t j = 0;
     uint32_t depth = 0;
+    uint32_t in_list = 0;  // bit d: the members of depth d are list elements
     if (nested) *nested = false;
+    if (has_list) *has_list = false;
     for (;;) {
         while (p < len && is_json_ws(s[p])) ++p;
-        if (p >= len || s[p] != '"') return -D_SYNTAX;
-        ++p;
-        const uint32_t kstart = p;
-        for (;;) {
-            if (p >= len) return -D_SYNTAX;
-            const uint8_t c = s[p];
-            if (c == '"') break;
-            if (c < 0x20) return -D_SYNTAX;
-            if (c >= 0x80 || c == '\\') return -D_ESCAPE_OR_NON_ASCII;
-            ++p;
-        }
-        const uint32_t klen = p - kstart;
-        if (klen > 0xFFFFu) return -D_TOO_LONG;
-        ++p;
-        while (p < len && is_json_ws(s[p])) ++p;
-        if (p >= len || s[p] != ':') return -D_SYNTAX;
-        ++p;
-        while (p < len && is_json_ws(s[p])) ++p;
-        if (p >= len) return -D_SYNTAX;
+        const bool elem = (in_list >> depth) & 1u;
         Tok t;
-        t.kstart = rel + kstart;
-        t.klen = (uint16_t)klen;
         t.flags = 0;
+        if (elem) {
+            t.kstart = rel + p;
+            t.klen = 0;
+        } else {
+            if (p >= len || s[p] != '"') return -D_SYNTAX;
+            ++p;
+            const uint32_t kstart = p;
+            for (;;) {
+                if (p >= len) return -D_SYNTAX;
+                const uint8_t c = s[p];
+                if (c == '"') break;
+                if (c < 0x20) return -D_SYNTAX;
+                if (c >= 0x80 || c == '\\') return -D_ESCAPE_OR_NON_ASCII;
+                ++p;
+            }
+            const uint32_t klen = p - kstart;
+            if (klen > 0xFFFFu) return -D_TOO_LONG;
+            ++p;
+            while (p < len && is_json_ws(s[p])) ++p;
+            if (p >= len || s[p] != ':') return -D_SYNTAX;
+            ++p;
+            while (p < len && is_json_ws(s[p])) ++p;
+            t.kstart = rel + kstart;
+            t.klen = (uint16_t)klen;
+        }
+        if (p >= len) return -D_SYNTAX;
         const uint8_t c = s[p];
         if (c == '"') {
             ++p;
@@ -158,13 +175,38 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
             t.kind = K_OPEN;
             t.vstart = rel + p;
             t.vlen = 0;
-            t.flags = (uint8_t)(depth << 4);
+            t.flags = (uint8_t)((depth << 4) | (elem ? TOK_ELEM : 0));
             if (j >= cap) return -D_TOO_MANY_FIELDS;
             if (toks) toks[(int64_t)j * stride] = t;
             ++j;
             ++depth;
+            in_list &= ~(1u << depth);
             if (nested) *nested = true;
             continue;  // the object's first member
+        } else if (c == '[' && lists) {
+            ++p;
+            if ((int32_t)depth >= kMaxNesting) return -D_NESTED;
+            if (has_list) *has_list = true;
+            if (nested) *nested = true;
+            t.kind = K_LOPEN;
+            t.vstart = rel + p;
+            t.vlen = 0;
+            t.flags = (uint8_t)((depth << 4) | (elem ? TOK_ELEM : 0));
+            if (j >= cap) return -D_TOO_MANY_FIELDS;
+            if (toks) toks[(int64_t)j * stride] = t;
+            ++j;
+            while (p < len && is_json_ws(s[p])) ++p;
+            if (p >= len || s[p] != ']') {
+                ++depth;
+                in_list |= 1u << depth;
+                continue;  // the list's first element
+            }
+            ++p;  // [] : its K_LCLOSE follows at once, then whatever follows a value
+            t.kind = K_LCLOSE;
+            t.vstart = rel + p;
+            t.kstart = rel + p;
+            t.klen = 0;
+            t.flags = (uint8_t)(depth << 4);
         } else if (c == 't') {
             if (len - p < 4 || s[p + 1] != 'r' || s[p + 2] != 'u' || s[p + 3] != 'e') return -D_SYNTAX;
             t.kind = K_TRUE;
@@ -218,19 +260,20 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
         } else {
             return -D_SYNTAX;
         }
-        t.flags = (uint8_t)(t.flags | (depth << 4));
+        if (t.kind != K_LCLOSE) t.flags = (uint8_t)(t.flags | (depth << 4) | (elem ? TOK_ELEM : 0));
         if (j >= cap) return -D_TOO_MANY_FIELDS;
         if (toks) toks[(int64_t)j * stride] = t;
         ++j;
         bool done = false;
-        for (;;) {  // after a value: the next member, or the end of one or more objects
+        for (;;) {  // after a value: the next member, or the end of one or more objects / lists
             while (p < len && is_json_ws(s[p])) ++p;
             if (p >= len) return -D_SYNTAX;
             if (s[p] == ',') {
                 ++p;
                 break;
             }
-            if (s[p] != '}') return -D_SYNTAX;
+            const bool closes_list = (in_list >> depth) & 1u;
+            if (s[p] != (closes_list ? ']' : '}')) return -D_SYNTAX;
             ++p;
             if (depth == 0) {
                 done = true;
@@ -238,7 +281,7 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
             }
             --depth;
             Tok e;
-            e.kind = K_CLOSE;
+            e.kind = closes_list ? K_LCLOSE : K_CLOSE;
             e.vstart = rel + p;
             e.vlen = 0;
             e.kstart = rel + p;

@@ -122,7 +122,7 @@ struct Worker {
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[7] = {};
     DBuf text, off, fcount, slot, status, vbase, xbase, counters, win, vmeta, xvalue, xmeta, len_c, len_l, out_c, out_l, scan_tmp, mcount,
-        scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, seq, vweight, pend, plist, ucand, ubase, usize, utok, unode, umap;
+        scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, seq, vweight, pend, plist, ucand, ubase, usize, utok, unode, umap, lst;
     DBuf slot_buf[kSlotArrays];  // slot_arrays
     PBuf h_small;  // totals and counters (pinned so the small D2H copies are asynchronous)
     PBuf h_scan;   // the scanned record offsets and the statuses of a chunk
@@ -317,9 +317,11 @@ int union_round(Worker &w, Chunk &ch, int64_t P, size_t &T, int team, int grid, 
 
 // One chunk on one worker: records [r0, r1) of the batch.  h_seq (NULL: count votes): the batch's candidate sums [R][n], the
 // vote leaves are likelihood-weighted (K3b over ragged records in K1's place).  xmedoid (KC_JSON_NUMERIC_MEDOID): numeric fields
-// are similarity medoids (K5 in K2's place).
-int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, bool key_union, int64_t r0, int64_t r1, int32_t n,
-              double rel_eps, double abs_eps, int sm_count, kc_json_result &res, ChunkStage &st) {
+// are similarity medoids (K5 in K2's place).  lists: Chunk::lists.  dst (NULL: the identity): the result index of each record
+// of the batch (the aligned round's batch is the list records, in the order of their result indices).
+int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, bool key_union, uint8_t lists,
+              const int64_t *dst, int64_t r0, int64_t r1, int32_t n, double rel_eps, double abs_eps, int sm_count, kc_json_result &res,
+              ChunkStage &st) {
     const int64_t Rc = r1 - r0;
     const int64_t b0 = h_off[r0 * n], b1 = h_off[r1 * n];
     const size_t bytes = (size_t)(b1 - b0);
@@ -333,6 +335,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     R_(w.nest.reserve((size_t)Rc));
     R_(w.pend.reserve((size_t)Rc));
     R_(w.plist.reserve((size_t)Rc * 4));
+    if (lists) R_(w.lst.reserve((size_t)Rc));
     R_(w.vbase.reserve((size_t)Rc * 4));
     R_(w.xbase.reserve((size_t)Rc * 4));
     R_(w.counters.reserve(48));
@@ -370,6 +373,9 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     ch.len_l = w.len_l.as<int64_t>();
     ch.xmedoid = xmedoid;
     ch.key_union = key_union;
+    ch.lst = lists ? w.lst.as<uint8_t>() : nullptr;
+    ch.lists = lists;
+    ch.aligned0 = INT32_MAX;  // a chunk is in one round: Chunk::lists says which
 
     nvtxRangePushA("kc_json: H2D texts");
     KC_CUDA_I(cudaEventRecord(w.ev[0], s));
@@ -483,7 +489,8 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     const int64_t pos = res.used.fetch_add(need);
     if (pos + need > (int64_t)res.blob.cap) {  // the estimate of the output size was too small: leave the chunk to the host path
         res.used.fetch_sub(need);
-        for (int64_t r = r0; r < r1; ++r) {
+        for (int64_t i = r0; i < r1; ++i) {
+            const int64_t r = dst ? dst[i] : i;
             res.status[(size_t)r] = 1;
             res.why[(size_t)r] = (uint8_t)kc::js::D_TOO_LONG;
         }
@@ -495,7 +502,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     KC_CUDA_I(cudaStreamSynchronize(s));
     nvtxRangePop();
     for (int64_t i = 0; i < Rc; ++i) {
-        const int64_t r = r0 + i;
+        const int64_t r = dst ? dst[r0 + i] : r0 + i;
         res.status[(size_t)r] = h_status[i] ? 1 : 0;
         res.why[(size_t)r] = h_status[i];
         res.c_off[(size_t)r] = pos + h_scan_c[i];
@@ -510,6 +517,110 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     cudaEventElapsedTime(&ms, w.ev[3], w.ev[4]); st.emit += ms;
     cudaEventElapsedTime(&ms, w.ev[4], w.ev[5]); st.d2h += ms;
     return KC_OK;
+}
+
+}  // namespace
+
+namespace {
+
+// The list round's alignment: the alignment pre-pass H2 (kc_align_json_batch) on host threads for the records in idx, which
+// the first round marked D_LIST.  The aligned texts of the records it aligns are packed record-major into one blob from
+// alloc(bytes) (off: their offsets, blob-relative; dst: their record indices); the records it declines go to `declined`.
+// The element similarities of the list nodes run in one kc_alignsim pass on `device`; device < 0 runs that pass on ONE host
+// thread: many times slower on a batch, faster for a few records (DESIGN.md §10).
+template <class Alloc>
+int align_listed(const char *h_text, const int64_t *h_off, int32_t n, int device, int32_t threads, const std::vector<int64_t> &idx, const Alloc &alloc,
+                 char *&blob, std::vector<int64_t> &off, std::vector<int64_t> &dst, std::vector<int64_t> &declined) {
+    const int64_t L = (int64_t)idx.size();
+    std::vector<const char *> texts((size_t)(L * n));
+    std::vector<int64_t> lens((size_t)(L * n));
+    for (int64_t i = 0; i < L; ++i)
+        for (int32_t c = 0; c < n; ++c) {
+            const int64_t k = idx[(size_t)i] * n + c;
+            texts[(size_t)(i * n + c)] = h_text + h_off[k];
+            lens[(size_t)(i * n + c)] = h_off[k + 1] - h_off[k];
+        }
+    std::vector<char *> out((size_t)(L * n), nullptr);
+    std::vector<int32_t> st((size_t)L, 0);
+    if (const int rc = kc_align_json_batch(texts.data(), lens.data(), L, n, /*min_support_ratio=*/0.51, device, threads, out.data(), st.data(), nullptr)) {
+        kc_free_strings(out.data(), L * n);  // whatever it allocated before it failed
+        return rc;
+    }
+    off.assign(1, 0);
+    dst.clear();
+    declined.clear();
+    for (int64_t i = 0; i < L; ++i) {
+        if (st[(size_t)i] != 0) {
+            declined.push_back(idx[(size_t)i]);
+            continue;
+        }
+        dst.push_back(idx[(size_t)i]);
+        for (int32_t c = 0; c < n; ++c) off.push_back(off.back() + (int64_t)strlen(out[(size_t)(i * n + c)]));
+    }
+    blob = alloc((size_t)off.back());
+    int rc = blob ? KC_OK : kc_fail(KC_ENOMEM, "kc_consolidate_json_packed: cannot allocate %lld bytes of aligned texts", (long long)off.back());
+    for (int64_t i = 0, k = 0; i < L && !rc; ++i) {
+        if (st[(size_t)i] != 0) continue;
+        for (int32_t c = 0; c < n; ++c, ++k) memcpy(blob + off[(size_t)k], out[(size_t)(i * n + c)], (size_t)(off[(size_t)k + 1] - off[(size_t)k]));
+    }
+    kc_free_strings(out.data(), L * n);
+    return rc;
+}
+
+// The list round of a call (KC_JSON_LISTS): the records the first round marked D_LIST are aligned (align_listed) and the
+// aligned texts consolidated by run_round with list nodes (Chunk::lists = 2) on the same workers, streams and chunking; their
+// results land at the records' own indices.  What H2 declines keeps status 1 with D_ALIGN.
+template <class Round>
+int list_round(kc_json_result &res, const char *h_text, const int64_t *h_off, const float *h_seq, int32_t n, int device, int32_t threads,
+               Round &run_round) {
+    std::vector<int64_t> idx;
+    for (int64_t r = 0; r < res.R; ++r)
+        if (res.status[(size_t)r] && res.why[(size_t)r] == kc::js::D_LIST) idx.push_back(r);
+    if (idx.empty()) return KC_OK;
+    PinnedBlob texts;
+    auto alloc = [&](size_t bytes) {
+        texts = acquire_blob(bytes + 16);
+        return texts.p;
+    };
+    char *blob = nullptr;
+    std::vector<int64_t> off, dst, declined;
+    // the similarity pass on the device pays a launch, an allocation and a synchronisation per call: a handful of records
+    // (single requests) align faster with the pass on the host
+    const int sim_device = idx.size() >= 64 ? device : -1;
+    int rc = align_listed(h_text, h_off, n, sim_device, threads, idx, alloc, blob, off, dst, declined);
+    for (int64_t r : declined) res.why[(size_t)r] = kc::js::D_ALIGN;
+    const int64_t M = (int64_t)dst.size();
+    if (!rc && M) {
+        std::vector<float> seq;
+        if (h_seq) {  // the aligned records' candidate sums, in the aligned batch's order
+            seq.resize((size_t)(M * n));
+            for (int64_t i = 0; i < M; ++i) memcpy(&seq[(size_t)(i * n)], h_seq + dst[(size_t)i] * n, (size_t)n * 4);
+        }
+        // grow the result blob to what the first round used plus the aligned round's output (no chunk is in flight between the
+        // rounds).  Sized from each record's structure, not its length: a leaf's value and confidence print in at most 24
+        // characters each (float.__repr__) plus their separators, so a list of small ints has likelihoods several times its text
+        size_t est = 4096;  // small: a single request's aligned round fits the pooled ~1 MiB blob its first round got
+        for (int64_t i = 0; i < M; ++i) {
+            const char *t = blob + off[(size_t)(i * n)];
+            const int64_t len = off[(size_t)(i * n + 1)] - off[(size_t)(i * n)];
+            int64_t tokens = 1;  // every value ends at a ',' or a closer; every closer is a token of its own
+            for (int64_t k = 0; k < len; ++k) tokens += t[k] == ',' ? 1 : (t[k] == ']' || t[k] == '}') ? 2 : 0;
+            est += (size_t)(2 * len + 32 * tokens);
+        }
+        const size_t need = (size_t)res.used.load() + est;
+        if (need > res.blob.cap) {
+            PinnedBlob bigger = acquire_blob(need);
+            if (!bigger.p) rc = kc_fail(KC_ENOMEM, "kc_consolidate_json_packed: cannot grow the pinned output blob to %zu bytes", need);
+            else {
+                memcpy(bigger.p, res.blob.p, (size_t)res.used.load());
+                release_blob(res.blob);
+                res.blob = bigger;
+            }
+        }
+        if (!rc) rc = run_round(blob, off.data(), h_seq ? seq.data() : nullptr, M, (uint8_t)2, dst.data());
+    }
+    release_blob(texts);
+    return rc;
 }
 
 }  // namespace
@@ -561,67 +672,78 @@ int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_
     // chunks of ~chunk_mb of text; records are never split
     size_t chunk_bytes = (size_t)64 << 20;
     if (const char *e = getenv("KC_JSON_CHUNK_MB")) chunk_bytes = (size_t)std::min(1024, std::max(1, atoi(e))) << 20;  // K4's CSR offsets are int32
-    std::vector<int64_t> cuts{0};
-    {
+    int max_workers = 3;
+    if (const char *e = getenv("KC_JSON_STREAMS")) max_workers = std::max(1, std::min(8, atoi(e)));
+    int n_chunks = 0, n_streams = 0;
+    std::vector<ChunkStage> stages((size_t)max_workers);
+    // one round of chunks over a batch of Rb records (the call's, or the aligned round's), several chunks in flight
+    auto run_round = [&](const char *text, const int64_t *off, const float *seq, int64_t Rb, uint8_t lists, const int64_t *dst) -> int {
+        std::vector<int64_t> cuts{0};
         int64_t r = 0;
-        while (r < R) {
+        while (r < Rb) {
             // records are a few KB: advance by estimate, then adjust
-            const int64_t start = h_off[r * n];
-            int64_t lo = r + 1, hi = R;
+            const int64_t start = off[r * n];
+            int64_t lo = r + 1, hi = Rb;
             while (lo < hi) {  // largest r1 with bytes(r, r1) <= chunk_bytes (at least one record)
                 const int64_t mid = lo + (hi - lo + 1) / 2;
-                if ((size_t)(h_off[mid * n] - start) <= chunk_bytes) lo = mid;
+                if ((size_t)(off[mid * n] - start) <= chunk_bytes) lo = mid;
                 else hi = mid - 1;
             }
             r = lo;
             cuts.push_back(r);
         }
-    }
-    const int n_chunks = (int)cuts.size() - 1;
-    int n_workers = 3;
-    if (const char *e = getenv("KC_JSON_STREAMS")) n_workers = std::max(1, std::min(8, atoi(e)));
-    n_workers = std::max(1, std::min(n_workers, n_chunks));
-    std::vector<Worker *> workers;
-    for (int i = 0; i < n_workers; ++i) workers.push_back(acquire_worker(device));
-    std::vector<int> rcs((size_t)n_workers, KC_OK);
-    std::vector<std::string> errs((size_t)n_workers);
-    std::vector<ChunkStage> stages((size_t)n_workers);
-    std::atomic<int> next{0};
-    auto body = [&](int wi) {
-        cudaSetDevice(device);
-        Worker &w = *workers[(size_t)wi];
-        int rc = w.init(device);
-        while (!rc) {
-            const int k = next.fetch_add(1);
-            if (k >= n_chunks) break;
-            rc = run_chunk(w, h_text, h_off, h_seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, (flags & KC_JSON_KEY_UNION) != 0, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps,
-                           abs_eps, sm_count, *res, stages[(size_t)wi]);
+        const int chunks = (int)cuts.size() - 1;
+        const int n_workers = std::max(1, std::min(max_workers, chunks));
+        n_chunks += chunks;
+        n_streams = std::max(n_streams, n_workers);
+        std::vector<Worker *> workers;
+        for (int i = 0; i < n_workers; ++i) workers.push_back(acquire_worker(device));
+        std::vector<int> rcs((size_t)n_workers, KC_OK);
+        std::vector<std::string> errs((size_t)n_workers);
+        std::atomic<int> next{0};
+        auto body = [&](int wi) {
+            cudaSetDevice(device);
+            Worker &w = *workers[(size_t)wi];
+            int rc = w.init(device);
+            while (!rc) {
+                const int k = next.fetch_add(1);
+                if (k >= chunks) break;
+                rc = run_chunk(w, text, off, seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, (flags & KC_JSON_KEY_UNION) != 0, lists, dst, cuts[(size_t)k],
+                               cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res, stages[(size_t)wi]);
+            }
+            if (rc) {
+                cudaStreamSynchronize(w.stream);
+                errs[(size_t)wi] = kc_last_error();
+            }
+            rcs[(size_t)wi] = rc;
+        };
+        if (n_workers == 1) {
+            body(0);
+        } else {
+            std::vector<std::thread> pool;
+            for (int i = 0; i < n_workers; ++i) pool.emplace_back(body, i);
+            for (auto &t : pool) t.join();
         }
-        if (rc) {
-            cudaStreamSynchronize(w.stream);
-            errs[(size_t)wi] = kc_last_error();
-        }
-        rcs[(size_t)wi] = rc;
+        for (Worker *w : workers) release_worker(w);
+        for (int i = 0; i < n_workers; ++i)
+            if (rcs[(size_t)i]) return kc_fail(rcs[(size_t)i], "%s", errs[(size_t)i].c_str());
+        return KC_OK;
     };
-    if (n_workers == 1) {
-        body(0);
-    } else {
-        std::vector<std::thread> pool;
-        for (int i = 0; i < n_workers; ++i) pool.emplace_back(body, i);
-        for (auto &t : pool) t.join();
-    }
-    for (Worker *w : workers) release_worker(w);
-    int rc = KC_OK;
-    for (int i = 0; i < n_workers && !rc; ++i)
-        if (rcs[(size_t)i]) rc = kc_fail(rcs[(size_t)i], "%s", errs[(size_t)i].c_str());
+    const bool lists = (flags & KC_JSON_LISTS) != 0;
+    int rc = run_round(h_text, h_off, h_seq, R, lists ? 1 : 0, nullptr);
+    if (!rc && lists) rc = list_round(*res, h_text, h_off, h_seq, n, device, threads, run_round);
     const auto t_gpu = std::chrono::steady_clock::now();
     // the records the device path declined: host path (H1), unless the caller only wants the device path
     int64_t n_declined = 0, n_host = 0;
     if (!rc) {
         std::vector<int64_t> idx;
-        for (int64_t r = 0; r < R; ++r)
-            if (res->status[(size_t)r]) idx.push_back(r);
-        n_declined = (int64_t)idx.size();
+        for (int64_t r = 0; r < R; ++r) {
+            if (!res->status[(size_t)r]) continue;
+            ++n_declined;
+            // what the list round's alignment declined, H1 would decline too: it runs the same pre-pass (align_values, the
+            // same min_support_ratio) on the same texts before anything else
+            if (res->why[(size_t)r] != kc::js::D_ALIGN) idx.push_back(r);
+        }
         if (!idx.empty() && !(flags & KC_JSON_DEVICE_ONLY)) {
             const int64_t D = (int64_t)idx.size();
             std::vector<const char *> texts((size_t)(D * n));
@@ -683,7 +805,7 @@ int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_
     s.input_bytes = total_bytes;
     s.output_bytes = res->used.load();
     s.chunks = n_chunks;
-    s.streams = n_workers;
+    s.streams = n_streams;
     for (auto &g : stages) {
         s.h2d_ms += g.h2d;
         s.plan_ms += g.plan;
@@ -753,6 +875,12 @@ struct kc_debug_jsongpu {
     std::vector<int32_t> mstr_off, mgrp_off;
     std::vector<int64_t> len_c, len_l;
     std::vector<uint8_t> out_c, out_l;
+    std::vector<uint8_t> lst;
+    // KC_JSON_LISTS: records [R_out, R) are the aligned round's (record src[i - R_out] of the call); emit splices them back
+    int64_t R_out = 0;
+    std::vector<int64_t> src;
+    std::vector<int64_t> spliced_c, spliced_l;
+    std::vector<uint8_t> spliced_out_c, spliced_out_l;
     Chunk ch{};
 };
 
@@ -760,12 +888,13 @@ int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_re
     return kc_debug_jsongpu_plan_flags(h_text, h_off, n_records, n, 0u, out);
 }
 
-int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, uint32_t flags,
-                                kc_debug_jsongpu **out) {
-    if (!h_text || !h_off || !out || n < 2 || n > KC_MAX_CANDIDATES || n_records < 0) return KC_EINVAL;
-    kc_debug_jsongpu *h = new kc_debug_jsongpu;
-    const int64_t R = n_records;
+namespace {
+
+// the device phases of one chunk on the host, in run_chunk's order (union round included) up to A2; records [aligned0, R) in
+// the aligned round
+void plan_twin(kc_debug_jsongpu *h, const char *h_text, const int64_t *h_off, int64_t R, int32_t n, uint32_t flags, uint8_t lists, int32_t aligned0) {
     h->R = R;
+    h->R_out = R;
     h->n = n;
     h->off.assign(h_off, h_off + R * n + 1);
     h->text.assign((const uint8_t *)h_text + h_off[0], (const uint8_t *)h_text + h_off[R * n]);
@@ -774,6 +903,7 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     h->status.assign((size_t)R, 0);
     h->nest.assign((size_t)R, 0);
     h->pend.assign((size_t)R, 0);
+    h->lst.assign((size_t)R, 0);
     h->plist.assign((size_t)R + 1, -1);
     h->vbase.assign((size_t)R, 0);
     h->xbase.assign((size_t)R, 0);
@@ -803,6 +933,9 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     ch.len_l = h->len_l.data();
     ch.xmedoid = (flags & KC_JSON_NUMERIC_MEDOID) != 0;
     ch.key_union = (flags & KC_JSON_KEY_UNION) != 0;
+    ch.lst = h->lst.data();
+    ch.lists = lists;
+    ch.aligned0 = aligned0;
     for (int32_t r = 0; r < R; ++r) kc::js::count_record(ch, r);
     for (int64_t r = 0; r < R; ++r) h->slot[(size_t)r + 1] = h->slot[(size_t)r] + h->fcount[(size_t)r];
     const size_t T = h->slot[(size_t)R];
@@ -843,6 +976,56 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     ch.mstr_off = h->mstr_off.data();
     ch.mgrp_off = h->mgrp_off.data();
     for (int32_t r = 0; r < R; ++r) kc::js::medoid_step(ch, r, team);
+}
+
+}  // namespace
+
+// With KC_JSON_LISTS the twin runs the list round as consolidate_packed does: the first round finds the D_LIST records, H2
+// aligns them (align_listed), and the aligned texts are appended to the batch as records of the aligned round, planned in the
+// same chunk behind the call's records.  The batch is planned twice on purpose: the first plan only finds the D_LIST records,
+// and the second replans the call's records next to the aligned ones, so that all groups live in one set of input arrays
+// (the call's records plan the same both times).  Their groups follow the first round's in every input hook; emit splices their texts
+// and statuses back to the call's records.
+int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, uint32_t flags,
+                                kc_debug_jsongpu **out) {
+    if (!h_text || !h_off || !out || n < 2 || n > KC_MAX_CANDIDATES || n_records < 0) return KC_EINVAL;
+    const int64_t R = n_records;
+    kc_debug_jsongpu *h = new kc_debug_jsongpu;
+    const bool lists = (flags & KC_JSON_LISTS) != 0;
+    plan_twin(h, h_text, h_off, R, n, flags, lists ? 1 : 0, INT32_MAX);
+    std::vector<int64_t> idx;
+    for (int64_t r = 0; r < R && lists; ++r)
+        if (h->status[(size_t)r] == kc::js::D_LIST) idx.push_back(r);
+    if (idx.empty()) {
+        *out = h;
+        return KC_OK;
+    }
+    std::vector<char> aligned;
+    auto alloc = [&](size_t bytes) {
+        aligned.resize(bytes + 1);
+        return aligned.data();
+    };
+    char *blob = nullptr;
+    std::vector<int64_t> aoff, dst, declined;
+    if (const int rc = align_listed(h_text, h_off, n, -1, 0, idx, alloc, blob, aoff, dst, declined)) {
+        delete h;
+        return rc;
+    }
+    const int64_t M = (int64_t)dst.size(), base = h_off[R * n] - h_off[0];
+    std::vector<char> text(h_text + h_off[0], h_text + h_off[R * n]);
+    text.insert(text.end(), blob, blob + aoff.back());
+    std::vector<int64_t> off((size_t)((R + M) * n + 1));
+    for (int64_t k = 0; k <= R * n; ++k) off[(size_t)k] = h_off[k] - h_off[0];
+    for (int64_t k = 1; k <= M * n; ++k) off[(size_t)(R * n + k)] = base + aoff[(size_t)k];
+    delete h;
+    h = new kc_debug_jsongpu;
+    plan_twin(h, text.data(), off.data(), R + M, n, flags, 1, (int32_t)R);
+    h->R_out = R;
+    h->src = dst;
+    for (int64_t r : declined) h->status[(size_t)r] = kc::js::D_ALIGN;
+    int32_t *vrec = h->ch.vrec;  // the aligned records' vote groups weigh with their call records' candidate sums
+    for (uint64_t g = 0; g < h->counters[0]; ++g)
+        if (vrec[g] >= R) vrec[g] = (int32_t)dst[(size_t)(vrec[g] - R)];
     *out = h;
     return KC_OK;
 }
@@ -914,6 +1097,32 @@ int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_met
     ch.out_c = h->out_c.data();
     ch.out_l = h->out_l.data();
     for (int32_t r = 0; r < R; ++r) kc::js::write_step(ch, r, team);
+    if (h->R_out < R) {  // the list round: each aligned record's texts and status go to its call record
+        const int64_t Ro = h->R_out;
+        std::vector<int64_t> from((size_t)Ro);
+        for (int64_t r = 0; r < Ro; ++r) from[(size_t)r] = r;
+        for (int64_t i = 0; i < R - Ro; ++i) {
+            from[(size_t)h->src[(size_t)i]] = Ro + i;
+            h->status[(size_t)h->src[(size_t)i]] = h->status[(size_t)(Ro + i)];
+        }
+        auto splice = [&](const std::vector<int64_t> &o, const std::vector<uint8_t> &blob, std::vector<int64_t> &so, std::vector<uint8_t> &sb) {
+            so.assign((size_t)Ro + 1, 0);
+            sb.clear();
+            for (int64_t r = 0; r < Ro; ++r) {
+                const int64_t k = from[(size_t)r];
+                sb.insert(sb.end(), blob.begin() + o[(size_t)k], blob.begin() + o[(size_t)k + 1]);
+                so[(size_t)r + 1] = (int64_t)sb.size();
+            }
+            sb.push_back(0);
+        };
+        splice(h->len_c, h->out_c, h->spliced_c, h->spliced_out_c);
+        splice(h->len_l, h->out_l, h->spliced_l, h->spliced_out_l);
+        if (content) *content = (const char *)h->spliced_out_c.data();
+        if (content_off) *content_off = h->spliced_c.data();
+        if (likelihoods) *likelihoods = (const char *)h->spliced_out_l.data();
+        if (likelihoods_off) *likelihoods_off = h->spliced_l.data();
+        return KC_OK;
+    }
     if (content) *content = (const char *)h->out_c.data();
     if (content_off) *content_off = h->len_c.data();
     if (likelihoods) *likelihoods = (const char *)h->out_l.data();

@@ -24,6 +24,10 @@
 //                              duplicate keys and object-against-value declined) and reserves its rows  (read-back: union rows)
 //     U3  union_plan_kernel    lane c writes column c of the [union rows x n] table (synthetic K_NULL / K_OPEN..K_CLOSE where
 //                              candidate c lacks the key or holds None), then type / order / slots / encode run on it as in A1
+//   list round          only under KC_JSON_LISTS and when A1 marked records D_LIST (some candidate holds a list): after the
+//                       call's chunks the host aligns them (H2, kc_align_json_batch) and the chunks run again over the aligned
+//                       texts with list nodes on (Chunk::lists = 2: K_LOPEN / K_LCLOSE tokens, keyless TOK_ELEM elements ranked
+//                       by their index), every stage from A0 to C1 unchanged otherwise (kc_jsongpu.cu, list_round)
 //   A2  medoid_kernel   only when the chunk has multi-word string fields (three exclusive scans of the per-record counts first):
 //                       lane j writes its field's normalised strings and their offsets in K4's CSR form
 //   K1  kc_vote_i8, K2  kc_numeric_f64, K4  kc_medoid_str on the cell matrices / string groups — the kernels of the columnar path
@@ -31,7 +35,7 @@
 //                       leader turns them into piece offsets and record lengths          (then two exclusive scans: offsets)
 //   C1  write_kernel    lane j writes `"key": value` / `"key": confidence` at its offset of the two output blobs
 //
-// A record the device path does not model exactly (\u escapes, escapes in keys, non-ASCII, lists, empty objects, an object in one
+// A record the device path does not model exactly (\u escapes, escapes in keys, non-ASCII, lists without KC_JSON_LISTS, empty objects, an object in one
 // candidate against a value in another, candidates of different shapes without KC_JSON_KEY_UNION, multi-word strings outside
 // K4's contract, numbers outside the exact-conversion range, ...) gets a non-zero status and is
 // consolidated by the host path (kc_consolidate_json) instead: the device path never guesses.
@@ -52,6 +56,9 @@ constexpr int32_t kMaxFields = 1024;  // per record; the key ranking is quadrati
 // status of a record between A1 and the union round (U1-U3): its candidates differ in shape.  Internal: the union round turns
 // it into 0 or a D_* code before anything reads the statuses back.
 constexpr uint8_t D_UNION = 0xFF;
+// status of a record after the first round under KC_JSON_LISTS: some candidate holds a list and none is declined for another
+// reason.  The list round aligns it on the host and consolidates the aligned texts in a round of its own.
+constexpr uint8_t D_LIST = 0xFE;
 
 // A node of a record's key-union tree (union round): one key path.  Indices are relative to the record's scratch region;
 // node 0 is the top-level object.
@@ -66,11 +73,12 @@ struct UNode {
     uint32_t row, close;       // its row in the union table; an object's K_CLOSE row (the root: the node count in `row`)
 };
 
-// field descriptor word: kind:3 | last of its siblings in key order:1 | rank among its siblings:12 | group index within the record:16
-KC_HD inline uint32_t fdesc_pack(uint32_t kind, uint32_t last, uint32_t rank, uint32_t gidx) { return kind | (last << 3) | (rank << 4) | (gidx << 16); }
-KC_HD inline uint32_t fdesc_kind(uint32_t d) { return d & 7u; }
-KC_HD inline uint32_t fdesc_last(uint32_t d) { return (d >> 3) & 1u; }
-KC_HD inline uint32_t fdesc_rank(uint32_t d) { return (d >> 4) & 0xFFFu; }
+// field descriptor word: kind:4 | last of its siblings in output order:1 | rank among its siblings:11 | group index within the
+// record:16.  The rank of a member is its key's position in sorted order, of a list element its index.
+KC_HD inline uint32_t fdesc_pack(uint32_t kind, uint32_t last, uint32_t rank, uint32_t gidx) { return kind | (last << 4) | (rank << 5) | (gidx << 16); }
+KC_HD inline uint32_t fdesc_kind(uint32_t d) { return d & 15u; }
+KC_HD inline uint32_t fdesc_last(uint32_t d) { return (d >> 4) & 1u; }
+KC_HD inline uint32_t fdesc_rank(uint32_t d) { return (d >> 5) & 0x7FFu; }
 KC_HD inline uint32_t fdesc_gidx(uint32_t d) { return d >> 16; }
 
 struct Chunk {
@@ -119,14 +127,23 @@ struct Chunk {
     int32_t *umap;      // [scratch] token -> node (-1: a K_CLOSE)
     uint32_t uslot;     // the first round's slot total: union rows are numbered from here
     bool key_union;     // KC_JSON_KEY_UNION: such records go to the union round; without it A1 declines them as the reason says
+    // KC_JSON_LISTS.  lists: 0 = a list declines the record (D_NESTED); 1 = first round: a record with a list in some candidate
+    // is marked for the list round (lst), D_LIST unless a candidate declines it for another reason; 2 = aligned round: the
+    // texts are the alignment pre-pass's output, list nodes are consolidated.  Records [aligned0, R) are in the aligned round
+    // whatever `lists` says (the host twin runs both rounds in one chunk; the device runs them as chunks of their own).
+    uint8_t *lst;       // [R]   A1: some candidate holds a list (first round)
+    uint8_t lists;
+    int32_t aligned0;
 };
 
 KC_HD inline uint8_t load_status(const Chunk &ch, int32_t r) { return *(volatile const uint8_t *)(ch.status + r); }
 KC_HD inline void decline(const Chunk &ch, int32_t r, int32_t why) { *(volatile uint8_t *)(ch.status + r) = (uint8_t)why; }
+KC_HD inline uint32_t list_mode(const Chunk &ch, int32_t r) { return r >= ch.aligned0 ? 2u : ch.lists; }
 // the candidates differ in shape (`why`: how A1 sees it): with KC_JSON_KEY_UNION the union round decides the record
-// (D_KEYS_DIFFER keeps the later phases off it until then), else it is declined
+// (D_KEYS_DIFFER keeps the later phases off it until then), else it is declined.  Aligned texts have one shape by construction:
+// the union round never takes them.
 KC_HD inline void differ(const Chunk &ch, int32_t r, int32_t why) {
-    if (ch.key_union) {
+    if (ch.key_union && list_mode(ch, r) != 2) {
         *(volatile uint8_t *)(ch.pend + r) = 1;
         why = D_KEYS_DIFFER;
     }
@@ -139,27 +156,62 @@ KC_HD inline void count_record(const Chunk &ch, int32_t r) {
     const int64_t b = ch.off[(int64_t)r * ch.n], e = ch.off[(int64_t)r * ch.n + 1];
     int32_t f = -D_TOO_LONG;
     bool nested = false;
-    if (e - b < ((int64_t)1 << 31)) f = scan_object(ch.text + (b - ch.off[0]), (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, &nested);
+    if (e - b < ((int64_t)1 << 31))
+        f = scan_object(ch.text + (b - ch.off[0]), (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, &nested, list_mode(ch, r) != 0);
     ch.fcount[r] = f > 0 ? (uint32_t)f : 0u;
     ch.nest[r] = nested ? 1 : 0;
     ch.pend[r] = 0;
+    if (ch.lst) ch.lst[r] = 0;
     ch.status[r] = f > 0 ? (uint8_t)D_OK : (uint8_t)(-f);
 }
 
 // ---------------------------------------------------------------- A1
 
 KC_HD inline void parse_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t team) {
-    if (load_status(ch, r)) return;
+    const uint32_t mode = list_mode(ch, r);
+    // first round under KC_JSON_LISTS: every lane scans its candidates whatever the other lanes found (a list in any candidate
+    // sends the record to the list round, on every schedule of the lanes), unless candidate 0 did not scan (fcount 0)
+    if (mode == 1 ? ch.fcount[r] == 0 : load_status(ch, r) != 0) return;
     const int32_t F = (int32_t)ch.fcount[r];
     const int64_t base0 = ch.off[0];
     for (int32_t c = lane; c < ch.n; c += team) {
         const int64_t b = ch.off[(int64_t)r * ch.n + c], e = ch.off[(int64_t)r * ch.n + c + 1];
         int32_t f = -D_TOO_LONG;
-        if (e - b < ((int64_t)1 << 31) && (b - base0) + (e - b) < ((int64_t)1 << 32))
-            f = scan_object(ch.text + (b - base0), (uint32_t)(e - b), (uint32_t)(b - base0), ch.toks + (int64_t)ch.slot[r] * ch.n + c, ch.n, F);
-        if (f == -D_TOO_MANY_FIELDS || (f >= 0 && f != F)) differ(ch, r, D_KEYS_DIFFER);  // more or fewer tokens than candidate 0
-        else if (f < 0) decline(ch, r, -f);
+        bool listed = false;
+        if (e - b < ((int64_t)1 << 31) && (b - base0) + (e - b) < ((int64_t)1 << 32)) {
+            const uint8_t *s = ch.text + (b - base0);
+            f = scan_object(s, (uint32_t)(e - b), (uint32_t)(b - base0), ch.toks + (int64_t)ch.slot[r] * ch.n + c, ch.n, F, nullptr, mode != 0, &listed);
+            // first round: whether a candidate longer than candidate 0 holds a list past the tokens it has room for (a text
+            // without a '[' byte holds none: the key-union records of the first round skip the full scan)
+            if (mode == 1 && f == -D_TOO_MANY_FIELDS && !listed && contains(s, (uint32_t)(e - b), "[", 1))
+                scan_object(s, (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, nullptr, true, &listed);
+        }
+        if (mode == 1 && listed) {  // the list round's record: slots_phase settles its status
+            *(volatile uint8_t *)(ch.lst + r) = 1;
+            decline(ch, r, D_LIST);
+        } else if (f == -D_TOO_MANY_FIELDS || (f >= 0 && f != F)) {
+            differ(ch, r, D_KEYS_DIFFER);  // more or fewer tokens than candidate 0
+        } else if (f < 0) {
+            decline(ch, r, -f);
+        }
     }
+}
+
+// First round, team leader, a record with a list in some candidate: the first candidate (in order) declined for a reason of
+// its own gives the record's reason, else it goes to the list round.  (Lanes that scanned in parallel may have left any of
+// their reasons in the status; this makes the outcome the same on every schedule.)
+KC_HD inline void settle_listed(const Chunk &ch, int32_t r) {
+    int32_t why = D_LIST;
+    for (int32_t c = 0; c < ch.n && why == D_LIST; ++c) {
+        int64_t b, len;
+        const int64_t base0 = ch.off[0];
+        b = ch.off[(int64_t)r * ch.n + c] - base0;
+        len = ch.off[(int64_t)r * ch.n + c + 1] - base0 - b;
+        int32_t f = -D_TOO_LONG;
+        if (len < ((int64_t)1 << 31)) f = scan_object(ch.text + b, (uint32_t)len, 0, nullptr, 0, kMaxFields, nullptr, true);
+        if (f < 0) why = -f;
+    }
+    decline(ch, r, why);
 }
 
 // The siblings of a token at depth d: the tokens of depth d (other than K_CLOSE) in [lo, hi), the widest range around it in which
@@ -182,45 +234,54 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
     for (int32_t j = lane; j < F; j += team) {
         const Tok *row = rt + (int64_t)j * n;
         const uint32_t k0 = row[0].kind, d = tok_depth(row[0]);
-        // the same SHAPE in every candidate: the same key at position j, nested objects open and close at the same positions
-        // (else, with KC_JSON_KEY_UNION, the union round applies the pre-pass's key union / missing -> None / None -> dict of
-        // Nones, cu:516-548; it also tells an object against a non-null value, D_NESTED, from a row that is only out of step)
-        int32_t ref = j;  // the token whose key orders this one among its siblings: itself, or a K_CLOSE's K_OPEN
-        if (k0 == K_CLOSE) {
+        // the same SHAPE in every candidate: the same key at position j, nested objects (and lists: aligned texts, where every
+        // list of a node has one width) open and close at the same positions (else, with KC_JSON_KEY_UNION, the union round
+        // applies the pre-pass's key union / missing -> None / None -> dict of Nones, cu:516-548; it also tells an object
+        // against a non-null value, D_NESTED, from a row that is only out of step)
+        int32_t ref = j;  // the token whose key orders this one among its siblings: itself, or a closer's opener
+        if (is_close(k0)) {
             for (int32_t c = 1; c < n; ++c)
-                if (row[c].kind != K_CLOSE || tok_depth(row[c]) != d) {
+                if (row[c].kind != k0 || tok_depth(row[c]) != d) {
                     differ(ch, r, D_KEYS_DIFFER);
                     return;
                 }
-            ref = j - 1;  // its K_OPEN: the nearest token to the left at the same depth (everything between them is deeper)
+            ref = j - 1;  // its opener: the nearest token to the left at the same depth (everything between them is deeper)
             while (ref > 0 && tok_depth(rt[(int64_t)ref * n]) != d) --ref;
         }
         const uint8_t *key = ch.text + rt[(int64_t)ref * n].kstart;
         const uint32_t klen = rt[(int64_t)ref * n].klen;
-        if (k0 != K_CLOSE) {
+        const uint8_t elem = rt[(int64_t)ref * n].flags & TOK_ELEM;
+        if (!is_close(k0)) {
             for (int32_t c = 1; c < n; ++c) {
-                if ((row[c].kind == K_OPEN) != (k0 == K_OPEN) || row[c].kind == K_CLOSE) {  // an object here, a scalar / None there
-                    differ(ch, r, D_NESTED);
+                if ((row[c].kind == K_OPEN) != (k0 == K_OPEN) || (row[c].kind == K_LOPEN) != (k0 == K_LOPEN) || is_close(row[c].kind)) {
+                    differ(ch, r, D_NESTED);  // an object or a list here, a scalar / None / the other there
                     return;
                 }
-                if (tok_depth(row[c]) != d || row[c].klen != klen || key_compare(ch.text + row[c].kstart, klen, key, klen) != 0) {
+                if (tok_depth(row[c]) != d || (row[c].flags & TOK_ELEM) != elem || row[c].klen != klen ||
+                    key_compare(ch.text + row[c].kstart, klen, key, klen) != 0) {
                     differ(ch, r, D_KEYS_DIFFER);
                     return;
                 }
             }
-            if (contains(key, klen, "reasoning___", 12) || contains(key, klen, "source___", 9) ||  // skipped by consensus_dict (cu:1287-1294)
-                (F == 1 && klen == 4 && key_compare(key, 4, (const uint8_t *)"text", 4) == 0)) {   // {"text": s} -> s (cons:55-57)
+            if (!elem && (contains(key, klen, "reasoning___", 12) || contains(key, klen, "source___", 9) ||  // skipped by consensus_dict (cu:1287-1294)
+                          (F == 1 && klen == 4 && key_compare(key, 4, (const uint8_t *)"text", 4) == 0))) {   // {"text": s} -> s (cons:55-57)
                 decline(ch, r, D_SPECIAL_KEY);
                 return;
             }
         }
-        // position of the key among its siblings in sorted order (cu:521-522, at every level); duplicates: dict semantics, host path
+        // position of the key among its siblings in sorted order (cu:521-522, at every level); duplicates: dict semantics, host
+        // path.  A list element's position is its index.
         int32_t lo, hi;
         sibling_range(rt, n, F, ref, d, flat, lo, hi);
         uint32_t rank = 0, after = 0;
         for (int32_t i = lo; i < hi; ++i) {
             const Tok &o = rt[(int64_t)i * n];
-            if (i == ref || (!flat && (tok_depth(o) != d || o.kind == K_CLOSE))) continue;
+            if (i == ref || (!flat && (tok_depth(o) != d || is_close(o.kind)))) continue;
+            if (elem) {
+                rank += i < ref ? 1u : 0u;
+                after += i > ref ? 1u : 0u;
+                continue;
+            }
             const int cmp = key_compare(ch.text + o.kstart, o.klen, key, klen);
             if (cmp == 0) {
                 decline(ch, r, D_DUP_KEY);
@@ -230,8 +291,9 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
             after += cmp > 0 ? 1u : 0u;
         }
         const uint32_t last = after == 0 ? 1u : 0u;
-        if (k0 == K_OPEN || k0 == K_CLOSE) {
-            ch.fdesc[ch.slot[r] + j] = fdesc_pack(k0 == K_OPEN ? F_OPEN : F_CLOSE, last, rank, 0);
+        if (is_open(k0) || is_close(k0)) {
+            const uint32_t kind = k0 == K_OPEN ? F_OPEN : (k0 == K_CLOSE ? F_CLOSE : (k0 == K_LOPEN ? F_LOPEN : F_LCLOSE));
+            ch.fdesc[ch.slot[r] + j] = fdesc_pack(kind, last, rank, 0);
             continue;
         }
         // which kernel decides the field (plan_leaf, kc_json.cpp; cu:1405-1411, :1443-1453)
@@ -303,14 +365,14 @@ KC_HD inline void order_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t 
     const Tok *rt = ch.toks + (int64_t)ch.slot[r] * n;
     const uint32_t *fd = ch.fdesc + ch.slot[r];
     auto subtree = [&](int32_t i) -> uint32_t {  // tokens in the subtree of token i (itself included)
-        if (rt[(int64_t)i * n].kind != K_OPEN) return 1u;
+        if (!is_open(rt[(int64_t)i * n].kind)) return 1u;
         const uint32_t d = tok_depth(rt[(int64_t)i * n]);
         int32_t e = i + 1;
-        while (tok_depth(rt[(int64_t)e * n]) != d) ++e;  // its K_CLOSE
+        while (tok_depth(rt[(int64_t)e * n]) != d) ++e;  // its K_CLOSE / K_LCLOSE
         return (uint32_t)(e - i + 1);
     };
     for (int32_t j = lane; j < F; j += team) {
-        const bool closing = rt[(int64_t)j * n].kind == K_CLOSE;
+        const bool closing = is_close(rt[(int64_t)j * n].kind);
         uint32_t d = tok_depth(rt[(int64_t)j * n]);
         int32_t cur = j;
         if (closing) {
@@ -324,7 +386,7 @@ KC_HD inline void order_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t 
             const uint32_t rank = fdesc_rank(fd[cur]);
             for (int32_t i = lo; i < hi; ++i) {
                 const Tok &o = rt[(int64_t)i * n];
-                if (i == cur || tok_depth(o) != d || o.kind == K_CLOSE) continue;
+                if (i == cur || tok_depth(o) != d || is_close(o.kind)) continue;
                 if (fdesc_rank(fd[i]) < rank) pos += subtree(i);
             }
             if (d == 0) break;
@@ -343,6 +405,10 @@ KC_HD inline uint32_t out_pos(const Chunk &ch, int32_t r, int32_t j) {
 // team leader only: number the groups, reserve rows of the cell matrices (chunk-wide counters).  First round: a record whose
 // candidates differ in shape goes to the union round, whatever else A1 found (the union round scans and checks it afresh).
 KC_HD inline void slots_phase(const Chunk &ch, int32_t r, bool first_round) {
+    if (first_round && ch.lst && ch.lst[r]) {
+        settle_listed(ch, r);
+        return;
+    }
     if (load_status(ch, r)) {
         if (first_round && ch.pend[r]) {
             decline(ch, r, D_UNION);
@@ -760,18 +826,19 @@ KC_HD inline void len_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t te
     const int32_t F = (int32_t)ch.fcount[r], n = ch.n;
     for (int32_t j = lane; j < F; j += team) {
         const uint32_t d = ch.fdesc[ch.slot[r] + j], kind = fdesc_kind(d), sep = fdesc_last(d) ? 0u : 2u;  // ", " unless last of its siblings
-        const uint32_t klen = ch.toks[((int64_t)ch.slot[r] + j) * n].klen;
+        const Tok &t0 = ch.toks[((int64_t)ch.slot[r] + j) * n];
+        const uint32_t head = (t0.flags & TOK_ELEM) ? 0u : t0.klen + 4u;  // "key": (a list element has no key)
         const uint32_t pos = out_pos(ch, r, j);
         uint32_t lc, ll;
-        if (kind == F_OPEN) {
-            lc = ll = klen + 5u;  // "key": {
-        } else if (kind == F_CLOSE) {
-            lc = ll = 1u + sep;   // }
+        if (kind == F_OPEN || kind == F_LOPEN) {
+            lc = ll = head + 1u;  // "key": {   "key": [
+        } else if (kind == F_CLOSE || kind == F_LCLOSE) {
+            lc = ll = 1u + sep;   // }   ]
         } else {
             Sink c{nullptr, 0}, l{nullptr, 0};
             format_field(ch, r, j, c, l);
-            lc = klen + 4u + (uint32_t)c.n + sep;  // "key": value
-            ll = klen + 4u + (uint32_t)l.n + sep;
+            lc = head + (uint32_t)c.n + sep;  // "key": value
+            ll = head + (uint32_t)l.n + sep;
         }
         ch.piece_c[ch.slot[r] + pos] = lc;
         ch.piece_l[ch.slot[r] + pos] = ll;
@@ -812,19 +879,23 @@ KC_HD inline void write_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t 
             oc[0] = '{';
             ol[0] = '{';
         }
-        if (kind == F_CLOSE) {
-            c.put('}');
-            l.put('}');
+        if (kind == F_CLOSE || kind == F_LCLOSE) {
+            const uint8_t b = kind == F_CLOSE ? '}' : ']';
+            c.put(b);
+            l.put(b);
         } else {
-            c.put('"');
-            c.put(ch.text + t0.kstart, t0.klen);
-            c.lit("\": ");
-            l.put('"');
-            l.put(ch.text + t0.kstart, t0.klen);
-            l.lit("\": ");
-            if (kind == F_OPEN) {
-                c.put('{');
-                l.put('{');
+            if (!(t0.flags & TOK_ELEM)) {
+                c.put('"');
+                c.put(ch.text + t0.kstart, t0.klen);
+                c.lit("\": ");
+                l.put('"');
+                l.put(ch.text + t0.kstart, t0.klen);
+                l.lit("\": ");
+            }
+            if (kind == F_OPEN || kind == F_LOPEN) {
+                const uint8_t b = kind == F_OPEN ? '{' : '[';
+                c.put(b);
+                l.put(b);
                 continue;
             }
             format_field(ch, r, j, c, l);

@@ -2,8 +2,9 @@
 
 1. requests/s and p50 / p99 latency of async_consolidate_parsed_chat_completions at 1, 16 and 256 concurrent requests on one event
    loop, on S32 texts (SURVEY.md section 8d) or (--workload invoice_optional) invoice texts whose candidates reorder, drop and add
-   keys (tools/jsonpacked_throughput.py), at n = 3 and 16: the native route (device JSON path, requests combined per device call)
-   against the Python async route (_consensus_async) on the same contents.
+   keys, (invoice_lines) invoice texts whose `items` is a list of line items, or (mixed_lines) S32 and invoice_lines requests
+   interleaved (tools/jsonpacked_throughput.py), at n = 3 and 16: the native route (device JSON path, requests combined per
+   device call) against the Python async route (_consensus_async) on the same contents.
 2. kernel time of K5 (kc_numeric_medoid_f64) against K2 (kc_numeric_f64) on the same S32 numeric cells, 1 M records x 8 fields,
    at n = 4, 16, 32, 64 (CUDA events, median of 20 launches).
 Prints one JSON line per row, with the GPU name and power limit read in the same run."""
@@ -30,13 +31,21 @@ async def _no_embeddings(texts):
 
 def s32_completions(count, n, seed, workload="s32"):
     from openai.types.chat import ParsedChatCompletion
+    def s32(count):
+        blob, off = K.s32_texts_packed(count, n, seed, pinned=False)
+        raw = bytes(blob[:int(off[-1])])
+        return [[raw[off[r * n + c]:off[r * n + c + 1]].decode("ascii") for c in range(n)] for r in range(count)]
     if workload == "invoice_optional":
         from tools.jsonpacked_throughput import invoice_texts
         records = invoice_texts(count, n, seed, optional=True)
+    elif workload == "invoice_lines":
+        from tools.jsonpacked_throughput import invoice_lines_texts
+        records = invoice_lines_texts(count, n, seed)
+    elif workload == "mixed_lines":
+        from tools.jsonpacked_throughput import invoice_lines_texts
+        records = [r for pair in zip(s32(count // 2), invoice_lines_texts(count - count // 2, n, seed)) for r in pair]
     else:
-        blob, off = K.s32_texts_packed(count, n, seed, pinned=False)
-        raw = bytes(blob[:int(off[-1])])
-        records = [[raw[off[r * n + c]:off[r * n + c + 1]].decode("ascii") for c in range(n)] for r in range(count)]
+        records = s32(count)
     out = []
     for texts in records:
         out.append(ParsedChatCompletion.model_validate({
@@ -60,21 +69,21 @@ async def _run(completions, concurrency):
     return time.perf_counter() - t0, lat
 
 
-def requests_rows(card, workload="s32"):
+def requests_rows(card, workload="s32", count=2048):
     native_route = C._consensus_of_choices_native_async
 
     async def python_only(*a, **k):
         return None
     for n in (3, 16):
-        comps = s32_completions(2048, n, 20261016 + n, workload)
+        comps = s32_completions(count, n, 20261016 + n, workload)
         for conc in (1, 16, 256):
             row = {"what": "async_requests", "workload": workload, "n": n, "concurrency": conc, "gpu": card}
             for route in ("python", "native", "python", "native"):  # alternated twice; the faster run of each is reported
                 C._consensus_of_choices_native_async = native_route if route == "native" else python_only
-                count = len(comps) if route == "native" else 256
+                k = len(comps) if route == "native" else min(256, len(comps))
                 asyncio.run(_run(comps[:64], min(conc, 64)))  # warm-up
-                wall, lat = asyncio.run(_run(comps[:count], conc))
-                rps = count / wall
+                wall, lat = asyncio.run(_run(comps[:k], conc))
+                rps = k / wall
                 if rps > row.get(f"{route}_req_per_s", 0.0):
                     row[f"{route}_req_per_s"] = round(rps, 1)
                     row[f"{route}_p50_ms"] = round(float(np.percentile(lat, 50)) * 1e3, 3)
@@ -110,14 +119,16 @@ def kernel_rows(card):
 def main():
     import argparse
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["s32", "invoice_optional"], default="s32", help="the request rows' candidate texts")
+    ap.add_argument("--workload", choices=["s32", "invoice_optional", "invoice_lines", "mixed_lines"], default="s32",
+                    help="the request rows' candidate texts")
+    ap.add_argument("--requests", type=int, default=2048, help="requests per row (the Python route runs at most 256 of them)")
     ap.add_argument("--requests-only", action="store_true", help="skip the K5 / K2 kernel rows")
     args = ap.parse_args()
     torch.cuda.set_device(0)
     card = gpu_card()
     if not args.requests_only:
         kernel_rows(card)
-    requests_rows(card, args.workload)
+    requests_rows(card, args.workload, args.requests)
 
 
 if __name__ == "__main__":

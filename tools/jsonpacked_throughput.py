@@ -72,6 +72,47 @@ def invoice_texts(records, n, seed, nested=False, optional=False):
     return out
 
 
+def invoice_lines_texts(records, n, seed):
+    """invoice_texts' schema with `items` as a LIST of 1..12 line items (a phrase description, a SKU enum, an int quantity, a
+    float price): each candidate copies the record's line items with per-field noise, reorders them (probability 0.3), drops
+    one (0.2) and adds one (0.1): the device path's list round."""
+    import random
+    rng = random.Random(seed + 1)
+    descriptions = ["steel bolts m8 zinc plated", "hydraulic hose half inch", "industrial safety gloves large", "pallet wrap clear film",
+                    "copper wire two millimetre", "led floodlight fifty watt", "cordless drill battery pack", "cable ties black 300mm"]
+    skus = ["SKU-1001", "SKU-1002", "SKU-2040", "SKU-3300", "SKU-4712", "SKU-5000"]
+    out = []
+    for cands in invoice_texts(records, n, seed):
+        truth = [{"description": rng.choice(descriptions), "sku": rng.choice(skus), "quantity": rng.randrange(1, 50),
+                  "price": round(rng.uniform(0.5, 400), 2)} for _ in range(rng.randrange(1, 13))]
+        lines_out = []
+        for text in cands:
+            d = json.loads(text)
+            items = []
+            for t in truth:
+                it = dict(t)
+                r = rng.random()
+                if r < 0.1:
+                    it["description"] = it["description"].upper()
+                elif r < 0.15:
+                    it["quantity"] = it["quantity"] + 1
+                elif r < 0.2:
+                    it["price"] = round(it["price"] * 1.01, 2)
+                elif r < 0.23:
+                    it["sku"] = None
+                items.append(it)
+            if len(items) > 1 and rng.random() < 0.2:
+                del items[rng.randrange(len(items))]
+            if rng.random() < 0.1:
+                items.append({"description": rng.choice(descriptions), "sku": rng.choice(skus), "quantity": 1, "price": 9.99})
+            if rng.random() < 0.3:
+                rng.shuffle(items)
+            d["items"] = items
+            lines_out.append(json.dumps(d))
+        out.append(lines_out)
+    return out
+
+
 def _optional(rng, d, top=False):
     items = [(k, _optional(rng, v) if isinstance(v, dict) else v) for k, v in d.items()]
     items = [(k, None if isinstance(v, dict) and rng.random() < P_NULL_SUB else v) for k, v in items
@@ -85,33 +126,74 @@ def _optional(rng, d, top=False):
     return dict(items)
 
 
+def batch_api(args):
+    """consolidate_contents_batch on the workload's records: what the batch API (and, weighted, its Python planner for what the
+    device path declines) does per call.  One JSON line, best of --reps after one warm-up call."""
+    import random
+    from k_llms_b200.utils import consolidation as C
+    if args.workload == "invoice_lines":
+        records = invoice_lines_texts(args.records, args.n, 11)
+    else:
+        records = invoice_texts(args.records, args.n, 11, nested="nested" in args.workload, optional="optional" in args.workload)
+    rng = random.Random(3)
+    lps = [[[-rng.random() * 4, -rng.random()] for _ in r] for r in records] if args.weighted else None
+    embed = lambda t: [[0.0] for _ in t]  # noqa: E731  (never called: no pair of long strings in these workloads)
+    walls, counts = [], {}
+    for i in range(args.reps + 1):
+        counts = {}
+        t0 = time.perf_counter()
+        out = C.consolidate_contents_batch(records, get_openai_embeddings_from_text=embed, token_logprobs=lps, counts=counts)
+        if i:
+            walls.append(time.perf_counter() - t0)
+    print(json.dumps({"what": "batch_api", "workload": args.workload, "weighted": args.weighted, "records": args.records, "n": args.n,
+                      "best_s": round(min(walls), 4), "records_per_s": round(args.records / min(walls)), "counts": counts,
+                      "example": str(out[0])[:80]}), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["s32", "invoice", "invoice_nested", "invoice_optional", "invoice_nested_optional"], default="s32",
+    ap.add_argument("--workload", choices=["s32", "invoice", "invoice_nested", "invoice_optional", "invoice_nested_optional", "invoice_lines"],
+                    default="s32",
                     help="s32: the bench schema (enum / bool / number fields); invoice: 12 fields, 4 of them free text (medoid, K4); "
                          "invoice_nested: the same fields in nested objects (depth 3); *_optional: candidates that reorder, drop and add "
-                         "keys and (nested) hold None or nothing for sub-objects")
+                         "keys and (nested) hold None or nothing for sub-objects; invoice_lines: `items` is a list of line items (list round)")
     ap.add_argument("--records", type=int, default=262144)
     ap.add_argument("--n", type=int, default=16)
     ap.add_argument("--reps", type=int, default=4)
     ap.add_argument("--chunk-mb", default="64")
     ap.add_argument("--streams", default="3")
     ap.add_argument("--pageable", action="store_true", help="input blob in ordinary (not page-locked) memory")
+    ap.add_argument("--weighted", action="store_true", help="the likelihood-weighted variant (random candidate sums)")
+    ap.add_argument("--no-lists", action="store_true", help="without JSON_LISTS: list records go to the host path (H1)")
+    ap.add_argument("--batch-api", action="store_true",
+                    help="time consolidate_contents_batch (with --weighted: token logprobs, two per candidate) instead of the C-ABI call")
     args = ap.parse_args()
+    if args.batch_api:
+        return batch_api(args)
     t0 = time.perf_counter()
-    if args.workload != "s32":
+    if args.workload == "invoice_lines":
+        blob, off, _n = K.pack_texts(invoice_lines_texts(args.records, args.n, 11), pinned=not args.pageable)
+    elif args.workload != "s32":
         blob, off, _n = K.pack_texts(invoice_texts(args.records, args.n, 11, nested="nested" in args.workload, optional="optional" in args.workload),
                                      pinned=not args.pageable)
     else:
         blob, off = K.s32_texts_packed(args.records, args.n, 11, pinned=not args.pageable)
     gen_s = time.perf_counter() - t0
+    flags = K.JSON_KEY_UNION | (0 if args.no_lists else K.JSON_LISTS)  # as the client functions call it
+    seq = None
+    if args.weighted:
+        import numpy as np
+        seq = (-np.random.default_rng(3).exponential(4.0, args.records * args.n)).astype(np.float32)
     for chunk in args.chunk_mb.split(","):
         for streams in args.streams.split(","):
             os.environ["KC_JSON_CHUNK_MB"], os.environ["KC_JSON_STREAMS"] = chunk, streams
             walls, stats = [], None
             for i in range(args.reps + 1):
                 t0 = time.perf_counter()
-                res = K.consolidate_json_packed(blob, off, args.n, flags=K.JSON_KEY_UNION)  # as the client functions call it
+                if seq is None:
+                    res = K.consolidate_json_packed(blob, off, args.n, flags=flags)
+                else:
+                    res = K.consolidate_json_packed_weighted(blob, off, args.n, seq, flags=flags)
                 dt = time.perf_counter() - t0
                 stats = res.stats.as_dict()
                 first = res.content(0)
@@ -119,7 +201,8 @@ def main():
                 if i:
                     walls.append(dt)
             best = min(walls)
-            print(json.dumps({"workload": args.workload, "records": args.records, "n": args.n, "chunk_mb": int(chunk), "streams": int(streams),
+            print(json.dumps({"workload": args.workload, "weighted": args.weighted, "flags": flags, "records": args.records, "n": args.n,
+                              "chunk_mb": int(chunk), "streams": int(streams),
                               "pinned_input": not args.pageable, "json_GB": round(stats["input_bytes"] / 1e9, 3),
                               "best_s": round(best, 4), "mean_s": round(sum(walls) / len(walls), 4),
                               "records_per_s": round(args.records / best), "n_device": stats["n_device"], "n_host": stats["n_host"],
