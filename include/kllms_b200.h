@@ -375,6 +375,12 @@ void kc_free_strings(char **arr, int64_t count);
  *                     declines keeps status 1 with why = 15 (D_ALIGN); what the aligned round declines follows the route of any
  *                     declined record (the host path, with the original texts).  Without it a list declines the record as before
  *                     (why = 4, D_NESTED).  The client functions set it.
+ *            KC_JSON_UNICODE: string values may hold non-ASCII text and \uXXXX escapes (UTF-8 validated as Python's strict
+ *                     decoder does).  A field decided by the similarity medoid (some value has >= 3 words) stays on the device:
+ *                     it compares normalize_string forms (ASCII alphanumerics, lower-cased; every other code point dropped) and
+ *                     prints the chosen original as json.dumps does (ensure_ascii).  A vote field with such a value, a non-ASCII or
+ *                     escaped key, and a record of the list round with such text are declined as without it (why = 3; the list
+ *                     round's alignment declines non-ASCII: why = 15).  The client functions set it.
  *   *out     result handle: one text blob + per-record spans (kc_json_result_view), released with kc_json_result_free
  * status per record: 0 = consolidated on the device, 2 = consolidated by the host path, 1 = needs the Python path.
  * Texts are byte-identical to the reference's json.dumps output.  Re-entrant (pooled per-call streams and buffers).
@@ -383,6 +389,7 @@ void kc_free_strings(char **arr, int64_t count);
 #define KC_JSON_NUMERIC_MEDOID 2u
 #define KC_JSON_KEY_UNION 4u
 #define KC_JSON_LISTS 8u
+#define KC_JSON_UNICODE 16u
 typedef struct kc_json_result kc_json_result;
 typedef struct {
     int64_t n_records, n_device, n_host, n_python; /* where the records were consolidated */
@@ -414,7 +421,7 @@ typedef struct kc_debug_jsongpu kc_debug_jsongpu;
 int kc_debug_jsongpu_plan(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, kc_debug_jsongpu **out);
 /* the same with the flags of kc_consolidate_json_packed that change the phases (KC_JSON_NUMERIC_MEDOID, KC_JSON_KEY_UNION,
  * KC_JSON_LISTS: the list round's alignment runs on the host inside the plan, the aligned round's groups follow the first
- * round's in the input hooks, and the emit puts their texts and statuses at the call's records) */
+ * round's in the input hooks, and the emit puts their texts and statuses at the call's records; KC_JSON_UNICODE) */
 int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_t n_records, int32_t n, uint32_t flags,
                                 kc_debug_jsongpu **out);
 int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells, int64_t *n_vote_groups, const double **num_cells,

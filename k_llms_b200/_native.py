@@ -474,6 +474,7 @@ JSON_DEVICE_ONLY = 1
 JSON_NUMERIC_MEDOID = 2  # the async dispatcher: numeric fields are similarity medoids (K5); implies JSON_DEVICE_ONLY
 JSON_KEY_UNION = 4  # candidates that differ in shape (key order, missing / extra keys, null sub-objects) stay on the device
 JSON_LISTS = 8  # records with list fields stay on the device: aligned by H2 on host threads, consolidated in a list round
+JSON_UNICODE = 16  # similarity-medoid fields with non-ASCII text or \uXXXX escapes stay on the device (vote fields decline)
 
 
 def pack_texts(records, pinned: bool = True):

@@ -35,8 +35,9 @@ constexpr int32_t kMaxNesting = 8;  // nested objects and lists below the top le
 
 // One (field, candidate) cell of a record: views into the chunk's text.  Strings: the raw inner span (no quotes); raw == value
 // unless TOK_ESCAPED (keys: always, the scanner declines escapes in keys).  flags: bit 0 TOK_MULTIWORD, bit 1 TOK_ESCAPED, bit 2
-// TOK_ELEM, bits 4-7 the nesting depth of the member.  K_OPEN / K_LOPEN carry the key of the nested value, K_CLOSE / K_LCLOSE no
-// key.  TOK_MULTIWORD: the string has >= 3 whitespace-separated words (not enum-like, cu:1405).  TOK_ELEM: a list element (no key).
+// TOK_ELEM, bit 3 TOK_UNICODE, bits 4-7 the nesting depth of the member.  K_OPEN / K_LOPEN carry the key of the nested value,
+// K_CLOSE / K_LCLOSE no key.  TOK_MULTIWORD: the string has >= 3 whitespace-separated words (not enum-like, cu:1405).  TOK_ELEM:
+// a list element (no key).
 struct alignas(16) Tok {
     uint32_t vstart, vlen;  // value span, relative to the chunk's first byte
     uint32_t kstart;        // key span (inner)
@@ -46,8 +47,11 @@ struct alignas(16) Tok {
 };
 constexpr uint8_t TOK_MULTIWORD = 1;
 KC_HD inline uint32_t tok_depth(const Tok &t) { return (uint32_t)t.flags >> 4; }  // 0 = a member of the top-level object
-constexpr uint8_t TOK_ESCAPED = 2;  // the span holds two-character escapes (\" \\ \/ \b \f \n \r \t), never \uXXXX
+constexpr uint8_t TOK_ESCAPED = 2;  // the span holds escapes: two-character ones (\" \\ \/ \b \f \n \r \t), \uXXXX only with TOK_UNICODE
 constexpr uint8_t TOK_ELEM = 4;
+// a string value (scanned with `unicode`) that holds raw UTF-8, a \uXXXX escape or a raw DEL: its readers decode it to code
+// points (decode_cp) instead of reading bytes
+constexpr uint8_t TOK_UNICODE = 8;
 
 // why a record left the device path (diagnostics only; every non-zero code means "host path").  D_ALIGN: the alignment
 // pre-pass of the list round declined the record (a pair of long strings for the embeddings service, non-ASCII text).
@@ -59,6 +63,45 @@ enum : int32_t {
 
 KC_HD inline bool is_json_ws(uint8_t c) { return c == ' ' || c == '\t' || c == '\n' || c == '\r'; }
 KC_HD inline bool is_digit(uint8_t c) { return (uint8_t)(c - '0') <= 9; }
+
+// str.isspace() of a code point: the 29 separators str.split() splits on
+KC_HD inline bool is_py_space(uint32_t c) {
+    if (c < 0x80) return c == ' ' || (c >= 0x09 && c <= 0x0D) || (c >= 0x1C && c <= 0x1F);
+    return c == 0x85 || c == 0xA0 || c == 0x1680 || (c >= 0x2000 && c <= 0x200A) || c == 0x2028 || c == 0x2029 || c == 0x202F ||
+           c == 0x205F || c == 0x3000;
+}
+
+// the four hex digits of a \uXXXX escape (either case); false if one is not a hex digit
+KC_HD inline bool hex4(const uint8_t *s, uint32_t &v) {
+    v = 0;
+    for (int k = 0; k < 4; ++k) {
+        const uint8_t c = s[k];
+        uint32_t d;
+        if (is_digit(c)) d = (uint32_t)(c - '0');
+        else if ((c | 32) >= 'a' && (c | 32) <= 'f') d = (uint32_t)((c | 32) - 'a' + 10);
+        else return false;
+        v = (v << 4) | d;
+    }
+    return true;
+}
+
+// One UTF-8 sequence at s[0..avail) (s[0] >= 0x80) as Python's strict decoder reads it: its length, 0 when it is invalid
+// (a stray continuation byte, an overlong form, an encoded surrogate ED A0..BF, a code point above U+10FFFF, a truncated sequence)
+KC_HD inline uint32_t utf8_decode(const uint8_t *s, uint32_t avail, uint32_t &cp) {
+    const uint8_t b = s[0];
+    if (b < 0xC2 || b > 0xF4) return 0;
+    const uint32_t k = b < 0xE0 ? 2u : (b < 0xF0 ? 3u : 4u);
+    if (avail < k) return 0;
+    // the second byte's range excludes overlong forms (E0, F0), surrogates (ED) and code points above U+10FFFF (F4)
+    const uint8_t lo = b == 0xE0 ? 0xA0 : (b == 0xF0 ? 0x90 : 0x80), hi = b == 0xED ? 0x9F : (b == 0xF4 ? 0x8F : 0xBF);
+    if (s[1] < lo || s[1] > hi) return 0;
+    cp = b & (0x7Fu >> k);
+    for (uint32_t i = 1; i < k; ++i) {
+        if ((s[i] & 0xC0) != 0x80) return 0;
+        cp = (cp << 6) | (s[i] & 0x3Fu);
+    }
+    return k;
+}
 
 KC_HD inline int clz64(uint64_t x) {
 #ifdef __CUDA_ARCH__
@@ -87,9 +130,11 @@ KC_HD inline double bits_f64(uint64_t b) {
 // it does not model exactly (\u escapes, non-ASCII, lists, NaN/Infinity, free text that the reference wraps as {"text": ...},
 // an empty object) is left to the host path.  *nested (optional): whether the object holds a nested object (or a list).
 // lists: `[` opens a list node (K_LOPEN, its elements keyless TOK_ELEM tokens one level deeper, K_LCLOSE) instead of declining
-// the record with D_NESTED; *has_list (optional): whether the text holds a list.
+// the record with D_NESTED; *has_list (optional): whether the text holds a list.  unicode: string VALUES may hold raw UTF-8
+// (validated), \uXXXX escapes and a raw DEL (the token gets TOK_UNICODE, its words are counted over Python's whitespace) instead
+// of declining the record with D_ESCAPE_OR_NON_ASCII; keys stay ASCII.
 KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, Tok *toks, int32_t stride, int32_t cap, bool *nested = nullptr,
-                                 bool lists = false, bool *has_list = nullptr) {
+                                 bool lists = false, bool *has_list = nullptr, bool unicode = false) {
     uint32_t p = 0;
     while (p < len && is_json_ws(s[p])) ++p;
     if (p >= len) return -D_EMPTY;
@@ -139,22 +184,40 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
             const uint32_t vs = p;
             uint32_t words = 0;
             bool prev_space = true;
-            bool escaped = false;
+            bool escaped = false, uni = false;
             for (;;) {
                 if (p >= len) return -D_SYNTAX;
                 const uint8_t d = s[p];
                 if (d == '"') break;
                 if (d < 0x20) return -D_SYNTAX;
-                if (d >= 0x80) return -D_ESCAPE_OR_NON_ASCII;
-                bool sp = d == ' ';  // the only str.split() whitespace a raw JSON string can hold unescaped
-                if (d == '\\') {
+                bool sp = d == ' ';  // the only ASCII str.split() whitespace a raw JSON string can hold unescaped
+                if (d >= 0x7F) {
+                    if (d == 0x7F) {
+                        uni |= unicode;  // DEL: json.dumps prints it as \u007f
+                    } else {
+                        uint32_t cp = 0;
+                        const uint32_t k = unicode ? utf8_decode(s + p, len - p, cp) : 0u;
+                        if (k == 0) return -D_ESCAPE_OR_NON_ASCII;
+                        sp = is_py_space(cp);
+                        uni = true;
+                        p += k - 1;
+                    }
+                } else if (d == '\\') {
                     // the two-character escapes stay in the token (TOK_ESCAPED; every reader of the value skips or maps them);
-                    // \uXXXX (any code point, surrogate pairs, non-ASCII) is the host path's
+                    // \uXXXX (any code point, surrogate pairs, non-ASCII) is the host path's unless `unicode`
                     if (p + 1 >= len) return -D_SYNTAX;
                     const uint8_t e = s[p + 1];
-                    if (e == 'u') return -D_ESCAPE_OR_NON_ASCII;
-                    if (!(e == '"' || e == '\\' || e == '/' || e == 'b' || e == 'f' || e == 'n' || e == 'r' || e == 't')) return -D_SYNTAX;
-                    sp = e == 't' || e == 'n' || e == 'r' || e == 'f';  // str.split() whitespace; \b (0x08) is not
+                    if (e == 'u') {
+                        if (!unicode) return -D_ESCAPE_OR_NON_ASCII;
+                        uint32_t v;
+                        if (p + 5 >= len || !hex4(s + p + 2, v)) return -D_SYNTAX;
+                        sp = is_py_space(v);  // no surrogate is whitespace: a pair need not be joined to count words
+                        uni = true;
+                        p += 4;
+                    } else {
+                        if (!(e == '"' || e == '\\' || e == '/' || e == 'b' || e == 'f' || e == 'n' || e == 'r' || e == 't')) return -D_SYNTAX;
+                        sp = e == 't' || e == 'n' || e == 'r' || e == 'f';  // str.split() whitespace; \b (0x08) is not
+                    }
                     escaped = true;
                     ++p;
                 }
@@ -165,7 +228,7 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
             t.kind = K_STR;
             t.vstart = rel + vs;
             t.vlen = p - vs;
-            t.flags = (uint8_t)((words >= 3 ? TOK_MULTIWORD : 0) | (escaped ? TOK_ESCAPED : 0));
+            t.flags = (uint8_t)((words >= 3 ? TOK_MULTIWORD : 0) | (escaped ? TOK_ESCAPED : 0) | (uni ? TOK_UNICODE : 0));
             ++p;
         } else if (c == '{') {
             ++p;
@@ -352,6 +415,56 @@ KC_HD inline uint32_t unescaped_length(const uint8_t *a, uint32_t la) {
     return k;
 }
 
+// The code point at a[i] of a TOK_UNICODE span (validated by scan_object), advancing i past it: what json.loads decodes.  A
+// \uXXXX high surrogate followed by a \uXXXX low surrogate is one code point; any other surrogate escape stands alone.
+KC_HD inline uint32_t decode_cp(const uint8_t *a, uint32_t la, uint32_t &i) {
+    const uint8_t b = a[i];
+    if (b == '\\') {
+        const uint8_t e = a[i + 1];
+        if (e != 'u') {
+            i += 2;
+            return e == 'b' ? 8u : (e == 'f' ? 12u : (e == 'n' ? 10u : (e == 'r' ? 13u : (e == 't' ? 9u : (uint32_t)e))));
+        }
+        uint32_t v, w;
+        hex4(a + i + 2, v);
+        i += 6;
+        if (v >= 0xD800 && v < 0xDC00 && i + 6 <= la && a[i] == '\\' && a[i + 1] == 'u' && hex4(a + i + 2, w) && w >= 0xDC00 && w < 0xE000) {
+            i += 6;
+            return 0x10000u + ((v - 0xD800u) << 10) + (w - 0xDC00u);
+        }
+        return v;
+    }
+    if (b < 0x80) {
+        ++i;
+        return b;
+    }
+    uint32_t cp = 0;
+    i += utf8_decode(a + i, la - i, cp);
+    return cp;
+}
+
+// normalize_string (consensus_utils.py:660-673) of a TOK_UNICODE span: re.sub(r"[^a-zA-Z0-9]", "", text).lower() drops every
+// non-ASCII code point before lower-casing (so the Kelvin sign and U+0130 leave nothing), keeps ASCII alphanumerics however they
+// are written (A is 'A').  Its length, and the characters written to `out` (K4's input) when out != nullptr.
+KC_HD inline uint32_t normalize_string(const uint8_t *a, uint32_t la, uint8_t *out) {
+    uint32_t k = 0;
+    for (uint32_t i = 0; i < la;) {
+        const uint32_t cp = decode_cp(a, la, i);
+        uint8_t c = (uint8_t)cp;
+        if (cp >= 0x80 || !is_alnum_lower(c)) continue;
+        if (out) out[k] = c;
+        ++k;
+    }
+    return k;
+}
+
+// len(value) of a TOK_UNICODE span: its code points
+KC_HD inline uint32_t code_points(const uint8_t *a, uint32_t la) {
+    uint32_t k = 0;
+    for (uint32_t i = 0; i < la; ++k) decode_cp(a, la, i);
+    return k;
+}
+
 // bytewise three-way comparison (Python's str ordering on ASCII keys)
 KC_HD inline int key_compare(const uint8_t *a, uint32_t la, const uint8_t *b, uint32_t lb) {
     const uint32_t m = la < lb ? la : lb;
@@ -487,11 +600,40 @@ struct Sink {
     KC_HD void lit(const char *s) {
         for (; *s; ++s) put((uint8_t)*s);
     }
-    // json.dumps of a string value, quotes included, from its raw span: the two-character escapes are already what json.dumps
-    // prints, except "\/", which it prints as "/"
-    KC_HD void json_string(const uint8_t *s, uint32_t len, bool escaped) {
+    KC_HD void u_escape(uint32_t v) {  // \uxxxx, lower-case hex as json.dumps writes it
+        put('\\');
+        put('u');
+        for (int k = 12; k >= 0; k -= 4) {
+            const uint32_t d = (v >> k) & 15u;
+            put((uint8_t)(d < 10 ? '0' + d : 'a' + d - 10));
+        }
+    }
+    // json.dumps of a string value (ensure_ascii), quotes included, from its raw span (token flags: TOK_ESCAPED, TOK_UNICODE).
+    // ASCII spans: the two-character escapes are already what json.dumps prints, except "\/", which it prints as "/".  TOK_UNICODE
+    // spans are decoded to code points and printed one by one: `"` `\` and \n \r \t \b \f as two-character escapes, other
+    // controls and DEL as \u00xx, printable ASCII as itself, the rest of the BMP (lone surrogates included) as \uxxxx, astral
+    // code points as a surrogate pair.  The length pass counts exactly what the write pass writes: it is this same code.
+    KC_HD void json_string(const uint8_t *s, uint32_t len, uint8_t flags) {
         put('"');
-        if (!escaped) {
+        if (flags & TOK_UNICODE) {
+            for (uint32_t i = 0; i < len;) {
+                const uint32_t cp = decode_cp(s, len, i);
+                if (cp == '"' || cp == '\\') {
+                    put('\\');
+                    put((uint8_t)cp);
+                } else if (cp >= 0x20 && cp < 0x7F) {
+                    put((uint8_t)cp);
+                } else if (cp == '\n' || cp == '\r' || cp == '\t' || cp == 8 || cp == 12) {
+                    put('\\');
+                    put(cp == '\n' ? 'n' : (cp == '\r' ? 'r' : (cp == '\t' ? 't' : (cp == 8 ? 'b' : 'f'))));
+                } else if (cp >= 0x10000) {
+                    u_escape(0xD800u + ((cp - 0x10000u) >> 10));
+                    u_escape(0xDC00u + ((cp - 0x10000u) & 0x3FFu));
+                } else {
+                    u_escape(cp);
+                }
+            }
+        } else if (!(flags & TOK_ESCAPED)) {
             put(s, len);
         } else {
             for (uint32_t i = 0; i < len; ++i) {

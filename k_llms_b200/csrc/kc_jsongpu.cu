@@ -319,7 +319,7 @@ int union_round(Worker &w, Chunk &ch, int64_t P, size_t &T, int team, int grid, 
 // vote leaves are likelihood-weighted (K3b over ragged records in K1's place).  xmedoid (KC_JSON_NUMERIC_MEDOID): numeric fields
 // are similarity medoids (K5 in K2's place).  lists: Chunk::lists.  dst (NULL: the identity): the result index of each record
 // of the batch (the aligned round's batch is the list records, in the order of their result indices).
-int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, bool key_union, uint8_t lists,
+int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, bool key_union, uint8_t lists, bool unicode,
               const int64_t *dst, int64_t r0, int64_t r1, int32_t n, double rel_eps, double abs_eps, int sm_count, kc_json_result &res,
               ChunkStage &st) {
     const int64_t Rc = r1 - r0;
@@ -376,6 +376,7 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     ch.lst = lists ? w.lst.as<uint8_t>() : nullptr;
     ch.lists = lists;
     ch.aligned0 = INT32_MAX;  // a chunk is in one round: Chunk::lists says which
+    ch.unicode = unicode;
 
     nvtxRangePushA("kc_json: H2D texts");
     KC_CUDA_I(cudaEventRecord(w.ev[0], s));
@@ -708,8 +709,8 @@ int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_
             while (!rc) {
                 const int k = next.fetch_add(1);
                 if (k >= chunks) break;
-                rc = run_chunk(w, text, off, seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, (flags & KC_JSON_KEY_UNION) != 0, lists, dst, cuts[(size_t)k],
-                               cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res, stages[(size_t)wi]);
+                rc = run_chunk(w, text, off, seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, (flags & KC_JSON_KEY_UNION) != 0, lists,
+                               (flags & KC_JSON_UNICODE) != 0, dst, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res, stages[(size_t)wi]);
             }
             if (rc) {
                 cudaStreamSynchronize(w.stream);
@@ -936,6 +937,7 @@ void plan_twin(kc_debug_jsongpu *h, const char *h_text, const int64_t *h_off, in
     ch.lst = h->lst.data();
     ch.lists = lists;
     ch.aligned0 = aligned0;
+    ch.unicode = (flags & KC_JSON_UNICODE) != 0;
     for (int32_t r = 0; r < R; ++r) kc::js::count_record(ch, r);
     for (int64_t r = 0; r < R; ++r) h->slot[(size_t)r + 1] = h->slot[(size_t)r] + h->fcount[(size_t)r];
     const size_t T = h->slot[(size_t)R];

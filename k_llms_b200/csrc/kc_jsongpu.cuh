@@ -35,7 +35,8 @@
 //                       leader turns them into piece offsets and record lengths          (then two exclusive scans: offsets)
 //   C1  write_kernel    lane j writes `"key": value` / `"key": confidence` at its offset of the two output blobs
 //
-// A record the device path does not model exactly (\u escapes, escapes in keys, non-ASCII, lists without KC_JSON_LISTS, empty objects, an object in one
+// A record the device path does not model exactly (\u escapes and non-ASCII without KC_JSON_UNICODE, or with it in vote fields, escapes in
+// keys, lists without KC_JSON_LISTS, empty objects, an object in one
 // candidate against a value in another, candidates of different shapes without KC_JSON_KEY_UNION, multi-word strings outside
 // K4's contract, numbers outside the exact-conversion range, ...) gets a non-zero status and is
 // consolidated by the host path (kc_consolidate_json) instead: the device path never guesses.
@@ -134,6 +135,9 @@ struct Chunk {
     uint8_t *lst;       // [R]   A1: some candidate holds a list (first round)
     uint8_t lists;
     int32_t aligned0;
+    // KC_JSON_UNICODE: string values may hold non-ASCII text and \uXXXX escapes (TOK_UNICODE tokens).  Similarity medoids take
+    // them (normalize_string drops every non-ASCII code point); a vote field with one declines (its classes need unidecode).
+    bool unicode;
 };
 
 KC_HD inline uint8_t load_status(const Chunk &ch, int32_t r) { return *(volatile const uint8_t *)(ch.status + r); }
@@ -157,7 +161,8 @@ KC_HD inline void count_record(const Chunk &ch, int32_t r) {
     int32_t f = -D_TOO_LONG;
     bool nested = false;
     if (e - b < ((int64_t)1 << 31))
-        f = scan_object(ch.text + (b - ch.off[0]), (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, &nested, list_mode(ch, r) != 0);
+        f = scan_object(ch.text + (b - ch.off[0]), (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, &nested, list_mode(ch, r) != 0, nullptr,
+                        ch.unicode);
     ch.fcount[r] = f > 0 ? (uint32_t)f : 0u;
     ch.nest[r] = nested ? 1 : 0;
     ch.pend[r] = 0;
@@ -180,11 +185,12 @@ KC_HD inline void parse_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t 
         bool listed = false;
         if (e - b < ((int64_t)1 << 31) && (b - base0) + (e - b) < ((int64_t)1 << 32)) {
             const uint8_t *s = ch.text + (b - base0);
-            f = scan_object(s, (uint32_t)(e - b), (uint32_t)(b - base0), ch.toks + (int64_t)ch.slot[r] * ch.n + c, ch.n, F, nullptr, mode != 0, &listed);
+            f = scan_object(s, (uint32_t)(e - b), (uint32_t)(b - base0), ch.toks + (int64_t)ch.slot[r] * ch.n + c, ch.n, F, nullptr, mode != 0, &listed,
+                            ch.unicode);
             // first round: whether a candidate longer than candidate 0 holds a list past the tokens it has room for (a text
             // without a '[' byte holds none: the key-union records of the first round skip the full scan)
             if (mode == 1 && f == -D_TOO_MANY_FIELDS && !listed && contains(s, (uint32_t)(e - b), "[", 1))
-                scan_object(s, (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, nullptr, true, &listed);
+                scan_object(s, (uint32_t)(e - b), 0, nullptr, 0, kMaxFields, nullptr, true, &listed, ch.unicode);
         }
         if (mode == 1 && listed) {  // the list round's record: slots_phase settles its status
             *(volatile uint8_t *)(ch.lst + r) = 1;
@@ -208,7 +214,7 @@ KC_HD inline void settle_listed(const Chunk &ch, int32_t r) {
         b = ch.off[(int64_t)r * ch.n + c] - base0;
         len = ch.off[(int64_t)r * ch.n + c + 1] - base0 - b;
         int32_t f = -D_TOO_LONG;
-        if (len < ((int64_t)1 << 31)) f = scan_object(ch.text + b, (uint32_t)len, 0, nullptr, 0, kMaxFields, nullptr, true);
+        if (len < ((int64_t)1 << 31)) f = scan_object(ch.text + b, (uint32_t)len, 0, nullptr, 0, kMaxFields, nullptr, true, nullptr, ch.unicode);
         if (f < 0) why = -f;
     }
     decline(ch, r, why);
@@ -305,6 +311,7 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
             kind = F_ALLNULL;
         } else if (row[first].kind == K_STR) {
             kind = F_VOTE_STR;
+            bool uni = false;
             for (int32_t c = 0; c < n; ++c) {
                 if (row[c].kind == K_NULL) continue;
                 if (row[c].kind != K_STR) {  // str(v) of numbers / bools inside a string field: host path
@@ -312,6 +319,11 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
                     return;
                 }
                 if (row[c].flags & TOK_MULTIWORD) kind = F_MEDOID;  // not enum-like (cu:1405): the similarity medoid (cu:1221-1237)
+                uni |= (row[c].flags & TOK_UNICODE) != 0;
+            }
+            if (kind == F_VOTE_STR && uni) {  // sanitize_value folds non-ASCII text through unidecode (cu:931): host path
+                decline(ch, r, D_ESCAPE_OR_NON_ASCII);
+                return;
             }
             if (kind == F_MEDOID) {
                 // K4 takes the group when every pair is a Levenshtein pair inside its contract (plan_leaf of kc_json.cpp, the
@@ -321,10 +333,14 @@ KC_HD inline void type_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t t
                 bool fits = true;
                 for (int32_t c = 0; c < n; ++c) {
                     if (row[c].kind == K_NULL) continue;
-                    const uint32_t nl = sanitized_copy(ch.text + row[c].vstart, row[c].vlen, nullptr);
+                    const uint8_t *v = ch.text + row[c].vstart;
+                    const uint32_t vl = row[c].vlen;
+                    const bool u = (row[c].flags & TOK_UNICODE) != 0;
+                    const uint32_t nl = u ? normalize_string(v, vl, nullptr) : sanitized_copy(v, vl, nullptr);
                     ++live;
                     chars += nl;
-                    const uint32_t raw = (row[c].flags & TOK_ESCAPED) ? unescaped_length(ch.text + row[c].vstart, row[c].vlen) : row[c].vlen;
+                    // len(str): code points
+                    const uint32_t raw = u ? code_points(v, vl) : ((row[c].flags & TOK_ESCAPED) ? unescaped_length(v, vl) : vl);
                     long_raw += raw > 50u ? 1u : 0u;
                     long_norm += nl > 64u ? 1u : 0u;
                     fits &= nl <= 2000u;
@@ -483,7 +499,8 @@ KC_HD inline void medoid_phase(const Chunk &ch, int32_t r, int32_t lane, int32_t
         for (int32_t c = 0; c < n; ++c) {
             if (row[c].kind == K_NULL) continue;
             ch.mstr_off[s++] = (int32_t)at;
-            at += sanitized_copy(ch.text + row[c].vstart, row[c].vlen, ch.mchars + at);
+            const uint8_t *v = ch.text + row[c].vstart;
+            at += (row[c].flags & TOK_UNICODE) ? normalize_string(v, row[c].vlen, ch.mchars + at) : sanitized_copy(v, row[c].vlen, ch.mchars + at);
         }
         if (g + 1 == n_groups) {  // the chunk's last group closes both offset arrays
             ch.mgrp_off[n_groups] = (int32_t)n_strings;
@@ -561,7 +578,7 @@ KC_HD inline void union_count_phase(const Chunk &ch, int32_t p, int32_t lane, in
     for (int32_t c = lane; c < ch.n; c += team) {
         int64_t b, len;
         int32_t f = -D_TOO_LONG;
-        if (candidate_span(ch, r, c, b, len)) f = scan_object(ch.text + b, (uint32_t)len, 0, nullptr, 0, kMaxFields);
+        if (candidate_span(ch, r, c, b, len)) f = scan_object(ch.text + b, (uint32_t)len, 0, nullptr, 0, kMaxFields, nullptr, false, nullptr, ch.unicode);
         if (f < 0) decline(ch, r, f == -D_TOO_MANY_FIELDS ? D_KEYS_DIFFER : -f);  // one candidate alone is over the union's limit
         ch.ucand[(int64_t)p * ch.n + c] = f > 0 ? (uint32_t)f : 0u;
     }
@@ -594,7 +611,8 @@ KC_HD inline void union_scan_phase(const Chunk &ch, int32_t p, int32_t lane, int
     for (int32_t c = lane; c < ch.n; c += team) {
         int64_t b, len;
         candidate_span(ch, r, c, b, len);  // U1 checked it
-        scan_object(ch.text + b, (uint32_t)len, (uint32_t)b, ch.utok + ch.ubase[p] + ch.ucand[(int64_t)p * ch.n + c], 1, kMaxFields);
+        scan_object(ch.text + b, (uint32_t)len, (uint32_t)b, ch.utok + ch.ubase[p] + ch.ucand[(int64_t)p * ch.n + c], 1, kMaxFields, nullptr, false,
+                    nullptr, ch.unicode);
     }
 }
 
@@ -745,7 +763,7 @@ KC_HD inline void put_original(const Chunk &ch, const Tok &t, Sink &content) {
         to_double(ch.text + t.vstart, t.vlen, v);
         float_repr(v, content);
     } else if (t.kind == K_STR) {
-        content.json_string(ch.text + t.vstart, t.vlen, t.flags & TOK_ESCAPED);
+        content.json_string(ch.text + t.vstart, t.vlen, t.flags);
     } else {
         content.lit(t.kind == K_TRUE ? "true" : (t.kind == K_FALSE ? "false" : "null"));
     }
@@ -765,7 +783,7 @@ KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &cont
         if (kind == F_VOTE_BOOL) {
             content.lit(row[idx].kind == K_TRUE ? "true" : "false");  // the processed key (cu:958)
         } else {
-            content.json_string(ch.text + row[idx].vstart, row[idx].vlen, row[idx].flags & TOK_ESCAPED);  // first original whose sanitised form wins (cu:971)
+            content.json_string(ch.text + row[idx].vstart, row[idx].vlen, row[idx].flags);  // first original whose sanitised form wins (cu:971)
         }
     } else if (kind == F_NUMERIC && ch.xmedoid) {  // the async dispatcher's similarity medoid (cu:1638-1688, K5)
         uint32_t live = 0;
@@ -806,7 +824,7 @@ KC_HD inline void format_field(const Chunk &ch, int32_t r, int32_t j, Sink &cont
         for (int32_t c = 0; c < n; ++c) {
             if (row[c].kind == K_NULL) continue;
             if (want-- == 0) {
-                content.json_string(ch.text + row[c].vstart, row[c].vlen, row[c].flags & TOK_ESCAPED);
+                content.json_string(ch.text + row[c].vstart, row[c].vlen, row[c].flags);
                 break;
             }
         }

@@ -187,11 +187,12 @@ def _native_consolidate(records, rel_eps, abs_eps, device: int = 0, seq_logprobs
     [R*n], the candidates' sums): likelihood-weighted votes (kc_consolidate_json_packed_weighted; no host path).  flags:
     _native.JSON_NUMERIC_MEDOID for the async dispatcher (no host path either).  Records whose candidates differ in shape (key
     order, missing or extra keys, null sub-objects) stay on the device (JSON_KEY_UNION, always set here), and so do records with
-    list fields (JSON_LISTS: the alignment pre-pass on host threads, then the aligned texts on the device).  counts (optional
-    dict): "device" += the records the device path consolidated."""
+    list fields (JSON_LISTS: the alignment pre-pass on host threads, then the aligned texts on the device), and so do records
+    whose similarity-medoid fields hold non-ASCII text or \\uXXXX escapes (JSON_UNICODE).  counts (optional dict): "device" +=
+    the records the device path consolidated."""
     from .. import _native
     blob, off, n = _native.pack_texts(records, pinned=len(records) >= 256)  # page-locking only pays for batches
-    flags |= _native.JSON_KEY_UNION | _native.JSON_LISTS
+    flags |= _native.JSON_KEY_UNION | _native.JSON_LISTS | _native.JSON_UNICODE
     if seq_logprobs is None:
         res = _native.consolidate_json_packed(blob, off, n, rel_eps, abs_eps, device, flags=flags)
     else:

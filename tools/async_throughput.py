@@ -3,7 +3,7 @@
 1. requests/s and p50 / p99 latency of async_consolidate_parsed_chat_completions at 1, 16 and 256 concurrent requests on one event
    loop, on S32 texts (SURVEY.md section 8d) or (--workload invoice_optional) invoice texts whose candidates reorder, drop and add
    keys, (invoice_lines) invoice texts whose `items` is a list of line items, or (mixed_lines) S32 and invoice_lines requests
-   interleaved (tools/jsonpacked_throughput.py), at n = 3 and 16: the native route (device JSON path, requests combined per
+   interleaved, or (unicode_invoice) invoice texts with accented, curly-quoted free text (tools/jsonpacked_throughput.py), at n = 3 and 16: the native route (device JSON path, requests combined per
    device call) against the Python async route (_consensus_async) on the same contents.
 2. kernel time of K5 (kc_numeric_medoid_f64) against K2 (kc_numeric_f64) on the same S32 numeric cells, 1 M records x 8 fields,
    at n = 4, 16, 32, 64 (CUDA events, median of 20 launches).
@@ -41,6 +41,9 @@ def s32_completions(count, n, seed, workload="s32"):
     elif workload == "invoice_lines":
         from tools.jsonpacked_throughput import invoice_lines_texts
         records = invoice_lines_texts(count, n, seed)
+    elif workload == "unicode_invoice":
+        from tools.jsonpacked_throughput import invoice_texts
+        records = invoice_texts(count, n, seed, accents=True)
     elif workload == "mixed_lines":
         from tools.jsonpacked_throughput import invoice_lines_texts
         records = [r for pair in zip(s32(count // 2), invoice_lines_texts(count - count // 2, n, seed)) for r in pair]
@@ -119,7 +122,7 @@ def kernel_rows(card):
 def main():
     import argparse
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["s32", "invoice_optional", "invoice_lines", "mixed_lines"], default="s32",
+    ap.add_argument("--workload", choices=["s32", "invoice_optional", "invoice_lines", "mixed_lines", "unicode_invoice"], default="s32",
                     help="the request rows' candidate texts")
     ap.add_argument("--requests", type=int, default=2048, help="requests per row (the Python route runs at most 256 of them)")
     ap.add_argument("--requests-only", action="store_true", help="skip the K5 / K2 kernel rows")

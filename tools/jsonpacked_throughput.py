@@ -15,17 +15,24 @@ from k_llms_b200 import _native as K  # noqa: E402
 P_REORDER, P_DROP, P_EXTRA, P_NULL_SUB, P_MISSING_SUB = 0.5, 0.2, 0.2, 0.1, 0.05
 
 
-def invoice_texts(records, n, seed, nested=False, optional=False):
+def invoice_texts(records, n, seed, nested=False, optional=False, accents=False):
     """An extraction-like schema with FREE-TEXT fields (multi-word strings -> similarity medoid, K4) next to enums, bools and
     numbers: 4 phrases, 3 enums, 2 bools, 3 numbers per record; every candidate copies the record's truth with probability 0.8
     per field, otherwise a variant (case / punctuation / one word changed / another value), None with probability 0.05.
-    optional: the candidates differ in shape as well (P_* above): the device path's key-union round."""
+    optional: the candidates differ in shape as well (P_* above): the device path's key-union round.  accents: the free-text
+    fields hold accented letters, curly quotes, dashes and the euro sign, as raw UTF-8 (the enums stay ASCII): the device
+    path's KC_JSON_UNICODE medoids."""
     import random
     rng = random.Random(seed)
     vendors = ["Acme Industrial Supply Co", "Globex Logistics and Freight", "Initech Software Services Ltd", "Umbrella Medical Devices Inc"]
     streets = ["12 Rue de la Paix 75002 Paris", "221B Baker Street London NW1", "1600 Amphitheatre Parkway Mountain View", "5 Avenue Anatole France Paris"]
     terms = ["net 30 days from invoice date", "payment due on receipt", "2 percent 10 net 30", "net 60 days end of month"]
     notes = ["deliver to the rear loading dock", "fragile handle with care", "partial shipment remaining items to follow", "customer will collect in person"]
+    if accents:
+        vendors = ["Société Générale d’Équipement", "Müller & Söhne Großhandel GmbH", "Café “Le Pâtissier” Fournitures", "Łódź Ćwiczenia Spółka z o.o."]
+        streets = ["12 Rue de la Paix — 75002 Paris", "Königstraße 5, 70173 Stuttgart", "Praça da Sé 108 — São Paulo", "Calle de Alcalá 48, Madrid"]
+        terms = ["net 30 days — 2 % escompte", "payment due on receipt (€)", "Zahlung binnen 14 Tagen netto", "net 60 days “end of month”"]
+        notes = ["livraison à l’entrée arrière", "fragile — handle with care", "envío parcial, el resto a continuación", "Kunde holt selbst ab"]
 
     def vary(p):
         r = rng.random()
@@ -67,7 +74,7 @@ def invoice_texts(records, n, seed, nested=False, optional=False):
                      "kind": d["kind"], "note": d["note"], "items": d["items"]}
             if optional:
                 d = _optional(rng, d, top=True)
-            cands.append(json.dumps(d))
+            cands.append(json.dumps(d, ensure_ascii=not accents))
         out.append(cands)
     return out
 
@@ -126,15 +133,19 @@ def _optional(rng, d, top=False):
     return dict(items)
 
 
+def workload_texts(workload, records, n, seed):
+    """The candidate texts of an invoice workload."""
+    if workload == "invoice_lines":
+        return invoice_lines_texts(records, n, seed)
+    return invoice_texts(records, n, seed, nested="nested" in workload, optional="optional" in workload, accents=workload == "unicode_invoice")
+
+
 def batch_api(args):
     """consolidate_contents_batch on the workload's records: what the batch API (and, weighted, its Python planner for what the
     device path declines) does per call.  One JSON line, best of --reps after one warm-up call."""
     import random
     from k_llms_b200.utils import consolidation as C
-    if args.workload == "invoice_lines":
-        records = invoice_lines_texts(args.records, args.n, 11)
-    else:
-        records = invoice_texts(args.records, args.n, 11, nested="nested" in args.workload, optional="optional" in args.workload)
+    records = workload_texts(args.workload, args.records, args.n, 11)
     rng = random.Random(3)
     lps = [[[-rng.random() * 4, -rng.random()] for _ in r] for r in records] if args.weighted else None
     embed = lambda t: [[0.0] for _ in t]  # noqa: E731  (never called: no pair of long strings in these workloads)
@@ -152,11 +163,13 @@ def batch_api(args):
 
 def main():
     ap = argparse.ArgumentParser()
-    ap.add_argument("--workload", choices=["s32", "invoice", "invoice_nested", "invoice_optional", "invoice_nested_optional", "invoice_lines"],
+    ap.add_argument("--workload", choices=["s32", "invoice", "invoice_nested", "invoice_optional", "invoice_nested_optional", "invoice_lines",
+                                           "unicode_invoice"],
                     default="s32",
                     help="s32: the bench schema (enum / bool / number fields); invoice: 12 fields, 4 of them free text (medoid, K4); "
                          "invoice_nested: the same fields in nested objects (depth 3); *_optional: candidates that reorder, drop and add "
-                         "keys and (nested) hold None or nothing for sub-objects; invoice_lines: `items` is a list of line items (list round)")
+                         "keys and (nested) hold None or nothing for sub-objects; invoice_lines: `items` is a list of line items (list round); "
+                         "unicode_invoice: invoice with accented, curly-quoted free text (KC_JSON_UNICODE)")
     ap.add_argument("--records", type=int, default=262144)
     ap.add_argument("--n", type=int, default=16)
     ap.add_argument("--reps", type=int, default=4)
@@ -165,21 +178,22 @@ def main():
     ap.add_argument("--pageable", action="store_true", help="input blob in ordinary (not page-locked) memory")
     ap.add_argument("--weighted", action="store_true", help="the likelihood-weighted variant (random candidate sums)")
     ap.add_argument("--no-lists", action="store_true", help="without JSON_LISTS: list records go to the host path (H1)")
+    ap.add_argument("--no-unicode", action="store_true",
+                    help="without JSON_UNICODE (here and in the batch API): non-ASCII records take the routes they took before it")
     ap.add_argument("--batch-api", action="store_true",
                     help="time consolidate_contents_batch (with --weighted: token logprobs, two per candidate) instead of the C-ABI call")
     args = ap.parse_args()
+    if args.no_unicode:
+        K.JSON_UNICODE = 0  # consolidation._native_consolidate reads it per call
     if args.batch_api:
         return batch_api(args)
     t0 = time.perf_counter()
-    if args.workload == "invoice_lines":
-        blob, off, _n = K.pack_texts(invoice_lines_texts(args.records, args.n, 11), pinned=not args.pageable)
-    elif args.workload != "s32":
-        blob, off, _n = K.pack_texts(invoice_texts(args.records, args.n, 11, nested="nested" in args.workload, optional="optional" in args.workload),
-                                     pinned=not args.pageable)
+    if args.workload != "s32":
+        blob, off, _n = K.pack_texts(workload_texts(args.workload, args.records, args.n, 11), pinned=not args.pageable)
     else:
         blob, off = K.s32_texts_packed(args.records, args.n, 11, pinned=not args.pageable)
     gen_s = time.perf_counter() - t0
-    flags = K.JSON_KEY_UNION | (0 if args.no_lists else K.JSON_LISTS)  # as the client functions call it
+    flags = K.JSON_KEY_UNION | (0 if args.no_lists else K.JSON_LISTS) | K.JSON_UNICODE  # as the client functions call it
     seq = None
     if args.weighted:
         import numpy as np
@@ -208,7 +222,7 @@ def main():
                               "records_per_s": round(args.records / best), "n_device": stats["n_device"], "n_host": stats["n_host"],
                               "n_python": stats["n_python"], "json_GBps": round(stats["input_bytes"] / best / 1e9, 2),
                               "stats": {k: (round(v, 2) if isinstance(v, float) else v) for k, v in stats.items()},
-                              "generate_s": round(gen_s, 1), "example": first[:80]}), flush=True)
+                              "generate_s": round(gen_s, 1), "example": (first or "")[:80]}), flush=True)
 
 
 if __name__ == "__main__":
