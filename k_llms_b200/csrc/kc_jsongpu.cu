@@ -92,28 +92,66 @@ struct PBuf {  // grow-only pinned host buffer
     T *as() const { return static_cast<T *>(p); }
 };
 
-constexpr int kSlotArrays = 8;
-
-// The chunk's slot-sized arrays, each named once: its buffer index, its elements per field slot, its minimum length and the
-// byte its new elements are filled with.  alloc(k, ptr, len, keep, fill, on_device) sizes buffer k for len elements keeping the
-// first `keep`, binds ptr to it and fills the rest: the host twin fills every array, the device only those marked on_device
-// (the cell matrices: a record declined while encoding leaves its rows untouched, and K1 / K2 read them; every other element
-// is written before it is read).  vrec: the vote groups' records, for weighted calls.
+// Every array of a chunk that the device worker and the host twin both size, each named once: the Stage that sizes it (OFF:
+// the chunk does not use it), its length (a count of one of the Units, times a number per unit, plus a constant), the byte
+// its new elements are filled with, and whether the device fills them too (the twin fills every array; the device only what
+// is read without having been written: rows of records declined while encoding, counts of records declined before
+// slots_phase, entry R of the scanned counts).  alloc(k, ptr, len, keep, fill, on_device) sizes buffer k for len elements
+// keeping the first `keep` (the slots A1 wrote, when the union round adds its rows), binds ptr to it and fills the rest.
+enum Stage { RECORDS, SLOTS, UNION, SCRATCH, CSR, OFF };  // before A0, after the slot scan and U2, before U1, after U1, before A2
+struct Units {  // records and text bytes; then field slots, union-round records and union scratch entries, counted on the device
+    size_t R, B, T = 0, P = 0, S = 0;
+};
 template <class Alloc>
-int slot_arrays(const Alloc &alloc, Chunk &ch, size_t T, size_t keep, bool vrec) {
+int chunk_arrays(const Alloc &alloc, Chunk &ch, Stage stage, const Units &u, size_t keep, bool vrec) {
     const size_t n = (size_t)ch.n;
-    auto a = [&](int k, auto *&ptr, size_t per, size_t min, int fill, bool on_device) {
-        return alloc(k, ptr, std::max(T * per, min), keep * per, fill, on_device);
+    int k = 0;
+    auto a = [&](Stage st, auto *&ptr, size_t count, size_t per, size_t plus, int fill, bool on_device) {
+        const int i = k++;
+        return st == stage ? alloc(i, ptr, count * per + plus, keep * per, fill, on_device) : KC_OK;
     };
-    R_(a(0, ch.toks, n, 1, 0, false));
-    R_(a(1, ch.fdesc, 1, 1, 0, false));
-    R_(a(2, ch.gpos, 1, 1, 0, false));
-    R_(a(3, ch.piece_c, 1, 1, 0, false));
-    R_(a(4, ch.piece_l, 1, 1, 0, false));
-    R_(a(5, ch.vcells, n, 16, 0xFF, true));  // KC_CODE_NONE
-    R_(a(6, ch.xcells, n, 2, 0, true));
-    if (vrec) R_(a(7, ch.vrec, 1, 1, 0xFF, false));  // -1
+    R_(a(RECORDS, ch.fcount, u.R, 1, 1, 0, true));
+    R_(a(RECORDS, ch.slot, u.R, 1, 1, 0, false));
+    R_(a(RECORDS, ch.status, u.R, 1, 0, 0, false));
+    R_(a(RECORDS, ch.nest, u.R, 1, 0, 0, false));
+    R_(a(RECORDS, ch.pend, u.R, 1, 0, 0, false));
+    R_(a(RECORDS, ch.plist, u.R, 1, 1, 0xFF, false));  // -1
+    R_(a(ch.lists ? RECORDS : OFF, ch.lst, u.R, 1, 0, 0, false));
+    R_(a(RECORDS, ch.vbase, u.R, 1, 0, 0, false));
+    R_(a(RECORDS, ch.xbase, u.R, 1, 0, 0, false));
+    R_(a(RECORDS, ch.mcount, u.R, 1, 1, 0, true));
+    R_(a(RECORDS, ch.scount, u.R, 1, 1, 0, true));
+    R_(a(RECORDS, ch.ccount, u.R, 1, 1, 0, true));
+    R_(a(RECORDS, ch.len_c, u.R, 1, 1, 0, true));
+    R_(a(RECORDS, ch.len_l, u.R, 1, 1, 0, true));
+    R_(a(SLOTS, ch.toks, u.T, n, 1, 0, false));
+    R_(a(SLOTS, ch.fdesc, u.T, 1, 1, 0, false));
+    R_(a(SLOTS, ch.gpos, u.T, 1, 1, 0, false));
+    R_(a(SLOTS, ch.piece_c, u.T, 1, 1, 0, false));
+    R_(a(SLOTS, ch.piece_l, u.T, 1, 1, 0, false));
+    R_(a(SLOTS, ch.vcells, u.T, n, 16, 0xFF, true));  // KC_CODE_NONE
+    R_(a(SLOTS, ch.xcells, u.T, n, 2, 0, true));
+    R_(a(vrec ? SLOTS : OFF, ch.vrec, u.T, 1, 1, 0xFF, false));  // -1
+    R_(a(UNION, ch.ucand, u.P, n, 0, 0, false));
+    R_(a(UNION, ch.ubase, u.P, 1, 0, 0, false));
+    R_(a(UNION, ch.usize, u.P, 1, 0, 0, false));
+    R_(a(SCRATCH, ch.utok, u.S, 1, 0, 0, false));
+    R_(a(SCRATCH, ch.unode, u.S, 1, 0, 0, false));
+    R_(a(SCRATCH, ch.umap, u.S, 1, 0, 0xFF, false));  // -1
+    // upper bounds (no read-back): normalised characters are a subset of the text, <= n strings a group, <= fcount groups a record
+    R_(a(CSR, ch.mchars, u.B, 1, 16, 0, false));
+    R_(a(CSR, ch.mstr_off, u.T, n, 2, 0, false));
+    R_(a(CSR, ch.mgrp_off, u.T, 1, 2, 0, false));
     return KC_OK;
+}
+
+// the Chunk's switches for a call's flags, in round `lists` (Chunk::lists); records [aligned0, R) are in the aligned round
+void set_flags(Chunk &ch, uint32_t flags, uint8_t lists, int32_t aligned0) {
+    ch.xmedoid = (flags & KC_JSON_NUMERIC_MEDOID) != 0;
+    ch.key_union = (flags & KC_JSON_KEY_UNION) != 0;
+    ch.unicode = (flags & KC_JSON_UNICODE) != 0;
+    ch.lists = lists;
+    ch.aligned0 = aligned0;
 }
 
 // Everything one in-flight chunk needs on the device.  Workers are pooled per device and reused across calls.
@@ -121,9 +159,8 @@ struct Worker {
     int device = -1;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[7] = {};
-    DBuf text, off, fcount, slot, status, vbase, xbase, counters, win, vmeta, xvalue, xmeta, len_c, len_l, out_c, out_l, scan_tmp, mcount,
-        scount, ccount, mchars, mstr_off, mgrp_off, midx, mavg, nest, seq, vweight, pend, plist, ucand, ubase, usize, utok, unode, umap, lst;
-    DBuf slot_buf[kSlotArrays];  // slot_arrays
+    DBuf text, off, counters, win, vmeta, xvalue, xmeta, out_c, out_l, scan_tmp, midx, mavg, seq, vweight;
+    std::vector<DBuf> arrays;  // chunk_arrays
     PBuf h_small;  // totals and counters (pinned so the small D2H copies are asynchronous)
     PBuf h_scan;   // the scanned record offsets and the statuses of a chunk
     bool busy = false;
@@ -215,18 +252,20 @@ int team_size(int n) {
     return t;
 }
 
-// the device slot arrays for T slots (the first `keep` kept), and the result arrays of K1 (or K3b), K2 (or K5) beside them
-int size_slots(Worker &w, Chunk &ch, size_t T, size_t keep, bool weighted) {
-    cudaStream_t s = w.stream;
+// the chunk arrays of one stage in the worker's device buffers (grown and filled on its stream), and with the slots the result
+// arrays of K1 (or K3b), K2 (or K5) beside them
+int device_arrays(Worker &w, Chunk &ch, Stage stage, const Units &u, size_t keep, bool weighted) {
     auto dev = [&](int k, auto *&ptr, size_t len, size_t keep_len, int fill, bool on_device) -> int {
         using E = std::remove_reference_t<decltype(*ptr)>;
-        R_(w.slot_buf[k].grow(len * sizeof(E), keep_len * sizeof(E), s));
-        ptr = w.slot_buf[k].as<E>();
-        if (on_device) KC_CUDA_I(cudaMemsetAsync(ptr + keep_len, fill, (len - keep_len) * sizeof(E), s));
+        if (w.arrays.size() <= (size_t)k) w.arrays.resize((size_t)k + 1);
+        R_(w.arrays[(size_t)k].grow(len * sizeof(E), keep_len * sizeof(E), w.stream));
+        ptr = w.arrays[(size_t)k].as<E>();
+        if (on_device) KC_CUDA_I(cudaMemsetAsync(ptr + keep_len, fill, (len - keep_len) * sizeof(E), w.stream));
         return KC_OK;
     };
-    R_(slot_arrays(dev, ch, T, keep, weighted));
-    const size_t T1 = std::max<size_t>(T, 1);
+    R_(chunk_arrays(dev, ch, stage, u, keep, weighted));
+    if (stage != SLOTS) return KC_OK;
+    const size_t T1 = std::max<size_t>(u.T, 1);
     R_(w.win.reserve(T1 * 4));
     R_(w.vmeta.reserve(T1 * 4));
     R_(w.xvalue.reserve(T1 * 8));
@@ -244,11 +283,11 @@ int size_slots(Worker &w, Chunk &ch, size_t T, size_t keep, bool weighted) {
 }
 
 template <typename T>
-void exclusive_scan(std::vector<T> &v) {  // in place, as cub::DeviceScan::ExclusiveSum
+void exclusive_scan(T *v, size_t len) {  // in place, as cub::DeviceScan::ExclusiveSum
     T acc = 0;
-    for (T &x : v) {
-        const T c = x;
-        x = acc;
+    for (size_t i = 0; i < len; ++i) {
+        const T c = v[i];
+        v[i] = acc;
         acc += c;
     }
 }
@@ -274,41 +313,30 @@ struct ChunkStage {  // per-chunk device-time split (CUDA events on the chunk's 
 // The union round of a chunk whose A1 sent P records to it (kc_jsongpu.cuh, U1-U3): U1 counts the candidates' tokens and
 // reserves scratch, U2 builds the union trees and reserves union rows behind the first round's T slots, U3 writes the tables
 // and runs A1's phases on them.  Two read-backs size the scratch and the rows; the arrays A1 has already written grow with
-// their contents kept.  On return T counts the union rows too, and h_cnt[0..2] the chunk's groups.
-int union_round(Worker &w, Chunk &ch, int64_t P, size_t &T, int team, int grid, bool weighted, unsigned long long *h_cnt) {
+// their contents kept.  On return u.T counts the union rows too, and h_cnt[0..2] the chunk's groups.
+int union_round(Worker &w, Chunk &ch, Units &u, int team, int grid, bool weighted, unsigned long long *h_cnt) {
     cudaStream_t s = w.stream;
-    const int32_t n = ch.n;
-    R_(w.ucand.reserve((size_t)P * n * 4));
-    R_(w.ubase.reserve((size_t)P * 4));
-    R_(w.usize.reserve((size_t)P * 4));
-    ch.ucand = w.ucand.as<uint32_t>();
-    ch.ubase = w.ubase.as<uint32_t>();
-    ch.usize = w.usize.as<uint32_t>();
-    ch.uslot = (uint32_t)T;
-    kc::js::union_count_kernel<<<grid, 128, 0, s>>>(ch, team, (int32_t)P);
+    const int32_t P = (int32_t)u.P;
+    R_(device_arrays(w, ch, UNION, u, 0, weighted));
+    ch.uslot = (uint32_t)u.T;
+    kc::js::union_count_kernel<<<grid, 128, 0, s>>>(ch, team, P);
     KC_CUDA_I(cudaGetLastError());
     KC_CUDA_I(cudaMemcpyAsync(h_cnt, ch.counters, 48, cudaMemcpyDeviceToHost, s));
     KC_CUDA_I(cudaStreamSynchronize(s));
-    const size_t S = std::max<size_t>(h_cnt[4], 1);  // scratch entries: tokens of the candidates, plus a root per record
-    if (S >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: %zu union scratch entries in one chunk", S);
-    R_(w.utok.reserve(S * sizeof(Tok)));
-    R_(w.unode.reserve(S * sizeof(kc::js::UNode)));
-    R_(w.umap.reserve(S * 4));
-    ch.utok = w.utok.as<Tok>();
-    ch.unode = w.unode.as<kc::js::UNode>();
-    ch.umap = w.umap.as<int32_t>();
-    kc::js::union_build_kernel<<<grid, 128, 0, s>>>(ch, team, (int32_t)P);
+    u.S = std::max<size_t>(h_cnt[4], 1);  // scratch entries: tokens of the candidates, plus a root per record
+    if (u.S >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: %zu union scratch entries in one chunk", u.S);
+    R_(device_arrays(w, ch, SCRATCH, u, 0, weighted));
+    kc::js::union_build_kernel<<<grid, 128, 0, s>>>(ch, team, P);
     KC_CUDA_I(cudaGetLastError());
     KC_CUDA_I(cudaMemcpyAsync(h_cnt, ch.counters, 48, cudaMemcpyDeviceToHost, s));
     KC_CUDA_I(cudaStreamSynchronize(s));
-    const size_t U = h_cnt[5];
-    if (U) {
-        const size_t T1 = T + U;
-        if (T1 >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: %zu field slots in one chunk", T1);
-        R_(size_slots(w, ch, T1, T, weighted));
-        T = T1;
+    if (const size_t U = h_cnt[5]) {
+        const size_t keep = u.T;
+        u.T += U;
+        if (u.T >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: %zu field slots in one chunk", u.T);
+        R_(device_arrays(w, ch, SLOTS, u, keep, weighted));
     }
-    kc::js::union_plan_kernel<<<grid, 128, 0, s>>>(ch, team, (int32_t)P);
+    kc::js::union_plan_kernel<<<grid, 128, 0, s>>>(ch, team, P);
     KC_CUDA_I(cudaGetLastError());
     KC_CUDA_I(cudaMemcpyAsync(h_cnt, ch.counters, 48, cudaMemcpyDeviceToHost, s));
     KC_CUDA_I(cudaStreamSynchronize(s));
@@ -316,34 +344,26 @@ int union_round(Worker &w, Chunk &ch, int64_t P, size_t &T, int team, int grid, 
 }
 
 // One chunk on one worker: records [r0, r1) of the batch.  h_seq (NULL: count votes): the batch's candidate sums [R][n], the
-// vote leaves are likelihood-weighted (K3b over ragged records in K1's place).  xmedoid (KC_JSON_NUMERIC_MEDOID): numeric fields
-// are similarity medoids (K5 in K2's place).  lists: Chunk::lists.  dst (NULL: the identity): the result index of each record
-// of the batch (the aligned round's batch is the list records, in the order of their result indices).
-int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, bool xmedoid, bool key_union, uint8_t lists, bool unicode,
-              const int64_t *dst, int64_t r0, int64_t r1, int32_t n, double rel_eps, double abs_eps, int sm_count, kc_json_result &res,
-              ChunkStage &st) {
+// vote leaves are likelihood-weighted (K3b over ragged records in K1's place).  flags: the call's KC_JSON_* flags (set_flags);
+// lists: Chunk::lists.  dst (NULL: the identity): the result index of each record of the batch (the aligned round's batch is
+// the list records, in the order of their result indices).
+int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *h_seq, uint32_t flags, uint8_t lists, const int64_t *dst,
+              int64_t r0, int64_t r1, int32_t n, double rel_eps, double abs_eps, int sm_count, kc_json_result &res, ChunkStage &st) {
     const int64_t Rc = r1 - r0;
     const int64_t b0 = h_off[r0 * n], b1 = h_off[r1 * n];
     const size_t bytes = (size_t)(b1 - b0);
     if (bytes >= ((size_t)1 << 32)) return kc_fail(KC_EINVAL, "kc_consolidate_json_packed: chunk of %zu bytes", bytes);
     cudaStream_t s = w.stream;
+    const bool weighted = h_seq != nullptr;
+    Chunk ch{};
+    ch.R = (int32_t)Rc;
+    ch.n = n;
+    set_flags(ch, flags, lists, INT32_MAX);  // a chunk is in one round: Chunk::lists says which
+    Units u{(size_t)Rc, bytes};
+    R_(device_arrays(w, ch, RECORDS, u, 0, weighted));
     R_(w.text.reserve(bytes + 16));
     R_(w.off.reserve((size_t)(Rc * n + 1) * 8));
-    R_(w.fcount.reserve((size_t)(Rc + 1) * 4));
-    R_(w.slot.reserve((size_t)(Rc + 1) * 4));
-    R_(w.status.reserve((size_t)Rc));
-    R_(w.nest.reserve((size_t)Rc));
-    R_(w.pend.reserve((size_t)Rc));
-    R_(w.plist.reserve((size_t)Rc * 4));
-    if (lists) R_(w.lst.reserve((size_t)Rc));
-    R_(w.vbase.reserve((size_t)Rc * 4));
-    R_(w.xbase.reserve((size_t)Rc * 4));
     R_(w.counters.reserve(48));
-    R_(w.mcount.reserve((size_t)(Rc + 1) * 4));
-    R_(w.scount.reserve((size_t)(Rc + 1) * 4));
-    R_(w.ccount.reserve((size_t)(Rc + 1) * 4));
-    R_(w.len_c.reserve((size_t)(Rc + 1) * 8));
-    R_(w.len_l.reserve((size_t)(Rc + 1) * 8));
     R_(w.h_small.reserve(64));  // the slot total, then the six counters
     R_(w.h_scan.reserve((size_t)(Rc + 1) * 16 + (size_t)Rc));
     if (h_seq) R_(w.seq.reserve((size_t)std::max<int64_t>(Rc * n, 1) * 4));
@@ -351,32 +371,9 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes, (const int64_t *)nullptr, (int64_t *)nullptr, (int)(Rc + 1), s);
     cub::DeviceScan::ExclusiveSum(nullptr, tmp_bytes32, (const uint32_t *)nullptr, (uint32_t *)nullptr, (int)(Rc + 1), s);
     R_(w.scan_tmp.reserve(std::max(tmp_bytes, tmp_bytes32) + 256));
-
-    Chunk ch{};
     ch.text = w.text.as<uint8_t>();
     ch.off = w.off.as<int64_t>();
-    ch.R = (int32_t)Rc;
-    ch.n = n;
-    ch.fcount = w.fcount.as<uint32_t>();
-    ch.slot = w.slot.as<uint32_t>();
-    ch.status = w.status.as<uint8_t>();
-    ch.nest = w.nest.as<uint8_t>();
-    ch.pend = w.pend.as<uint8_t>();
-    ch.plist = w.plist.as<int32_t>();
-    ch.vbase = w.vbase.as<uint32_t>();
-    ch.xbase = w.xbase.as<uint32_t>();
     ch.counters = w.counters.as<unsigned long long>();
-    ch.mcount = w.mcount.as<uint32_t>();
-    ch.scount = w.scount.as<uint32_t>();
-    ch.ccount = w.ccount.as<uint32_t>();
-    ch.len_c = w.len_c.as<int64_t>();
-    ch.len_l = w.len_l.as<int64_t>();
-    ch.xmedoid = xmedoid;
-    ch.key_union = key_union;
-    ch.lst = lists ? w.lst.as<uint8_t>() : nullptr;
-    ch.lists = lists;
-    ch.aligned0 = INT32_MAX;  // a chunk is in one round: Chunk::lists says which
-    ch.unicode = unicode;
 
     nvtxRangePushA("kc_json: H2D texts");
     KC_CUDA_I(cudaEventRecord(w.ev[0], s));
@@ -395,7 +392,6 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     };
     auto team_grid = [&](int64_t units) { return grid_for((units + tpw - 1) / tpw * 32); };  // a warp per tpw units
     // A0: fields per record, then their exclusive scan (entry Rc of fcount is 0, so slot[Rc] is the total)
-    KC_CUDA_I(cudaMemsetAsync(ch.fcount + Rc, 0, 4, s));
     kc::js::count_kernel<<<grid_for(Rc), 128, 0, s>>>(ch);
     KC_CUDA_I(cudaGetLastError());
     size_t tb = w.scan_tmp.cap;
@@ -403,37 +399,27 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
     uint32_t *h_total = w.h_small.as<uint32_t>();
     KC_CUDA_I(cudaMemcpyAsync(h_total, ch.slot + Rc, 4, cudaMemcpyDeviceToHost, s));
     KC_CUDA_I(cudaStreamSynchronize(s));
-    size_t T = *h_total;  // field slots of the chunk (after a union round: its rows too)
-    R_(size_slots(w, ch, T, 0, h_seq != nullptr));
+    u.T = *h_total;  // field slots of the chunk (after a union round: its rows too)
+    R_(device_arrays(w, ch, SLOTS, u, 0, weighted));
     KC_CUDA_I(cudaMemsetAsync(w.counters.p, 0, 48, s));
-    // records declined before slots_phase own no medoid groups
-    KC_CUDA_I(cudaMemsetAsync(w.mcount.p, 0, (size_t)(Rc + 1) * 4, s));
-    KC_CUDA_I(cudaMemsetAsync(w.scount.p, 0, (size_t)(Rc + 1) * 4, s));
-    KC_CUDA_I(cudaMemsetAsync(w.ccount.p, 0, (size_t)(Rc + 1) * 4, s));
     int64_t gv = 0, gx = 0, gm = 0;
-    if (T) {
+    if (u.T) {
         kc::js::plan_kernel<<<team_grid(Rc), 128, 0, s>>>(ch, team);
         KC_CUDA_I(cudaGetLastError());
         unsigned long long *h_cnt = w.h_small.as<unsigned long long>() + 1;
         KC_CUDA_I(cudaMemcpyAsync(h_cnt, w.counters.p, 32, cudaMemcpyDeviceToHost, s));
         KC_CUDA_I(cudaStreamSynchronize(s));
-        if (const int64_t P = (int64_t)h_cnt[3])  // records whose candidates differ in shape
-            R_(union_round(w, ch, P, T, team, team_grid(P), h_seq != nullptr, h_cnt));
+        if ((u.P = h_cnt[3]))  // records whose candidates differ in shape
+            R_(union_round(w, ch, u, team, team_grid((int64_t)u.P), weighted, h_cnt));
         gv = (int64_t)h_cnt[0];
         gx = (int64_t)h_cnt[1];
         gm = (int64_t)h_cnt[2];
     }
     if (gm) {
-        // A2: multi-word string fields -> K4's CSR input.  Sizes by upper bound (no read-back): the normalised characters are a
-        // subset of the chunk's text, a group has at most n strings, a record at most fcount groups.
-        R_(w.mchars.reserve(bytes + 16));
-        R_(w.mstr_off.reserve((T * (size_t)n + 2) * 4));
-        R_(w.mgrp_off.reserve((T + 2) * 4));
-        R_(w.midx.reserve((T + 1) * 4));
-        R_(w.mavg.reserve((T + 1) * 8));
-        ch.mchars = w.mchars.as<uint8_t>();
-        ch.mstr_off = w.mstr_off.as<int32_t>();
-        ch.mgrp_off = w.mgrp_off.as<int32_t>();
+        // A2: multi-word string fields -> K4's CSR input
+        R_(device_arrays(w, ch, CSR, u, 0, weighted));
+        R_(w.midx.reserve((u.T + 1) * 4));
+        R_(w.mavg.reserve((u.T + 1) * 8));
         ch.midx = w.midx.as<int32_t>();
         ch.mavg = w.mavg.as<double>();
         for (uint32_t *cnt : {ch.mcount, ch.scount, ch.ccount}) {
@@ -452,15 +438,13 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
                                       w.vweight.as<float>(), s));
     else if (gv)
         R_(kc_vote_i8(ch.vcells, gv, n, nullptr, 1, w.win.as<int32_t>(), w.vmeta.as<uint32_t>(), s));
-    if (gx && xmedoid) R_(kc_numeric_medoid_f64(ch.xcells, gx, n, w.xmeta.as<int32_t>(), w.xvalue.as<double>(), s));
+    if (gx && ch.xmedoid) R_(kc_numeric_medoid_f64(ch.xcells, gx, n, w.xmeta.as<int32_t>(), w.xvalue.as<double>(), s));
     else if (gx) R_(kc_numeric_f64(ch.xcells, gx, n, rel_eps, abs_eps, w.xvalue.as<double>(), w.xmeta.as<uint32_t>(), s));
     if (gm) R_(kc_medoid_str(ch.mchars, ch.mstr_off, ch.mgrp_off, gm, std::max(2, n), w.midx.as<int32_t>(), w.mavg.as<double>(), s));
     KC_CUDA_I(cudaEventRecord(w.ev[3], s));
     nvtxRangePop();
     nvtxRangePushA("kc_json: emit (C0 lengths, C1 write)");
     // C0: piece lengths and record lengths, then record offsets in the two output blobs
-    KC_CUDA_I(cudaMemsetAsync(ch.len_c + Rc, 0, 8, s));
-    KC_CUDA_I(cudaMemsetAsync(ch.len_l + Rc, 0, 8, s));
     kc::js::len_kernel<<<team_grid(Rc), 128, 0, s>>>(ch, team);
     KC_CUDA_I(cudaGetLastError());
     tb = w.scan_tmp.cap;
@@ -524,6 +508,19 @@ int run_chunk(Worker &w, const char *h_text, const int64_t *h_off, const float *
 
 namespace {
 
+// the candidate texts of the records in idx, record-major, as pointers into h_text and their lengths
+void gather(const char *h_text, const int64_t *h_off, int32_t n, const std::vector<int64_t> &idx, std::vector<const char *> &texts,
+            std::vector<int64_t> &lens) {
+    texts.resize(idx.size() * n);
+    lens.resize(idx.size() * n);
+    for (size_t i = 0; i < idx.size(); ++i)
+        for (int32_t c = 0; c < n; ++c) {
+            const int64_t k = idx[i] * n + c;
+            texts[i * n + c] = h_text + h_off[k];
+            lens[i * n + c] = h_off[k + 1] - h_off[k];
+        }
+}
+
 // The list round's alignment: the alignment pre-pass H2 (kc_align_json_batch) on host threads for the records in idx, which
 // the first round marked D_LIST.  The aligned texts of the records it aligns are packed record-major into one blob from
 // alloc(bytes) (off: their offsets, blob-relative; dst: their record indices); the records it declines go to `declined`.
@@ -533,14 +530,9 @@ template <class Alloc>
 int align_listed(const char *h_text, const int64_t *h_off, int32_t n, int device, int32_t threads, const std::vector<int64_t> &idx, const Alloc &alloc,
                  char *&blob, std::vector<int64_t> &off, std::vector<int64_t> &dst, std::vector<int64_t> &declined) {
     const int64_t L = (int64_t)idx.size();
-    std::vector<const char *> texts((size_t)(L * n));
-    std::vector<int64_t> lens((size_t)(L * n));
-    for (int64_t i = 0; i < L; ++i)
-        for (int32_t c = 0; c < n; ++c) {
-            const int64_t k = idx[(size_t)i] * n + c;
-            texts[(size_t)(i * n + c)] = h_text + h_off[k];
-            lens[(size_t)(i * n + c)] = h_off[k + 1] - h_off[k];
-        }
+    std::vector<const char *> texts;
+    std::vector<int64_t> lens;
+    gather(h_text, h_off, n, idx, texts, lens);
     std::vector<char *> out((size_t)(L * n), nullptr);
     std::vector<int32_t> st((size_t)L, 0);
     if (const int rc = kc_align_json_batch(texts.data(), lens.data(), L, n, /*min_support_ratio=*/0.51, device, threads, out.data(), st.data(), nullptr)) {
@@ -709,8 +701,8 @@ int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_
             while (!rc) {
                 const int k = next.fetch_add(1);
                 if (k >= chunks) break;
-                rc = run_chunk(w, text, off, seq, (flags & KC_JSON_NUMERIC_MEDOID) != 0, (flags & KC_JSON_KEY_UNION) != 0, lists,
-                               (flags & KC_JSON_UNICODE) != 0, dst, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res, stages[(size_t)wi]);
+                rc = run_chunk(w, text, off, seq, flags, lists, dst, cuts[(size_t)k], cuts[(size_t)k + 1], n, rel_eps, abs_eps, sm_count, *res,
+                               stages[(size_t)wi]);
             }
             if (rc) {
                 cudaStreamSynchronize(w.stream);
@@ -747,14 +739,9 @@ int consolidate_packed(const char *h_text, const int64_t *h_off, const float *h_
         }
         if (!idx.empty() && !(flags & KC_JSON_DEVICE_ONLY)) {
             const int64_t D = (int64_t)idx.size();
-            std::vector<const char *> texts((size_t)(D * n));
-            std::vector<int64_t> lens((size_t)(D * n));
-            for (int64_t i = 0; i < D; ++i)
-                for (int32_t c = 0; c < n; ++c) {
-                    const int64_t k = idx[(size_t)i] * n + c;
-                    texts[(size_t)(i * n + c)] = h_text + h_off[k];
-                    lens[(size_t)(i * n + c)] = h_off[k + 1] - h_off[k];
-                }
+            std::vector<const char *> texts;
+            std::vector<int64_t> lens;
+            gather(h_text, h_off, n, idx, texts, lens);
             std::vector<char *> oc((size_t)D, nullptr), ol((size_t)D, nullptr);
             std::vector<uint8_t> hs((size_t)D, 1);
             rc = kc_consolidate_json(texts.data(), lens.data(), D, n, rel_eps, abs_eps, device, threads, oc.data(), ol.data(), hs.data());
@@ -863,20 +850,9 @@ struct kc_debug_jsongpu {
     std::vector<uint8_t> text;
     int32_t n = 0;
     int64_t R = 0;
-    std::vector<uint32_t> fcount, slot, vbase, xbase;
-    std::vector<uint8_t> status, nest, pend;
-    std::vector<uint8_t> slot_mem[kSlotArrays];  // slot_arrays (operator new aligns them for any type, Tok's 16 bytes included)
+    std::vector<std::vector<uint8_t>> arrays;  // chunk_arrays (operator new aligns them for any type, Tok's 16 bytes included)
     unsigned long long counters[6] = {0, 0, 0, 0, 0, 0};
-    std::vector<int32_t> plist, umap;
-    std::vector<uint32_t> ucand, ubase, usize;
-    std::vector<Tok> utok;
-    std::vector<kc::js::UNode> unode;
-    std::vector<uint32_t> mcount, scount, ccount;
-    std::vector<uint8_t> mchars;
-    std::vector<int32_t> mstr_off, mgrp_off;
-    std::vector<int64_t> len_c, len_l;
     std::vector<uint8_t> out_c, out_l;
-    std::vector<uint8_t> lst;
     // KC_JSON_LISTS: records [R_out, R) are the aligned round's (record src[i - R_out] of the call); emit splices them back
     int64_t R_out = 0;
     std::vector<int64_t> src;
@@ -899,84 +875,43 @@ void plan_twin(kc_debug_jsongpu *h, const char *h_text, const int64_t *h_off, in
     h->n = n;
     h->off.assign(h_off, h_off + R * n + 1);
     h->text.assign((const uint8_t *)h_text + h_off[0], (const uint8_t *)h_text + h_off[R * n]);
-    h->fcount.assign((size_t)R + 1, 0);
-    h->slot.assign((size_t)R + 1, 0);
-    h->status.assign((size_t)R, 0);
-    h->nest.assign((size_t)R, 0);
-    h->pend.assign((size_t)R, 0);
-    h->lst.assign((size_t)R, 0);
-    h->plist.assign((size_t)R + 1, -1);
-    h->vbase.assign((size_t)R, 0);
-    h->xbase.assign((size_t)R, 0);
-    h->len_c.assign((size_t)R + 1, 0);
-    h->len_l.assign((size_t)R + 1, 0);
-    h->mcount.assign((size_t)R + 1, 0);
-    h->scount.assign((size_t)R + 1, 0);
-    h->ccount.assign((size_t)R + 1, 0);
     Chunk &ch = h->ch;
     ch.text = h->text.data();
     ch.off = h->off.data();
     ch.R = (int32_t)R;
     ch.n = n;
-    ch.fcount = h->fcount.data();
-    ch.slot = h->slot.data();
-    ch.status = h->status.data();
-    ch.nest = h->nest.data();
-    ch.pend = h->pend.data();
-    ch.plist = h->plist.data();
-    ch.vbase = h->vbase.data();
-    ch.xbase = h->xbase.data();
     ch.counters = h->counters;
-    ch.mcount = h->mcount.data();
-    ch.scount = h->scount.data();
-    ch.ccount = h->ccount.data();
-    ch.len_c = h->len_c.data();
-    ch.len_l = h->len_l.data();
-    ch.xmedoid = (flags & KC_JSON_NUMERIC_MEDOID) != 0;
-    ch.key_union = (flags & KC_JSON_KEY_UNION) != 0;
-    ch.lst = h->lst.data();
-    ch.lists = lists;
-    ch.aligned0 = aligned0;
-    ch.unicode = (flags & KC_JSON_UNICODE) != 0;
-    for (int32_t r = 0; r < R; ++r) kc::js::count_record(ch, r);
-    for (int64_t r = 0; r < R; ++r) h->slot[(size_t)r + 1] = h->slot[(size_t)r] + h->fcount[(size_t)r];
-    const size_t T = h->slot[(size_t)R];
+    set_flags(ch, flags, lists, aligned0);
     auto host = [&](int k, auto *&ptr, size_t len, size_t, int fill, bool) -> int {
         using E = std::remove_reference_t<decltype(*ptr)>;
-        h->slot_mem[k].resize(len * sizeof(E), (uint8_t)fill);  // keeps what is there, fills the rest
-        ptr = reinterpret_cast<E *>(h->slot_mem[k].data());
+        if (h->arrays.size() <= (size_t)k) h->arrays.resize((size_t)k + 1);
+        h->arrays[(size_t)k].resize(len * sizeof(E), (uint8_t)fill);  // keeps what is there, fills the rest
+        ptr = reinterpret_cast<E *>(h->arrays[(size_t)k].data());
         return KC_OK;
     };
-    slot_arrays(host, ch, T, 0, true);
+    Units u{(size_t)R, h->text.size()};
+    chunk_arrays(host, ch, RECORDS, u, 0, true);
+    for (int32_t r = 0; r < R; ++r) kc::js::count_record(ch, r);
+    for (int64_t r = 0; r < R; ++r) ch.slot[r + 1] = ch.slot[r] + ch.fcount[r];
+    u.T = ch.slot[R];
+    chunk_arrays(host, ch, SLOTS, u, 0, true);
     const kc::js::HostTeam team{team_size(n)};
     for (int32_t r = 0; r < R; ++r) kc::js::plan_step(ch, r, team);
-    if (const int64_t P = (int64_t)h->counters[3]) {  // the union round, as run_chunk / union_round run it
-        h->ucand.assign((size_t)(P * n), 0);
-        h->ubase.assign((size_t)P, 0);
-        h->usize.assign((size_t)P, 0);
-        ch.ucand = h->ucand.data();
-        ch.ubase = h->ubase.data();
-        ch.usize = h->usize.data();
-        ch.uslot = (uint32_t)T;
+    if ((u.P = h->counters[3])) {  // the union round, as run_chunk / union_round run it
+        const int32_t P = (int32_t)u.P;
+        chunk_arrays(host, ch, UNION, u, 0, true);
+        ch.uslot = (uint32_t)u.T;
         for (int32_t p = 0; p < P; ++p) kc::js::union_count_step(ch, p, team);
-        const size_t S = std::max<size_t>(h->counters[4], 1);
-        h->utok.assign(S, Tok{});
-        h->unode.assign(S, kc::js::UNode{});
-        h->umap.assign(S, -1);
-        ch.utok = h->utok.data();
-        ch.unode = h->unode.data();
-        ch.umap = h->umap.data();
+        u.S = std::max<size_t>(h->counters[4], 1);
+        chunk_arrays(host, ch, SCRATCH, u, 0, true);
         for (int32_t p = 0; p < P; ++p) kc::js::union_build_step(ch, p, team);
-        slot_arrays(host, ch, T + (size_t)h->counters[5], T, true);
+        const size_t keep = u.T;
+        u.T += h->counters[5];
+        chunk_arrays(host, ch, SLOTS, u, keep, true);
         for (int32_t p = 0; p < P; ++p) kc::js::union_plan_step(ch, p, team);
     }
-    for (std::vector<uint32_t> *cnt : {&h->mcount, &h->scount, &h->ccount}) exclusive_scan(*cnt);
-    h->mchars.assign((size_t)h->ccount[(size_t)R] + 1, 0);
-    h->mstr_off.assign((size_t)h->scount[(size_t)R] + 1, 0);
-    h->mgrp_off.assign((size_t)h->mcount[(size_t)R] + 1, 0);
-    ch.mchars = h->mchars.data();
-    ch.mstr_off = h->mstr_off.data();
-    ch.mgrp_off = h->mgrp_off.data();
+    for (uint32_t *cnt : {ch.mcount, ch.scount, ch.ccount}) exclusive_scan(cnt, u.R + 1);
+    chunk_arrays(host, ch, CSR, u, 0, true);
     for (int32_t r = 0; r < R; ++r) kc::js::medoid_step(ch, r, team);
 }
 
@@ -997,7 +932,7 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     plan_twin(h, h_text, h_off, R, n, flags, lists ? 1 : 0, INT32_MAX);
     std::vector<int64_t> idx;
     for (int64_t r = 0; r < R && lists; ++r)
-        if (h->status[(size_t)r] == kc::js::D_LIST) idx.push_back(r);
+        if (h->ch.status[r] == kc::js::D_LIST) idx.push_back(r);
     if (idx.empty()) {
         *out = h;
         return KC_OK;
@@ -1024,7 +959,7 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
     plan_twin(h, text.data(), off.data(), R + M, n, flags, 1, (int32_t)R);
     h->R_out = R;
     h->src = dst;
-    for (int64_t r : declined) h->status[(size_t)r] = kc::js::D_ALIGN;
+    for (int64_t r : declined) h->ch.status[r] = kc::js::D_ALIGN;
     int32_t *vrec = h->ch.vrec;  // the aligned records' vote groups weigh with their call records' candidate sums
     for (uint64_t g = 0; g < h->counters[0]; ++g)
         if (vrec[g] >= R) vrec[g] = (int32_t)dst[(size_t)(vrec[g] - R)];
@@ -1036,9 +971,9 @@ int kc_debug_jsongpu_plan_flags(const char *h_text, const int64_t *h_off, int64_
 int kc_debug_jsongpu_medoid_inputs(const kc_debug_jsongpu *h, const uint8_t **chars, const int32_t **str_off, const int32_t **grp_off,
                                    int64_t *n_groups) {
     if (!h) return KC_EINVAL;
-    if (chars) *chars = h->mchars.data();
-    if (str_off) *str_off = h->mstr_off.data();
-    if (grp_off) *grp_off = h->mgrp_off.data();
+    if (chars) *chars = h->ch.mchars;
+    if (str_off) *str_off = h->ch.mstr_off;
+    if (grp_off) *grp_off = h->ch.mgrp_off;
     if (n_groups) *n_groups = (int64_t)h->counters[2];
     return KC_OK;
 }
@@ -1064,7 +999,7 @@ int kc_debug_jsongpu_inputs(const kc_debug_jsongpu *h, const int8_t **vote_cells
     if (n_vote_groups) *n_vote_groups = (int64_t)h->counters[0];
     if (num_cells) *num_cells = h->ch.xcells;
     if (n_num_groups) *n_num_groups = (int64_t)h->counters[1];
-    if (status) *status = h->status.data();
+    if (status) *status = h->ch.status;
     return KC_OK;
 }
 
@@ -1091,9 +1026,9 @@ int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_met
     const int64_t R = h->R;
     const kc::js::HostTeam team{team_size(h->n)};
     for (int32_t r = 0; r < R; ++r) kc::js::len_step(ch, r, team);
-    exclusive_scan(h->len_c);
-    exclusive_scan(h->len_l);
-    const int64_t ac = h->len_c[(size_t)R], al = h->len_l[(size_t)R];
+    exclusive_scan(ch.len_c, (size_t)R + 1);
+    exclusive_scan(ch.len_l, (size_t)R + 1);
+    const int64_t ac = ch.len_c[R], al = ch.len_l[R];
     h->out_c.assign((size_t)std::max<int64_t>(ac, 1), 0);
     h->out_l.assign((size_t)std::max<int64_t>(al, 1), 0);
     ch.out_c = h->out_c.data();
@@ -1105,9 +1040,9 @@ int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_met
         for (int64_t r = 0; r < Ro; ++r) from[(size_t)r] = r;
         for (int64_t i = 0; i < R - Ro; ++i) {
             from[(size_t)h->src[(size_t)i]] = Ro + i;
-            h->status[(size_t)h->src[(size_t)i]] = h->status[(size_t)(Ro + i)];
+            ch.status[h->src[(size_t)i]] = ch.status[Ro + i];
         }
-        auto splice = [&](const std::vector<int64_t> &o, const std::vector<uint8_t> &blob, std::vector<int64_t> &so, std::vector<uint8_t> &sb) {
+        auto splice = [&](const int64_t *o, const std::vector<uint8_t> &blob, std::vector<int64_t> &so, std::vector<uint8_t> &sb) {
             so.assign((size_t)Ro + 1, 0);
             sb.clear();
             for (int64_t r = 0; r < Ro; ++r) {
@@ -1117,8 +1052,8 @@ int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_met
             }
             sb.push_back(0);
         };
-        splice(h->len_c, h->out_c, h->spliced_c, h->spliced_out_c);
-        splice(h->len_l, h->out_l, h->spliced_l, h->spliced_out_l);
+        splice(ch.len_c, h->out_c, h->spliced_c, h->spliced_out_c);
+        splice(ch.len_l, h->out_l, h->spliced_l, h->spliced_out_l);
         if (content) *content = (const char *)h->spliced_out_c.data();
         if (content_off) *content_off = h->spliced_c.data();
         if (likelihoods) *likelihoods = (const char *)h->spliced_out_l.data();
@@ -1126,9 +1061,9 @@ int kc_debug_jsongpu_emit_weighted(kc_debug_jsongpu *h, const uint32_t *vote_met
         return KC_OK;
     }
     if (content) *content = (const char *)h->out_c.data();
-    if (content_off) *content_off = h->len_c.data();
+    if (content_off) *content_off = ch.len_c;
     if (likelihoods) *likelihoods = (const char *)h->out_l.data();
-    if (likelihoods_off) *likelihoods_off = h->len_l.data();
+    if (likelihoods_off) *likelihoods_off = ch.len_l;
     return KC_OK;
 }
 
