@@ -65,6 +65,49 @@ struct PlaneRow {  // [cell][thread] plane: pitch = threads*8 bytes, a multiple 
     }
 };
 
+// ---------------------------------------------------------------- row loader: cells 2q and 2q+1 arrive as one 16-byte load
+
+// the 2Q cells at p (one row, or several small rows) as Q 16-byte loads
+template <int Q>
+__device__ __forceinline__ void load_cells(const double *p, int4 (&c)[Q]) {
+#pragma unroll
+    for (int q = 0; q < Q; ++q) c[q] = ldg_nc_v4(reinterpret_cast<const int4 *>(p) + q);
+}
+
+// grid-stride over units u < n_units: the next unit is requested before body(u, cells) works on this one
+template <int Q, class Body>
+__device__ __forceinline__ void prefetch_units(const double *vals, int64_t u, int64_t n_units, int64_t stride, Body body) {
+    int4 cur[Q];
+    if (u < n_units) load_cells(vals + u * (2 * Q), cur);
+    for (; u < n_units; u += stride) {
+        int4 nxt[Q];
+        if (u + stride < n_units) load_cells(vals + (u + stride) * (2 * Q), nxt);
+        body(u, cur);
+#pragma unroll
+        for (int q = 0; q < Q; ++q) cur[q] = nxt[q];
+    }
+}
+
+__device__ __forceinline__ void put_pair(const PlaneRow row, int q, int4 c) {
+    sts_f64(row.addr(2 * q + 0), __hiloint2double(c.y, c.x));
+    sts_f64(row.addr(2 * q + 1), __hiloint2double(c.w, c.z));
+}
+
+// numeric_core's input: the high words in hi[], the cells in the plane
+template <int N>
+__device__ __forceinline__ void load_pair(int4 c, int q, uint32_t (&hi)[N], const PlaneRow row) {
+    hi[2 * q + 0] = (uint32_t)c.y;
+    hi[2 * q + 1] = (uint32_t)c.w;
+    put_pair(row, q, c);
+}
+
+// the high words of a row parked in the plane
+template <int N>
+__device__ __forceinline__ void plane_hi(const PlaneRow row, uint32_t (&hi)[N]) {
+#pragma unroll
+    for (int i = 0; i < N; ++i) hi[i] = lds_u32x2(row.addr(i)).y;
+}
+
 // ---------------------------------------------------------------- numpy reductions over sorted row memory
 
 // numpy DOUBLE_pairwise_sum (n <= 128) over f(0..n-1), then the +0.0 seed of add.reduce.
@@ -467,20 +510,7 @@ __device__ __forceinline__ void numeric_pair(uint2 a, uint2 b, double rel_eps, d
 __global__ void __launch_bounds__(256) numeric_pairs_kernel(const double *__restrict__ vals, int64_t n_units, double rel_eps, double abs_eps,
                                                             double *__restrict__ out_value, uint32_t *__restrict__ out_meta) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int4 cur[4];
-    if (u < n_units) {
-        const int4 *p = reinterpret_cast<const int4 *>(vals) + u * 4;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) cur[q] = ldg_nc_v4(p + q);
-    }
-    for (; u < n_units; u += stride) {
-        int4 nxt[4];
-        if (u + stride < n_units) {
-            const int4 *p = reinterpret_cast<const int4 *>(vals) + (u + stride) * 4;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) nxt[q] = ldg_nc_v4(p + q);
-        }
+    prefetch_units<4>(vals, (int64_t)blockIdx.x * blockDim.x + threadIdx.x, n_units, stride, [&](int64_t u, const int4 (&cur)[4]) {
         double v[4];
         uint32_t m[4];
 #pragma unroll
@@ -492,9 +522,7 @@ __global__ void __launch_bounds__(256) numeric_pairs_kernel(const double *__rest
         asm volatile("st.global.L1::no_allocate.v2.f64 [%0], {%1,%2};" ::"l"(ov + 2), "d"(v[2]), "d"(v[3]) : "memory");
         asm volatile("st.global.L1::no_allocate.v4.u32 [%0], {%1,%2,%3,%4};" ::"l"(out_meta + u * 4), "r"(m[0]), "r"(m[1]), "r"(m[2]), "r"(m[3])
                      : "memory");
-#pragma unroll
-        for (int q = 0; q < 4; ++q) cur[q] = nxt[q];
-    }
+    });
 }
 
 // ---------------------------------------------------------------- n = 4: sort four, read the cluster pattern off three bits
@@ -611,20 +639,7 @@ __device__ __forceinline__ void numeric_quad(const uint2 (&w)[4], double rel_eps
 __global__ void __launch_bounds__(256) numeric_quads_kernel(const double *__restrict__ vals, int64_t n_units, double rel_eps, double abs_eps,
                                                             double *__restrict__ out_value, uint32_t *__restrict__ out_meta) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    int4 cur[4];
-    if (u < n_units) {
-        const int4 *p = reinterpret_cast<const int4 *>(vals) + u * 4;
-#pragma unroll
-        for (int q = 0; q < 4; ++q) cur[q] = ldg_nc_v4(p + q);
-    }
-    for (; u < n_units; u += stride) {
-        int4 nxt[4];
-        if (u + stride < n_units) {
-            const int4 *p = reinterpret_cast<const int4 *>(vals) + (u + stride) * 4;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) nxt[q] = ldg_nc_v4(p + q);
-        }
+    prefetch_units<4>(vals, (int64_t)blockIdx.x * blockDim.x + threadIdx.x, n_units, stride, [&](int64_t u, const int4 (&cur)[4]) {
         double v[2];
         uint32_t m[2];
 #pragma unroll
@@ -636,9 +651,7 @@ __global__ void __launch_bounds__(256) numeric_quads_kernel(const double *__rest
         }
         asm volatile("st.global.L1::no_allocate.v2.f64 [%0], {%1,%2};" ::"l"(out_value + u * 2), "d"(v[0]), "d"(v[1]) : "memory");
         asm volatile("st.global.L1::no_allocate.v2.u32 [%0], {%1,%2};" ::"l"(out_meta + u * 2), "r"(m[0]), "r"(m[1]) : "memory");
-#pragma unroll
-        for (int q = 0; q < 4; ++q) cur[q] = nxt[q];
-    }
+    });
 }
 
 // (The same shape for n = 8 — a 19-comparator network on the doubles, seven closeness bits, numeric_tie for the rare ties — was
@@ -646,6 +659,12 @@ __global__ void __launch_bounds__(256) numeric_quads_kernel(const double *__rest
 // FP64 compares costs more than proving a majority on 32-bit words; removed.)
 
 // ---------------------------------------------------------------- direct front-end (any n <= NP)
+
+// dynamic shared memory of the direct kernels (numeric_direct_kernel, numeric_direct_fast_kernel): the [cell][thread] plane
+template <int NP, int T>
+constexpr size_t numeric_direct_smem() {
+    return (size_t)NP * T * 8;
+}
 
 template <int NP, int T, bool PREFETCH>
 __global__ void __launch_bounds__(T) numeric_direct_kernel(const double *__restrict__ vals, int64_t n_groups, int n,
@@ -656,62 +675,36 @@ __global__ void __launch_bounds__(T) numeric_direct_kernel(const double *__restr
     const double thr = abs_eps > rel_eps ? abs_eps : rel_eps;
     const int64_t stride = (int64_t)gridDim.x * T;
     int64_t g = (int64_t)blockIdx.x * T + threadIdx.x;
-    int4 cur[NP / 2 > 0 ? NP / 2 : 1];
-    if constexpr (PREFETCH) {  // requires n == NP
-        if (g < n_groups) {
-            const int4 *p4 = reinterpret_cast<const int4 *>(vals + g * NP);
-#pragma unroll
-            for (int q = 0; q < NP / 2; ++q) cur[q] = ldg_nc_v4(p4 + q);
-        }
-    }
+    int4 cur[NP / 2];
+    if (PREFETCH && g < n_groups) load_cells(vals + g * NP, cur);  // PREFETCH requires n == NP
     for (; g < n_groups; g += stride) {
+        const double *p = vals + g * n;
         uint32_t hi[NP];
+        int4 nxt[NP / 2];
+        if (PREFETCH || n == NP) {
+            if constexpr (PREFETCH) {
+                if (g + stride < n_groups) load_cells(vals + (g + stride) * NP, nxt);  // request the next row before working on this one
+            } else {
+                load_cells(p, cur);
+            }
+#pragma unroll
+            for (int q = 0; q < NP / 2; ++q) load_pair(cur[q], q, hi, row);
+        } else {
+#pragma unroll
+            for (int i = 0; i < NP; ++i) {
+                const double v = (i < n) ? __ldg(p + i) : __longlong_as_double((long long)KC_F64_ABSENT_BITS);
+                hi[i] = (uint32_t)__double2hiint(v);
+                sts_f64(row.addr(i), v);
+            }
+        }
+        double v;
+        uint32_t m;
+        numeric_core<NP, PlaneRow>(hi, row, rel_eps, abs_eps, thr, v, m);
+        store_out_f64(out_value + g, v, mc);
+        store_out_u32(out_meta + g, m, mc);
         if constexpr (PREFETCH) {
-            int4 nxt[NP / 2];
-            if (g + stride < n_groups) {  // request the next row before working on this one
-                const int4 *p4 = reinterpret_cast<const int4 *>(vals + (g + stride) * NP);
-#pragma unroll
-                for (int q = 0; q < NP / 2; ++q) nxt[q] = ldg_nc_v4(p4 + q);
-            }
-#pragma unroll
-            for (int q = 0; q < NP / 2; ++q) {
-                hi[2 * q + 0] = (uint32_t)cur[q].y;
-                hi[2 * q + 1] = (uint32_t)cur[q].w;
-                sts_f64(row.addr(2 * q + 0), __hiloint2double(cur[q].y, cur[q].x));
-                sts_f64(row.addr(2 * q + 1), __hiloint2double(cur[q].w, cur[q].z));
-            }
-            double v;
-            uint32_t m;
-            numeric_core<NP, PlaneRow>(hi, row, rel_eps, abs_eps, thr, v, m);
-            store_out_f64(out_value + g, v, mc);
-            store_out_u32(out_meta + g, m, mc);
 #pragma unroll
             for (int q = 0; q < NP / 2; ++q) cur[q] = nxt[q];
-        } else {
-            const double *p = vals + g * n;
-            if (n == NP) {
-                const int4 *p4 = reinterpret_cast<const int4 *>(p);
-#pragma unroll
-                for (int q = 0; q < NP / 2; ++q) {
-                    const int4 t = ldg_nc_v4(p4 + q);
-                    hi[2 * q + 0] = (uint32_t)t.y;
-                    hi[2 * q + 1] = (uint32_t)t.w;
-                    sts_f64(row.addr(2 * q + 0), __hiloint2double(t.y, t.x));
-                    sts_f64(row.addr(2 * q + 1), __hiloint2double(t.w, t.z));
-                }
-            } else {
-#pragma unroll
-                for (int i = 0; i < NP; ++i) {
-                    const double v = (i < n) ? __ldg(p + i) : __longlong_as_double((long long)KC_F64_ABSENT_BITS);
-                    hi[i] = (uint32_t)__double2hiint(v);
-                    sts_f64(row.addr(i), v);
-                }
-            }
-            double v;
-            uint32_t m;
-            numeric_core<NP, PlaneRow>(hi, row, rel_eps, abs_eps, thr, v, m);
-            store_out_f64(out_value + g, v, mc);
-            store_out_u32(out_meta + g, m, mc);
         }
     }
 }
@@ -723,6 +716,13 @@ __global__ void __launch_bounds__(T) numeric_direct_kernel(const double *__restr
 // conflict-free LDS.128 and copied to a [cell][thread] plane: the data-dependent accesses of the core would
 // bank-conflict on a row-per-thread layout, while in the plane the bank depends on the thread only.  The stage
 // is handed back to the TMA unit right after that copy.
+
+// dynamic shared memory of the TMA kernels (numeric_tma_kernel, numeric_tma_fast_kernel): the rings, then the plane
+template <int N, int WARPS, int STAGES>
+constexpr size_t numeric_tma_smem() {
+    return WarpTiles<N * 8, WARPS, STAGES>::RING_BYTES + numeric_direct_smem<N, WARPS * 32>();
+}
+
 // ---------------------------------------------------------------- K2 fast path: a strict majority of identical cells
 //
 // Candidates of one field mostly agree bit for bit.  If one value v fills a strict majority of the m finite cells, its
@@ -766,6 +766,16 @@ __device__ __forceinline__ void match_cell(uint32_t h, uint32_t l, uint32_t hv, 
 
 // Callers pass x = hi + 2^20 (kFastBias) for every cell and top = the largest raw high word (unsigned).
 constexpr uint32_t kFastBias = 0x00100000u;
+
+// the row loader's load_pair for numeric_fast_decide: cells 2q and 2q+1 into x[] and lo[], their high words into top
+template <int N>
+__device__ __forceinline__ void fast_pair(const int4 &c, int q, uint32_t (&x)[N], uint32_t (&lo)[N], uint32_t &top) {
+    lo[2 * q + 0] = (uint32_t)c.x;
+    x[2 * q + 0] = (uint32_t)c.y + kFastBias;
+    lo[2 * q + 1] = (uint32_t)c.z;
+    x[2 * q + 1] = (uint32_t)c.w + kFastBias;
+    top = max(top, max((uint32_t)c.y, (uint32_t)c.w));
+}
 
 struct FastDecision {
     double v;       // the majority value
@@ -954,111 +964,122 @@ __device__ __forceinline__ void numeric_fast_finish(const FastDecision &d, doubl
     meta = (d.word & ~15u) + ((nb + na) << 6);
 }
 
-// Register-prefetch front-end (n == NP, small rows) with the fast path: same deferral queue as the TMA variant below.
+// ---------------------------------------------------------------- the fast kernels' deferral queue
+//
+// Cells stay in registers for the fast path; a group it does not decide parks its cells in one of the warp's 32 plane rows
+// (slot s = the row of lane s) and its index in the warp's 64 `slot` entries.  When 32 wait, the warp runs numeric_core on
+// them with every lane busy: the general path costs its instructions only for the groups that need it.  Groups parked
+// past the 32nd keep only their index; when they move down, their cells are fetched again from `rows` (a few groups at
+// most).  Whole warps call put() together, once per step (so that the count stays warp-uniform), and finish() at the end.
+// A kernel passes its plane (the first 8-byte cell of thread 0), the warp's first thread, and the warp's row of slots.
+// The kernels call numeric_fast_decide themselves: called inside put(), it compiles the TMA kernels to other code.
+template <int N, int T, typename Idx>
+struct DeferQueue {
+    int count = 0;  // warp-uniform; the first member, since the member order shows in the fast kernels' register allocation
+    Idx *slot;
+    const double *rows;  // group g's cells at rows + g * N
+    double *out_value;
+    uint32_t *out_meta;
+    double rel_eps, abs_eps, thr;
+    PlaneRow row;  // this lane's
+    uint32_t warp_plane, lane;
+
+    __device__ __forceinline__ DeferQueue(Idx *slot_, uint32_t plane, uint32_t warp_thread0, uint32_t lane_, const double *rows_,
+                                          double rel_eps_, double abs_eps_, double *out_value_, uint32_t *out_meta_)
+        : slot(slot_), rows(rows_), out_value(out_value_), out_meta(out_meta_), rel_eps(rel_eps_), abs_eps(abs_eps_),
+          thr(abs_eps_ > rel_eps_ ? abs_eps_ : rel_eps_), row{plane + threadIdx.x * 8u, T * 8u}, warp_plane(plane + warp_thread0 * 8u),
+          lane(lane_) {}
+
+    // the first `n` parked groups through the general path, one per lane
+    __device__ __forceinline__ void drain(int n) {
+        if ((int)lane < n) {
+            const Idx g = slot[lane];
+            uint32_t hi[N];
+            plane_hi(row, hi);
+            double v;
+            uint32_t m;
+            numeric_core<N, PlaneRow>(hi, row, rel_eps, abs_eps, thr, v, m);
+            store_local_f64(out_value + g, v);
+            store_local_u32(out_meta + g, m);
+        }
+        __syncwarp();
+    }
+
+    // group g of this lane (g >= n_groups: none), cells as fast_pair loads them: stored if the fast path decided it, else parked
+    __device__ __forceinline__ void put(Idx g, Idx n_groups, const uint32_t (&x)[N], const uint32_t (&lo)[N], bool decided,
+                                        const FastDecision &fd) {
+        const bool defer = !decided && g < n_groups;
+        const uint32_t dm = __ballot_sync(0xFFFFFFFFu, defer);
+        if (defer) {  // park the cells in a free plane row; past the 32nd only the index is kept (re-read below)
+            const uint32_t s = (uint32_t)count + (uint32_t)__popc(dm & ((1u << lane) - 1u));
+            slot[s] = g;
+            if (s < 32u) {
+#pragma unroll
+                for (int i = 0; i < N; ++i)
+                    sts_f64(warp_plane + s * 8u + (uint32_t)i * (T * 8u), __hiloint2double((int)(x[i] - kFastBias), (int)lo[i]));
+            }
+        }
+        count += __popc(dm);
+        if (decided && g < n_groups) {
+            double v;
+            uint32_t m;
+            numeric_fast_finish<N>(fd, v, m);
+            store_local_f64(out_value + g, v);
+            store_local_u32(out_meta + g, m);
+        }
+        __syncwarp();
+        if (count >= 32) {  // nothing of this step is live in registers any more
+            drain(32);
+            count -= 32;
+            const Idx moved = ((int)lane < count) ? slot[32 + lane] : Idx(0);
+            __syncwarp();
+            if ((int)lane < count) {  // the overflow: fetch its cells again
+                slot[lane] = moved;
+                const int4 *p4 = reinterpret_cast<const int4 *>(rows + (size_t)moved * N);
+#pragma unroll
+                for (int q = 0; q < N / 2; ++q) put_pair(row, q, ldg_nc_v4(p4 + q));
+            }
+            __syncwarp();
+        }
+    }
+
+    __device__ __forceinline__ void finish() {
+        if (count > 0) drain(count);
+    }
+};
+
+// Register-prefetch front-end (n == NP, small rows) with the fast path.
 template <int NP, int T>
 __global__ void __launch_bounds__(T) numeric_direct_fast_kernel(const double *__restrict__ vals, int64_t n_groups, double rel_eps,
                                                                 double abs_eps, double *__restrict__ out_value,
                                                                 uint32_t *__restrict__ out_meta, const __grid_constant__ OutRoute /* local only: see the launcher */) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     __shared__ int64_t defer_q[T / 32][64];
-    const PlaneRow row{smem_u32(smem_raw) + threadIdx.x * 8u, T * 8u};
-    const double thr = abs_eps > rel_eps ? abs_eps : rel_eps;
-    const int lane = threadIdx.x & 31;
-    int64_t *my_q = defer_q[threadIdx.x >> 5];
-    int q_count = 0;  // warp-uniform
+    const uint32_t lane = threadIdx.x & 31;
+    DeferQueue<NP, T, int64_t> queue(defer_q[threadIdx.x >> 5], smem_u32(smem_raw), threadIdx.x & ~31u, lane, vals, rel_eps, abs_eps, out_value,
+                                     out_meta);
     const int64_t stride = (int64_t)gridDim.x * T;
     const int64_t g0 = (int64_t)blockIdx.x * T + threadIdx.x;
-
-    // deferred groups wait in the warp's 32 plane rows (slot s = the row of lane s), their indices in my_q
-    const uint32_t warp_plane = smem_u32(smem_raw) + (threadIdx.x & ~31u) * 8u;
-    auto drain = [&](int count) {
-        if (lane < count) {
-            const int64_t g = my_q[lane];
-            uint32_t hi[NP];
-#pragma unroll
-            for (int i = 0; i < NP; ++i) hi[i] = lds_u32x2(row.addr(i)).y;
-            double v;
-            uint32_t m;
-            numeric_core<NP, PlaneRow>(hi, row, rel_eps, abs_eps, thr, v, m);
-            store_local_f64(out_value + g, v);
-            store_local_u32(out_meta + g, m);
-        }
-        __syncwarp();
-    };
-
     int4 cur[NP / 2];
-    if (g0 < n_groups) {
-        const int4 *p4 = reinterpret_cast<const int4 *>(vals + g0 * NP);
-#pragma unroll
-        for (int q = 0; q < NP / 2; ++q) cur[q] = ldg_nc_v4(p4 + q);
-    }
+    if (g0 < n_groups) load_cells(vals + g0 * NP, cur);
     // whole warps iterate together (the tail lanes idle) so that the queue bookkeeping stays warp-uniform
     for (int64_t gw = g0 - lane; gw < n_groups; gw += stride) {
         const int64_t g = gw + lane;
         int4 nxt[NP / 2];
-        if (g + stride < n_groups) {  // request the next row before working on this one
-            const int4 *p4 = reinterpret_cast<const int4 *>(vals + (g + stride) * NP);
+        if (g + stride < n_groups) load_cells(vals + (g + stride) * NP, nxt);  // request the next row before working on this one
+        uint32_t x[NP], lo[NP], top = 0;
 #pragma unroll
-            for (int q = 0; q < NP / 2; ++q) nxt[q] = ldg_nc_v4(p4 + q);
-        }
-        uint32_t x[NP], lo[NP], top = 0;  // x = high word + kFastBias
-#pragma unroll
-        for (int q = 0; q < NP / 2; ++q) {
-            lo[2 * q + 0] = (uint32_t)cur[q].x;
-            x[2 * q + 0] = (uint32_t)cur[q].y + kFastBias;
-            lo[2 * q + 1] = (uint32_t)cur[q].z;
-            x[2 * q + 1] = (uint32_t)cur[q].w + kFastBias;
-            top = max(top, max((uint32_t)cur[q].y, (uint32_t)cur[q].w));
-        }
+        for (int q = 0; q < NP / 2; ++q) fast_pair(cur[q], q, x, lo, top);
         FastDecision fd;
-        const bool decided = numeric_fast_decide<NP>(x, lo, top, rel_eps, thr, fd);
-        const bool defer = !decided && g < n_groups;
-        const uint32_t dm = __ballot_sync(0xFFFFFFFFu, defer);
-        if (defer) {  // park the cells in a free plane row; past the 32nd only the index is kept (re-read below)
-            const uint32_t slot = (uint32_t)q_count + (uint32_t)__popc(dm & ((1u << lane) - 1u));
-            my_q[slot] = g;
-            if (slot < 32u) {
-#pragma unroll
-                for (int i = 0; i < NP; ++i)
-                    sts_f64(warp_plane + slot * 8u + (uint32_t)i * (T * 8u), __hiloint2double((int)(x[i] - kFastBias), (int)lo[i]));
-            }
-        }
-        q_count += __popc(dm);
-        if (decided && g < n_groups) {
-            double v;
-            uint32_t m;
-            numeric_fast_finish<NP>(fd, v, m);
-            store_local_f64(out_value + g, v);
-            store_local_u32(out_meta + g, m);
-        }
-        __syncwarp();
-        if (q_count >= 32) {
-            drain(32);
-            q_count -= 32;
-            const int64_t moved = (lane < q_count) ? my_q[32 + lane] : 0;
-            __syncwarp();
-            if (lane < q_count) {
-                my_q[lane] = moved;
-                const int4 *p4 = reinterpret_cast<const int4 *>(vals + moved * NP);
-#pragma unroll
-                for (int q = 0; q < NP / 2; ++q) {
-                    const int4 v4 = ldg_nc_v4(p4 + q);
-                    sts_f64(row.addr(2 * q + 0), __hiloint2double(v4.y, v4.x));
-                    sts_f64(row.addr(2 * q + 1), __hiloint2double(v4.w, v4.z));
-                }
-            }
-            __syncwarp();
-        }
+        const bool decided = numeric_fast_decide<NP>(x, lo, top, rel_eps, queue.thr, fd);
+        queue.put(g, n_groups, x, lo, decided, fd);
 #pragma unroll
         for (int q = 0; q < NP / 2; ++q) cur[q] = nxt[q];
     }
-    if (q_count > 0) drain(q_count);
+    queue.finish();
 }
 
-// The TMA pipeline of numeric_tma_kernel with the fast path in front: cells stay in registers; a group the fast path
-// does not decide parks its cells in one of the warp's 32 plane rows, and when those are (nearly) full the warp runs
-// numeric_core on them with every lane busy — the general path costs its instructions only for the groups that need it,
-// and nothing is read twice.
+// The TMA pipeline of numeric_tma_kernel with the fast path in front; nothing is read twice but the queue's overflow.
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
 __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_fast_kernel(const __grid_constant__ CUtensorMap tmap,
                                                                       const double *__restrict__ in, uint32_t n_groups,
@@ -1068,89 +1089,25 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_fast_kernel(
     constexpr int T = WARPS * 32;
     WarpTiles<N * 8, WARPS, STAGES> tiles(&tmap, n_groups);
     __shared__ uint32_t defer_q[WARPS][64];
-
-    const uint32_t lane = tiles.lane;
-    uint32_t *my_q = defer_q[tiles.warp];
-    int q_count = 0;  // warp-uniform
-    const PlaneRow row{tiles.end() + threadIdx.x * 8u, T * 8u};
-    const double thr = abs_eps > rel_eps ? abs_eps : rel_eps;
+    DeferQueue<N, T, uint32_t> queue(defer_q[tiles.warp], tiles.end(), tiles.warp * 32u, tiles.lane, in, rel_eps, abs_eps, out_value, out_meta);
     tiles.start(L2Policy::evict_normal);
-
-    // Deferred groups wait in the warp's 32 plane rows (slot s = the row of lane s) with their group index in my_q;
-    // drain: the first `count` of them through the general path, one per lane.
-    const uint32_t warp_plane = tiles.end() + tiles.warp * 32u * 8u;
-    auto drain = [&](int count) {
-        if ((int)lane < count) {
-            const uint32_t g = my_q[lane];
-            uint32_t hi[N];
-#pragma unroll
-            for (int i = 0; i < N; ++i) hi[i] = lds_u32x2(row.addr(i)).y;
-            double v;
-            uint32_t m;
-            numeric_core<N, PlaneRow>(hi, row, rel_eps, abs_eps, thr, v, m);
-            store_local_f64(out_value + g, v);
-            store_local_u32(out_meta + g, m);
-        }
-        __syncwarp();
-    };
 
     for (; tiles.t < tiles.n_tiles; tiles.next()) {
         const uint32_t tile = tiles.wait();
-        uint32_t x[N], lo[N];  // x = high word + kFastBias
-        uint32_t touch = 0, top = 0;
+        uint32_t x[N], lo[N], touch = 0, top = 0;
 #pragma unroll
         for (int q = 0; q < N / 2; ++q) {
-            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
-            lo[2 * q + 0] = (uint32_t)v4.x;
-            x[2 * q + 0] = (uint32_t)v4.y + kFastBias;
-            lo[2 * q + 1] = (uint32_t)v4.z;
-            x[2 * q + 1] = (uint32_t)v4.w + kFastBias;
-            top = max(top, max((uint32_t)v4.y, (uint32_t)v4.w));
-            touch |= (uint32_t)v4.w;  // one word of every LDS.128 is enough to depend on all of them
+            const int4 c = lds_v4(tile + tiles.at(q * 16));
+            fast_pair(c, q, x, lo, top);
+            touch |= (uint32_t)c.w;  // one word of every LDS.128 is enough to depend on all of them
         }
         tiles.release(touch);
-        const uint32_t g = tiles.t * 32 + lane;
+        const uint32_t g = tiles.t * 32 + tiles.lane;
         FastDecision fd;
-        const bool decided = numeric_fast_decide<N>(x, lo, top, rel_eps, thr, fd);
-        const bool defer = !decided && g < n_groups;
-        const uint32_t dm = __ballot_sync(0xFFFFFFFFu, defer);
-        if (defer) {  // park the cells in a free plane row; past the 32nd only the index is kept (re-read below)
-            const uint32_t slot = (uint32_t)q_count + (uint32_t)__popc(dm & ((1u << lane) - 1u));
-            my_q[slot] = g;
-            if (slot < 32u) {
-#pragma unroll
-                for (int i = 0; i < N; ++i)
-                    sts_f64(warp_plane + slot * 8u + (uint32_t)i * (T * 8u), __hiloint2double((int)(x[i] - kFastBias), (int)lo[i]));
-            }
-        }
-        q_count += __popc(dm);
-        if (decided && g < n_groups) {
-            double v;
-            uint32_t m;
-            numeric_fast_finish<N>(fd, v, m);
-            store_local_f64(out_value + g, v);
-            store_local_u32(out_meta + g, m);
-        }
-        __syncwarp();
-        if (q_count >= 32) {  // nothing of this tile is live in registers any more
-            drain(32);
-            q_count -= 32;
-            const uint32_t moved = ((int)lane < q_count) ? my_q[32 + lane] : 0u;
-            __syncwarp();
-            if ((int)lane < q_count) {  // the overflow (a few groups at most): fetch their cells again
-                my_q[lane] = moved;
-                const int4 *p4 = reinterpret_cast<const int4 *>(in + (size_t)moved * N);
-#pragma unroll
-                for (int q = 0; q < N / 2; ++q) {
-                    const int4 v4 = ldg_nc_v4(p4 + q);
-                    sts_f64(row.addr(2 * q + 0), __hiloint2double(v4.y, v4.x));
-                    sts_f64(row.addr(2 * q + 1), __hiloint2double(v4.w, v4.z));
-                }
-            }
-            __syncwarp();
-        }
+        const bool decided = numeric_fast_decide<N>(x, lo, top, rel_eps, queue.thr, fd);
+        queue.put(g, n_groups, x, lo, decided, fd);
     }
-    if (q_count > 0) drain(q_count);
+    queue.finish();
 }
 
 template <int N, int WARPS, int STAGES, int MIN_CTAS>
@@ -1170,12 +1127,9 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) numeric_tma_kernel(const
         uint32_t touch = 0;
 #pragma unroll
         for (int q = 0; q < N / 2; ++q) {
-            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
-            hi[2 * q + 0] = (uint32_t)v4.y;
-            hi[2 * q + 1] = (uint32_t)v4.w;
-            sts_f64(row.addr(2 * q + 0), __hiloint2double(v4.y, v4.x));
-            sts_f64(row.addr(2 * q + 1), __hiloint2double(v4.w, v4.z));
-            touch |= (uint32_t)v4.w;  // one word of every LDS.128 is enough to depend on all of them
+            const int4 c = lds_v4(tile + tiles.at(q * 16));
+            load_pair(c, q, hi, row);
+            touch |= (uint32_t)c.w;  // one word of every LDS.128 is enough to depend on all of them
         }
         tiles.release(touch);
         const uint32_t g = tiles.t * 32 + tiles.lane;

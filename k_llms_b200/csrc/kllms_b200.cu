@@ -249,44 +249,45 @@ int launch_vote_i8(const int8_t *codes, int64_t G, int n, const int32_t *none_co
 
 // ---------------------------------------------------------------- K2 launchers
 
-template <int N, int WARPS, int STAGES, int MIN_CTAS>
+// FAST: the fast path in front (kc::numeric_tma_fast_kernel), local results only; it re-reads its queue's overflow from `vals`
+template <int N, int WARPS, int STAGES, int MIN_CTAS, bool FAST = false>
 int launch_numeric_tma(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
                        cudaStream_t st, kc::OutRoute mc) {
-    auto kernel = kc::numeric_tma_kernel<N, WARPS, STAGES, MIN_CTAS>;
-    const size_t smem = kc::WarpTiles<N * 8, WARPS, STAGES>::RING_BYTES + (size_t)WARPS * 32 * N * 8;  // + the [cell][thread] plane
-    return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
-        kernel<<<grid, WARPS * 32, smem, st>>>(map, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
-    });
+    constexpr size_t smem = kc::numeric_tma_smem<N, WARPS, STAGES>();
+    auto go = [&](auto kernel) {
+        return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
+            if constexpr (FAST)
+                kernel<<<grid, WARPS * 32, smem, st>>>(map, vals + g0 * N, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0);
+            else
+                kernel<<<grid, WARPS * 32, smem, st>>>(map, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0, mc);
+        });
+    };
+    if constexpr (FAST) return go(kc::numeric_tma_fast_kernel<N, WARPS, STAGES, MIN_CTAS>);
+    else return go(kc::numeric_tma_kernel<N, WARPS, STAGES, MIN_CTAS>);
 }
 
-// fast path in front (kc::numeric_fast), general path for the groups it leaves open
-template <int N, int WARPS, int STAGES, int MIN_CTAS>
-int launch_numeric_tma_fast(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
-                            cudaStream_t st) {
-    auto kernel = kc::numeric_tma_fast_kernel<N, WARPS, STAGES, MIN_CTAS>;
-    const size_t smem = kc::WarpTiles<N * 8, WARPS, STAGES>::RING_BYTES + (size_t)WARPS * 32 * N * 8;  // + the [cell][thread] plane
-    return launch_tma_slabs(kernel, WARPS, smem, vals, G, N * 8, 1, [&](int grid, const CUtensorMap &map, int64_t g0, int64_t gs) {
-        kernel<<<grid, WARPS * 32, smem, st>>>(map, vals + g0 * N, (uint32_t)gs, rel_eps, abs_eps, value + g0, meta + g0);
-    });
-}
-
-// PREFETCH (n == NP, NP in [4, 16]): the next row is requested before this one is worked on
-template <int NP, int T>
+// FAST: the fast path in front (kc::numeric_direct_fast_kernel; n == NP, local results only).  Otherwise PREFETCH (the next
+// row requested before this one is worked on) when n == NP and NP is 4 or 8, the sizes whose n == NP reaches this launcher.
+template <int NP, int T, bool FAST = false>
 int launch_numeric_direct(const double *vals, int64_t G, int n, double rel_eps, double abs_eps, double *value,
                           uint32_t *meta, cudaStream_t st, kc::OutRoute mc) {
-    const size_t smem = (size_t)NP * T * 8;
-    auto launch = [&](auto kernel) -> int {
+    constexpr size_t smem = kc::numeric_direct_smem<NP, T>();
+    auto launch = [&](auto kernel, auto... n_arg) -> int {  // n_arg: n, except for the fast kernel
         int grid = 0;
         int rc = persistent_grid(kernel, T, smem, (G + T - 1) / T, grid);
         if (rc) return rc;
-        kernel<<<grid, T, smem, st>>>(vals, G, n, rel_eps, abs_eps, value, meta, mc);
+        kernel<<<grid, T, smem, st>>>(vals, G, n_arg..., rel_eps, abs_eps, value, meta, mc);
         KC_CUDA_I(cudaGetLastError());
         return KC_OK;
     };
-    if constexpr (NP >= 4 && NP <= 16) {
-        if (n == NP) return launch(kc::numeric_direct_kernel<NP, T, true>);
+    if constexpr (FAST) {
+        return launch(kc::numeric_direct_fast_kernel<NP, T>);
+    } else {
+        if constexpr (NP == 4 || NP == 8) {
+            if (n == NP) return launch(kc::numeric_direct_kernel<NP, T, true>, n);
+        }
+        return launch(kc::numeric_direct_kernel<NP, T, false>, n);
     }
-    return launch(kc::numeric_direct_kernel<NP, T, false>);
 }
 
 // the n = 2 and n = 4 case analyses (kc::numeric_pairs_kernel, kc::numeric_quads_kernel): GPT groups per thread; the last
@@ -306,21 +307,6 @@ int launch_numeric_units(Kernel kernel, const double *vals, int64_t G, double re
     if (done == G) return KC_OK;
     return launch_numeric_direct<NP, 128>(vals + done * NP, G - done, NP, rel_eps, abs_eps, value + done, meta + done, st, mc);
 }
-
-template <int NP>
-int launch_numeric_direct_fast(const double *vals, int64_t G, double rel_eps, double abs_eps, double *value, uint32_t *meta,
-                               cudaStream_t st, kc::OutRoute mc) {
-    constexpr int T = 128;
-    auto kernel = kc::numeric_direct_fast_kernel<NP, T>;
-    const size_t smem = (size_t)T * NP * 8;
-    int grid = 0;
-    int rc = persistent_grid(kernel, T, smem, (G + T - 1) / T, grid);
-    if (rc) return rc;
-    kernel<<<grid, T, smem, st>>>(vals, G, rel_eps, abs_eps, value, meta, mc);
-    KC_CUDA_I(cudaGetLastError());
-    return KC_OK;
-}
-
 
 // Never launched (n = 4 and 8 take other K2 kernels).  The K2 kernels share __noinline__ helpers with these two
 // instantiations, and without them compile to different SASS: numeric_tma_fast_kernel<16, 4, 1, 6> spills 12 bytes and
@@ -604,9 +590,9 @@ static int numeric_f64_routed(const double *d_vals, int64_t n_groups, int32_t n,
         switch (n) {
             case 2: return launch_numeric_units<2, 4>(kc::numeric_pairs_kernel, d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
             case 4: return launch_numeric_units<4, 2>(kc::numeric_quads_kernel, d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 8: return launch_numeric_direct_fast<8>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
-            case 16: return launch_numeric_tma_fast<16, 4, 1, 6>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st);
-            case 32: return launch_numeric_tma_fast<32, 4, 1, 4>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st);
+            case 8: return launch_numeric_direct<8, 128, true>(d_vals, n_groups, 8, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 16: return launch_numeric_tma<16, 4, 1, 6, true>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
+            case 32: return launch_numeric_tma<32, 4, 1, 4, true>(d_vals, n_groups, rel_eps, abs_eps, d_value, d_meta, st, mc);
             default: break;
         }
     }

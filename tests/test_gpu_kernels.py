@@ -132,7 +132,7 @@ def test_numeric_other_eps():
         assert ok.all()
 
 
-@pytest.mark.parametrize("n", [16, 32])
+@pytest.mark.parametrize("n", [8, 16, 32])
 def test_numeric_fast_path_edges(n):
     """K2's majority shortcut (kc::numeric_fast) against the oracle where it has to give up or sit on a boundary:
     neighbours right at the tolerance, cells sharing v's high word, signed zeros, -inf / negative NaN / odd NaN payloads,

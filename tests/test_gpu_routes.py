@@ -457,7 +457,7 @@ COVERAGE = (
     # K2 local: n = 2, 4 (+ their one-group tails), 8, 16, 32 fast kernels
     + ["numeric_pairs_kernel", "numeric_quads_kernel", "numeric_direct_fast_kernel<8,128>", "numeric_tma_fast_kernel<16,4,1,6>",
        "numeric_tma_fast_kernel<32,4,1,4>"]
-    # K2 general kernels: n = 16, 32 non-local, n = 64 both; direct kernels for the other n (PREFETCH where n == NP in [4, 16])
+    # K2 general kernels: n = 16, 32 non-local, n = 64 both; direct kernels for the other n (PREFETCH where n == NP in {4, 8})
     + ["numeric_tma_kernel<16,4,1,7>", "numeric_tma_kernel<32,4,1,4>", "numeric_tma_kernel<64,2,1,3>",
        "numeric_direct_kernel<2,128,false>", "numeric_direct_kernel<4,128,false>", "numeric_direct_kernel<4,128,true>",
        "numeric_direct_kernel<8,128,false>", "numeric_direct_kernel<8,128,true>", "numeric_direct_kernel<16,128,false>",
