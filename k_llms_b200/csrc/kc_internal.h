@@ -1,4 +1,5 @@
-// kc_internal.h — helpers shared by the translation units of libkllms_b200.so (not part of the C ABI).
+// kc_internal.h — helpers shared by the translation units of libkllms_b200.so (not part of the C ABI), among them the one
+// owner of the library's device and page-locked host allocations (at the end).
 //
 // It also holds the one copy of each small CPython rule that the kernels and the host code must apply bit for bit
 // (kc_json.cpp is host C++ and cannot include the .cuh headers, so these live here, __host__ __device__):
@@ -16,6 +17,9 @@
 #include <stddef.h>
 #include <stdint.h>
 #include <string.h>
+
+#include <initializer_list>
+#include <utility>
 
 #include "../../include/kllms_b200.h"
 
@@ -154,3 +158,112 @@ extern "C" __attribute__((visibility("hidden"))) int kc_alignsim(const KcAsNode 
         cudaError_t e_ = (call);                                                                                      \
         if (e_ != cudaSuccess) return kc_fail(KC_ECUDA, "%s: %s (%s:%d)", #call, cudaGetErrorString(e_), __FILE__, __LINE__); \
     } while (0)
+
+// ---- device and page-locked host memory of the library (host code only).  Every cudaMalloc, cudaFree, cudaHostAlloc and
+// cudaFreeHost of libkllms_b200.so is in the four functions below; a failed allocation clears CUDA's last error and reports
+// KC_ENOMEM.  Owners of these allocations that live in pools are never destroyed: no CUDA call may run from a static
+// destructor, after the CUDA runtime may have been torn down.
+namespace kc {
+
+inline int device_alloc(void **p, size_t bytes, const char *who) {
+    if (cudaMalloc(p, bytes) == cudaSuccess) return KC_OK;
+    cudaGetLastError();
+    *p = nullptr;
+    return kc_fail(KC_ENOMEM, "%s: cudaMalloc(%zu) failed", who, bytes);
+}
+inline void device_free(void *p) {
+    if (p) cudaFree(p);
+}
+inline int pinned_alloc(void **p, size_t bytes, const char *who) {
+    if (cudaHostAlloc(p, bytes, cudaHostAllocDefault) == cudaSuccess) return KC_OK;
+    cudaGetLastError();
+    *p = nullptr;
+    return kc_fail(KC_ENOMEM, "%s: cudaHostAlloc(%zu) failed", who, bytes);
+}
+inline void pinned_free(void *p) {
+    if (p) cudaFreeHost(p);
+}
+
+enum class Mem { Device, Pinned };
+
+// A grow-only buffer of device or page-locked host memory.  It reallocates only when a request exceeds its capacity, and
+// then with an eighth more plus 256 bytes, so that sizes that creep up from call to call do not reallocate every call.
+template <Mem M>
+struct GrowBuf {
+    void *p = nullptr;
+    size_t cap = 0;
+    GrowBuf() = default;
+    GrowBuf(GrowBuf &&o) noexcept : p(o.p), cap(o.cap) {
+        o.p = nullptr;
+        o.cap = 0;
+    }
+    ~GrowBuf() { release(); }
+    void release() {
+        M == Mem::Device ? device_free(p) : pinned_free(p);
+        p = nullptr;
+        cap = 0;
+    }
+    // at least `need` bytes; the contents are not kept
+    int reserve(size_t need) {
+        if (p && need <= cap) return KC_OK;
+        release();
+        const size_t bytes = need + need / 8 + 256;
+        if (const int rc = M == Mem::Device ? device_alloc(&p, bytes, "device buffer") : pinned_alloc(&p, bytes, "pinned buffer")) return rc;
+        cap = bytes;
+        return KC_OK;
+    }
+    // reserve() that keeps the first `keep` bytes (device memory only): they are copied on stream s, and s is synchronised
+    // before the old allocation is freed.  The old allocation is freed on every path.
+    int grow(size_t need, size_t keep, cudaStream_t s) {
+        static_assert(M == Mem::Device, "grow() copies device memory");
+        if (!keep || (p && need <= cap)) return reserve(need);
+        GrowBuf old = std::move(*this);
+        if (const int rc = reserve(need)) return rc;
+        if (old.p) KC_CUDA_I(cudaMemcpyAsync(p, old.p, keep < old.cap ? keep : old.cap, cudaMemcpyDeviceToDevice, s));
+        KC_CUDA_I(cudaStreamSynchronize(s));
+        return KC_OK;
+    }
+    template <typename T>
+    T *as() const { return static_cast<T *>(p); }
+};
+
+// One synchronous call that uploads its inputs, launches and downloads its results: one device allocation cut into parts
+// that each start 256-byte aligned, one non-blocking stream, and the call's first error in rc (where the caller also stores
+// the code of a launcher it calls).  finish() waits for the stream and returns rc; the destructor destroys the stream and
+// frees the allocation.
+struct Staged {
+    const char *who;
+    void *base = nullptr;
+    cudaStream_t stream = nullptr;
+    int rc = KC_OK;
+    explicit Staged(const char *who_) : who(who_) {}
+    Staged(const Staged &) = delete;
+    void operator=(const Staged &) = delete;
+    ~Staged() {
+        if (stream) cudaStreamDestroy(stream);
+        device_free(base);
+    }
+    // parts[i] = the part of sizes[i] bytes; then the stream
+    int alloc(std::initializer_list<size_t> sizes, uint8_t **parts) {
+        auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
+        size_t end = 0;
+        for (size_t b : sizes) end = up(end) + b;
+        if (const int e = device_alloc(&base, end, who)) return e;
+        end = 0;
+        for (size_t b : sizes) {
+            *parts++ = static_cast<uint8_t *>(base) + up(end);
+            end = up(end) + b;
+        }
+        check(cudaStreamCreateWithFlags(&stream, cudaStreamNonBlocking), "stream");
+        return rc;
+    }
+    void check(cudaError_t e, const char *what) {
+        if (e != cudaSuccess && rc == KC_OK) rc = kc_fail(KC_ECUDA, "%s: %s: %s", who, what, cudaGetErrorString(e));
+    }
+    int finish() {
+        check(cudaStreamSynchronize(stream), "sync");
+        return rc;
+    }
+};
+
+}  // namespace kc

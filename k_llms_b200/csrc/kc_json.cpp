@@ -1100,20 +1100,11 @@ int kc_consolidate_json(const char *const *texts, const int64_t *lens, int64_t n
     const int64_t gv = batch.gv, gx = batch.gx, gm = batch.gm;
     std::vector<int32_t> m_idx((size_t)gm);
     std::vector<double> m_avg((size_t)gm);
-    // page-locked staging buffers are expensive to create: keep them (grow-only) across calls
+    // page-locked staging buffers are expensive to create: keep them (grow-only) across calls, never destroyed
     static std::mutex pool_mu;
-    static struct { void *p = nullptr; size_t cap = 0; } pool[6];
+    static kc::GrowBuf<kc::Mem::Pinned> *const pool = new kc::GrowBuf<kc::Mem::Pinned>[6];
     std::lock_guard<std::mutex> pool_lock(pool_mu);  // also serialises callers (one staging pool per process)
-    auto pinned = [&](int slot, size_t bytes) -> void * {
-        if (bytes == 0) return nullptr;
-        if (pool[slot].cap < bytes) {
-            kc_host_free(pool[slot].p);
-            pool[slot].cap = bytes + bytes / 4;
-            pool[slot].p = kc_host_alloc(pool[slot].cap);
-            if (!pool[slot].p) pool[slot].cap = 0;
-        }
-        return pool[slot].p;
-    };
+    auto pinned = [&](int slot, size_t bytes) { return bytes && pool[slot].reserve(bytes) == KC_OK ? pool[slot].p : nullptr; };
     int8_t *h_codes = (int8_t *)pinned(0, (size_t)gv * n);
     double *h_vals = (double *)pinned(1, (size_t)gx * n * 8);
     int32_t *h_win = (int32_t *)pinned(2, (size_t)gv * 4);

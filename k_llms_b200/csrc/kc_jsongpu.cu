@@ -35,63 +35,6 @@ using kc::js::Tok;
         if (const int rc_ = (call)) return rc_; \
     } while (0)
 
-struct DBuf {  // grow-only device buffer
-    void *p = nullptr;
-    size_t cap = 0;
-    int reserve(size_t need) {
-        if (p && need <= cap) return KC_OK;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        need += need / 8 + 256;
-        if (cudaMalloc(&p, need) != cudaSuccess) {
-            cudaGetLastError();
-            return kc_fail(KC_ENOMEM, "kc_consolidate_json_packed: cudaMalloc(%zu) failed", need);
-        }
-        cap = need;
-        return KC_OK;
-    }
-    // reserve() that keeps the first `keep` bytes (copied on stream s; the stream is synchronised before the old buffer is freed)
-    int grow(size_t need, size_t keep, cudaStream_t s) {
-        if (!keep) return reserve(need);
-        if (p && need <= cap) return KC_OK;
-        void *old = p;
-        const size_t old_cap = cap;
-        p = nullptr;
-        cap = 0;
-        if (const int rc = reserve(need)) {
-            cudaFree(old);
-            return rc;
-        }
-        if (old) KC_CUDA_I(cudaMemcpyAsync(p, old, std::min(keep, old_cap), cudaMemcpyDeviceToDevice, s));
-        KC_CUDA_I(cudaStreamSynchronize(s));
-        if (old) cudaFree(old);
-        return KC_OK;
-    }
-    template <typename T>
-    T *as() const { return static_cast<T *>(p); }
-};
-
-struct PBuf {  // grow-only pinned host buffer
-    void *p = nullptr;
-    size_t cap = 0;
-    int reserve(size_t need) {
-        if (p && need <= cap) return KC_OK;
-        if (p) cudaFreeHost(p);
-        p = nullptr;
-        cap = 0;
-        need += need / 8 + 256;
-        if (cudaHostAlloc(&p, need, cudaHostAllocDefault) != cudaSuccess) {
-            cudaGetLastError();
-            return kc_fail(KC_ENOMEM, "kc_consolidate_json_packed: cudaHostAlloc(%zu) failed", need);
-        }
-        cap = need;
-        return KC_OK;
-    }
-    template <typename T>
-    T *as() const { return static_cast<T *>(p); }
-};
-
 // Every array of a chunk that the device worker and the host twin both size, each named once: the Stage that sizes it (OFF:
 // the chunk does not use it), its length (a count of one of the Units, times a number per unit, plus a constant), the byte
 // its new elements are filled with, and whether the device fills them too (the twin fills every array; the device only what
@@ -159,10 +102,10 @@ struct Worker {
     int device = -1;
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[7] = {};
-    DBuf text, off, counters, win, vmeta, xvalue, xmeta, out_c, out_l, scan_tmp, midx, mavg, seq, vweight;
-    std::vector<DBuf> arrays;  // chunk_arrays
-    PBuf h_small;  // totals and counters (pinned so the small D2H copies are asynchronous)
-    PBuf h_scan;   // the scanned record offsets and the statuses of a chunk
+    kc::GrowBuf<kc::Mem::Device> text, off, counters, win, vmeta, xvalue, xmeta, out_c, out_l, scan_tmp, midx, mavg, seq, vweight;
+    std::vector<kc::GrowBuf<kc::Mem::Device>> arrays;  // chunk_arrays
+    kc::GrowBuf<kc::Mem::Pinned> h_small;  // totals and counters (pinned so the small D2H copies are asynchronous)
+    kc::GrowBuf<kc::Mem::Pinned> h_scan;   // the scanned record offsets and the statuses of a chunk
     bool busy = false;
     int init(int dev) {
         if (device == dev) return KC_OK;
@@ -212,15 +155,9 @@ PinnedBlob acquire_blob(size_t need) {
             return b;
         }
     }
-    PinnedBlob b;
     void *p = nullptr;
-    if (cudaHostAlloc(&p, need, cudaHostAllocDefault) != cudaSuccess) {
-        cudaGetLastError();
-        return b;
-    }
-    b.p = (char *)p;
-    b.cap = need;
-    return b;
+    if (kc::pinned_alloc(&p, need, "kc_consolidate_json_packed")) return PinnedBlob{};
+    return PinnedBlob{(char *)p, need};
 }
 void release_blob(PinnedBlob b) {
     if (!b.p) return;
@@ -237,10 +174,10 @@ void release_blob(PinnedBlob b) {
         for (int i = 0; i < (int)g_blob_pool.size(); ++i)
             if (g_blob_pool[i].cap > ((size_t)4 << 20) && (smallest < 0 || g_blob_pool[i].cap < g_blob_pool[smallest].cap)) smallest = i;
         if (smallest < 0 || g_blob_pool[smallest].cap >= b.cap) {
-            cudaFreeHost(b.p);
+            kc::pinned_free(b.p);
             return;
         }
-        cudaFreeHost(g_blob_pool[smallest].p);
+        kc::pinned_free(g_blob_pool[smallest].p);
         g_blob_pool.erase(g_blob_pool.begin() + smallest);
     }
     g_blob_pool.push_back(b);
@@ -1119,26 +1056,6 @@ __global__ void float_reprs_kernel(const double *__restrict__ xs, int64_t count,
     }
 }
 
-// One device allocation cut into `n` buffers of bytes[i] (each 256-byte aligned), freed on scope exit.
-struct DebugDev {
-    uint8_t *base = nullptr;
-    ~DebugDev() {
-        if (base) cudaFree(base);
-    }
-    int alloc(const size_t *bytes, uint8_t **ptrs, int n, const char *who) {
-        size_t total = 0;
-        for (int i = 0; i < n; ++i) total += (bytes[i] + 255) & ~size_t(255);
-        if (cudaMalloc(&base, total ? total : 256) != cudaSuccess) {
-            cudaGetLastError();
-            base = nullptr;
-            return kc_fail(KC_ENOMEM, "%s: cudaMalloc(%zu) failed", who, total);
-        }
-        size_t o = 0;
-        for (int i = 0; i < n; o += (bytes[i] + 255) & ~size_t(255), ++i) ptrs[i] = base + o;
-        return KC_OK;
-    }
-};
-
 constexpr int kDebugBlock = 256, kDebugGrid = 264;  // a grid stride of 67,584 threads: large batches loop
 
 }  // namespace
@@ -1151,33 +1068,33 @@ int kc_debug_parse_doubles_device(const char *text, const int64_t *off, int64_t 
     if (count == 0) return KC_OK;
     KC_CUDA_I(cudaSetDevice(device));
     const size_t n_text = (size_t)off[count];
-    const size_t bytes[4] = {n_text, ((size_t)count + 1) * 8, (size_t)count * 8, (size_t)count};
-    uint8_t *d[4];
-    DebugDev mem;
-    if (const int rc = mem.alloc(bytes, d, 4, "kc_debug_parse_doubles_device")) return rc;
-    if (n_text) KC_CUDA_I(cudaMemcpy(d[0], text, n_text, cudaMemcpyHostToDevice));
-    KC_CUDA_I(cudaMemcpy(d[1], off, bytes[1], cudaMemcpyHostToDevice));
-    parse_doubles_kernel<<<kDebugGrid, kDebugBlock>>>(d[0], reinterpret_cast<const int64_t *>(d[1]), count, reinterpret_cast<double *>(d[2]), d[3]);
+    kc::Staged st("kc_debug_parse_doubles_device");
+    uint8_t *d[4];  // text, offsets, values, flags
+    R_(st.alloc({n_text, ((size_t)count + 1) * 8, (size_t)count * 8, (size_t)count}, d));
+    if (n_text) KC_CUDA_I(cudaMemcpyAsync(d[0], text, n_text, cudaMemcpyHostToDevice, st.stream));
+    KC_CUDA_I(cudaMemcpyAsync(d[1], off, ((size_t)count + 1) * 8, cudaMemcpyHostToDevice, st.stream));
+    parse_doubles_kernel<<<kDebugGrid, kDebugBlock, 0, st.stream>>>(d[0], reinterpret_cast<const int64_t *>(d[1]), count,
+                                                                   reinterpret_cast<double *>(d[2]), d[3]);
     KC_CUDA_I(cudaGetLastError());
-    KC_CUDA_I(cudaMemcpy(out, d[2], bytes[2], cudaMemcpyDeviceToHost));
-    KC_CUDA_I(cudaMemcpy(ok, d[3], bytes[3], cudaMemcpyDeviceToHost));
-    return KC_OK;
+    KC_CUDA_I(cudaMemcpyAsync(out, d[2], (size_t)count * 8, cudaMemcpyDeviceToHost, st.stream));
+    KC_CUDA_I(cudaMemcpyAsync(ok, d[3], (size_t)count, cudaMemcpyDeviceToHost, st.stream));
+    return st.finish();
 }
 
 int kc_debug_float_reprs_device(const double *xs, int64_t count, char *out /* [count][32] */, int32_t *lens, int device) {
     if (!xs || !out || !lens || count < 0) return KC_EINVAL;
     if (count == 0) return KC_OK;
     KC_CUDA_I(cudaSetDevice(device));
-    const size_t bytes[3] = {(size_t)count * 8, (size_t)count * 32, (size_t)count * 4};
-    uint8_t *d[3];
-    DebugDev mem;
-    if (const int rc = mem.alloc(bytes, d, 3, "kc_debug_float_reprs_device")) return rc;
-    KC_CUDA_I(cudaMemcpy(d[0], xs, bytes[0], cudaMemcpyHostToDevice));
-    float_reprs_kernel<<<kDebugGrid, kDebugBlock>>>(reinterpret_cast<const double *>(d[0]), count, d[1], reinterpret_cast<int32_t *>(d[2]));
+    kc::Staged st("kc_debug_float_reprs_device");
+    uint8_t *d[3];  // values, texts, lengths
+    R_(st.alloc({(size_t)count * 8, (size_t)count * 32, (size_t)count * 4}, d));
+    KC_CUDA_I(cudaMemcpyAsync(d[0], xs, (size_t)count * 8, cudaMemcpyHostToDevice, st.stream));
+    float_reprs_kernel<<<kDebugGrid, kDebugBlock, 0, st.stream>>>(reinterpret_cast<const double *>(d[0]), count, d[1],
+                                                                 reinterpret_cast<int32_t *>(d[2]));
     KC_CUDA_I(cudaGetLastError());
-    KC_CUDA_I(cudaMemcpy(out, d[1], bytes[1], cudaMemcpyDeviceToHost));
-    KC_CUDA_I(cudaMemcpy(lens, d[2], bytes[2], cudaMemcpyDeviceToHost));
-    return KC_OK;
+    KC_CUDA_I(cudaMemcpyAsync(out, d[1], (size_t)count * 32, cudaMemcpyDeviceToHost, st.stream));
+    KC_CUDA_I(cudaMemcpyAsync(lens, d[2], (size_t)count * 4, cudaMemcpyDeviceToHost, st.stream));
+    return st.finish();
 }
 
 }  // extern "C"

@@ -165,6 +165,24 @@ int launch_tma_slabs(Kernel kernel, int warps, size_t smem, const void *rows, in
     return KC_OK;
 }
 
+// K3b's weight rows: `wrow` floats per record in stream-ordered scratch on st, written by pre(grid, rows) (a weight_rows
+// kernel, 8 records per 256-thread CTA) and read by vote(rows); the scratch is freed on st on every path.  Without records
+// there are no rows: vote(nullptr).
+template <typename Pre, typename Vote>
+int with_weight_rows(int64_t n_records, int wrow, cudaStream_t st, const char *who, Pre &&pre, Vote &&vote) {
+    if (n_records == 0) return vote(nullptr);
+    int grid = 0;
+    int rc = stride_grid((n_records + 7) / 8, grid);
+    if (rc) return rc;
+    float *rows = nullptr;
+    KC_CUDA_I(cudaMallocAsync(reinterpret_cast<void **>(&rows), (size_t)n_records * wrow * 4, st));
+    pre(grid, rows);
+    rc = cudaGetLastError() == cudaSuccess ? KC_OK : kc_fail(KC_ECUDA, "%s: weight_rows_kernel launch failed", who);
+    if (!rc) rc = vote(rows);
+    cudaFreeAsync(rows, st);
+    return rc;
+}
+
 // ---------------------------------------------------------------- K1 launchers
 
 kc::FieldMap make_field_map(const int32_t *none_code, int n_fields) {
@@ -317,32 +335,14 @@ int launch_numeric_units(Kernel kernel, const double *vals, int64_t G, double re
 // ---------------------------------------------------------------- host-buffer context
 
 namespace {
-struct DevBuf {
-    void *p = nullptr;
-    size_t cap = 0;
-    int reserve(size_t need) {
-        if (p && need <= cap) return KC_OK;
-        if (p) cudaFree(p);
-        p = nullptr;
-        cap = 0;
-        if (cudaMalloc(&p, need) != cudaSuccess) {
-            cudaGetLastError();
-            return kc_fail(KC_ENOMEM, "cudaMalloc(%zu) failed", need);
-        }
-        cap = need;
-        return KC_OK;
-    }
-    template <typename T>
-    T *as() const { return static_cast<T *>(p); }
-};
 struct HostCtx {
     static constexpr int kStreams = 3;
     int device = -1;
     cudaStream_t streams[kStreams] = {};
-    DevBuf codes[kStreams], vals[kStreams], win[kStreams], vmeta[kStreams], value[kStreams], nmeta[kStreams], none;
+    kc::GrowBuf<kc::Mem::Device> codes[kStreams], vals[kStreams], win[kStreams], vmeta[kStreams], value[kStreams], nmeta[kStreams], none;
 };
 std::mutex g_host_mu;
-HostCtx g_host[16];
+HostCtx *const g_host = new HostCtx[16];  // never destroyed, like every pooled owner of device memory (kc_internal.h)
 
 }  // namespace
 
@@ -670,17 +670,13 @@ int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int
         };
         if (n == 32 && rec_cap <= 8) {  // weights by a pre-pass, fetched per tile by a bulk copy (n_fields >= 6; n = 32 only)
             constexpr int N = 32, WARPS = 8, STAGES = 2, WROW = kc::kWRowBulk<N>;
-            int pre_grid = 0;
-            int rc = stride_grid((n_records + 7) / 8, pre_grid);
-            if (rc) return rc;
-            float *d_rows = nullptr;
-            KC_CUDA_I(cudaMallocAsync(reinterpret_cast<void **>(&d_rows), (size_t)n_records * WROW * 4, st));
-            kc::weight_rows_kernel<N><<<pre_grid, 256, 0, st>>>(d_seq_logprob, n_records, d_rows);
-            rc = cudaGetLastError() == cudaSuccess ? KC_OK : kc_fail(KC_ECUDA, "kc_weighted_vote_i32: weight_rows_kernel launch failed");
-            const size_t smem = kc::weighted_vote_rows_smem<N, WARPS, STAGES>(rec_cap);
-            if (!rc) rc = launch_tma(kc::weighted_vote_rows_kernel<N, WARPS, STAGES, 3>, N, WARPS, smem, d_rows, WROW);
-            cudaFreeAsync(d_rows, st);
-            return rc;
+            return with_weight_rows(
+                n_records, WROW, st, "kc_weighted_vote_i32",
+                [&](int grid, float *rows) { kc::weight_rows_kernel<N><<<grid, 256, 0, st>>>(d_seq_logprob, n_records, rows); },
+                [&](float *rows) {
+                    const size_t smem = kc::weighted_vote_rows_smem<N, WARPS, STAGES>(rec_cap);
+                    return launch_tma(kc::weighted_vote_rows_kernel<N, WARPS, STAGES, 3>, N, WARPS, smem, rows, WROW);
+                });
         }
         // n = 32 with 3 CTAs / SM (80 registers) and the logprobs requested a tile ahead; n = 64 (2 x the registers per row)
         // without the prefetch (not re-timed on H100)
@@ -729,29 +725,19 @@ int kc_weighted_vote_groups_i8(const int8_t *d_codes, int64_t n_groups, int32_t 
     // the buckets and row loads of kc_vote_i8: n a power of two from 4 on reads whole rows, any other n the next power of two
     // with the cells beyond n absent
     return with_pow2<4>(n, [&](auto np) -> int {
-        constexpr int NP = decltype(np)::value, WROW = kc::kWRowBulk<NP>;
-        float *d_rows = nullptr;
-        if (n_records > 0) {
-            int pre_grid = 0;
-            int rc = stride_grid((n_records + 7) / 8, pre_grid);
-            if (rc) return rc;
-            KC_CUDA_I(cudaMallocAsync(reinterpret_cast<void **>(&d_rows), (size_t)n_records * WROW * 4, st));
-            kc::weight_rows_n_kernel<NP><<<pre_grid, 256, 0, st>>>(d_seq_logprob, n_records, n, d_rows);
-            if (cudaGetLastError() != cudaSuccess) {
-                cudaFreeAsync(d_rows, st);
-                return kc_fail(KC_ECUDA, "kc_weighted_vote_groups_i8: weight_rows_kernel launch failed");
-            }
-        }
-        const int threads = 128;
-        int grid = 0;
-        int rc = stride_grid((n_groups + threads - 1) / threads, grid);
-        if (!rc) {
-            auto kernel = n == NP ? kc::weighted_vote_groups_kernel<NP, true> : kc::weighted_vote_groups_kernel<NP, false>;
-            kernel<<<grid, threads, 0, st>>>(d_codes, n_groups, n, d_group_record, n_records, d_rows, d_win_code, d_meta, d_weight);
-            if (cudaGetLastError() != cudaSuccess) rc = kc_fail(KC_ECUDA, "kc_weighted_vote_groups_i8: launch failed");
-        }
-        if (d_rows) cudaFreeAsync(d_rows, st);
-        return rc;
+        constexpr int NP = decltype(np)::value;
+        return with_weight_rows(
+            n_records, kc::kWRowBulk<NP>, st, "kc_weighted_vote_groups_i8",
+            [&](int grid, float *rows) { kc::weight_rows_n_kernel<NP><<<grid, 256, 0, st>>>(d_seq_logprob, n_records, n, rows); },
+            [&](float *rows) {
+                const int threads = 128;
+                int grid = 0;
+                int rc = stride_grid((n_groups + threads - 1) / threads, grid);
+                if (rc) return rc;
+                auto kernel = n == NP ? kc::weighted_vote_groups_kernel<NP, true> : kc::weighted_vote_groups_kernel<NP, false>;
+                kernel<<<grid, threads, 0, st>>>(d_codes, n_groups, n, d_group_record, n_records, rows, d_win_code, d_meta, d_weight);
+                return cudaGetLastError() == cudaSuccess ? KC_OK : kc_fail(KC_ECUDA, "kc_weighted_vote_groups_i8: launch failed");
+            });
     });
 }
 
@@ -806,32 +792,19 @@ int kc_medoid_str_host(const uint8_t *h_chars, int64_t n_chars, const int32_t *h
     KC_CUDA_I(cudaSetDevice(device));
     const int64_t n_str = h_grp_off[n_groups];
     if (n_str < 0 || h_str_off[n_str] != n_chars) return kc_fail(KC_EINVAL, "kc_medoid_str_host: offsets do not add up to n_chars");
-    const size_t b_chars = ((size_t)n_chars + 255) & ~size_t(255), b_str = (((size_t)n_str + 1) * 4 + 255) & ~size_t(255),
-                 b_grp = (((size_t)n_groups + 1) * 4 + 255) & ~size_t(255), b_idx = ((size_t)n_groups * 4 + 255) & ~size_t(255),
-                 b_avg = (size_t)n_groups * 8;
-    uint8_t *d = nullptr;
-    KC_CUDA_I(cudaMalloc(&d, b_chars + b_str + b_grp + b_idx + b_avg + 256));
-    uint8_t *d_chars = d, *d_str = d + b_chars + 256, *d_grp = d_str + b_str, *d_idx = d_grp + b_grp, *d_avg = d_idx + b_idx;
-    int rc = KC_OK;
-    cudaStream_t st = nullptr;
-    auto guard = [&](cudaError_t e, const char *what) {
-        if (e != cudaSuccess && rc == KC_OK) rc = kc_fail(KC_ECUDA, "kc_medoid_str_host: %s: %s", what, cudaGetErrorString(e));
-    };
-    guard(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking), "stream");
-    if (n_chars) guard(cudaMemcpyAsync(d_chars, h_chars, (size_t)n_chars, cudaMemcpyHostToDevice, st), "H2D chars");
-    guard(cudaMemcpyAsync(d_str, h_str_off, ((size_t)n_str + 1) * 4, cudaMemcpyHostToDevice, st), "H2D str_off");
-    guard(cudaMemcpyAsync(d_grp, h_grp_off, ((size_t)n_groups + 1) * 4, cudaMemcpyHostToDevice, st), "H2D grp_off");
-    if (rc == KC_OK)
-        rc = kc_medoid_str(d_chars, reinterpret_cast<int32_t *>(d_str), reinterpret_cast<int32_t *>(d_grp), n_groups, max_group,
-                           reinterpret_cast<int32_t *>(d_idx), reinterpret_cast<double *>(d_avg), st);
-    guard(cudaMemcpyAsync(h_best_idx, d_idx, (size_t)n_groups * 4, cudaMemcpyDeviceToHost, st), "D2H idx");
-    guard(cudaMemcpyAsync(h_best_avg, d_avg, (size_t)n_groups * 8, cudaMemcpyDeviceToHost, st), "D2H avg");
-    if (st) {
-        guard(cudaStreamSynchronize(st), "sync");
-        cudaStreamDestroy(st);
-    }
-    cudaFree(d);
-    return rc;
+    kc::Staged st("kc_medoid_str_host");
+    uint8_t *d[5];  // chars, str_off, grp_off, best_idx, best_avg
+    if (const int rc = st.alloc({(size_t)n_chars + 256, ((size_t)n_str + 1) * 4, ((size_t)n_groups + 1) * 4, (size_t)n_groups * 4, (size_t)n_groups * 8}, d))
+        return rc;
+    if (n_chars) st.check(cudaMemcpyAsync(d[0], h_chars, (size_t)n_chars, cudaMemcpyHostToDevice, st.stream), "H2D chars");
+    st.check(cudaMemcpyAsync(d[1], h_str_off, ((size_t)n_str + 1) * 4, cudaMemcpyHostToDevice, st.stream), "H2D str_off");
+    st.check(cudaMemcpyAsync(d[2], h_grp_off, ((size_t)n_groups + 1) * 4, cudaMemcpyHostToDevice, st.stream), "H2D grp_off");
+    if (st.rc == KC_OK)
+        st.rc = kc_medoid_str(d[0], reinterpret_cast<int32_t *>(d[1]), reinterpret_cast<int32_t *>(d[2]), n_groups, max_group,
+                              reinterpret_cast<int32_t *>(d[3]), reinterpret_cast<double *>(d[4]), st.stream);
+    st.check(cudaMemcpyAsync(h_best_idx, d[3], (size_t)n_groups * 4, cudaMemcpyDeviceToHost, st.stream), "D2H idx");
+    st.check(cudaMemcpyAsync(h_best_avg, d[4], (size_t)n_groups * 8, cudaMemcpyDeviceToHost, st.stream), "D2H avg");
+    return st.finish();
 }
 
 // Element similarities of the list-alignment pre-pass (kc_alignsim.cuh): H2D of the value table, one launch, D2H of the
@@ -852,56 +825,37 @@ int kc_alignsim(const KcAsNode *nodes, int64_t n_nodes, const KcAsVal *vals, int
         return KC_OK;
     }
     KC_CUDA_I(cudaSetDevice(device));
-    auto up = [](size_t b) { return (b + 255) & ~size_t(255); };
-    const size_t b_nodes = up((size_t)n_nodes * sizeof(KcAsNode)), b_vals = up((size_t)n_vals * sizeof(KcAsVal)), b_chars = up((size_t)n_chars),
-                 b_out = (size_t)n_out * 8;
-    uint8_t *d = nullptr;
-    KC_CUDA_I(cudaMalloc(&d, 256 + b_nodes + b_vals + b_chars + b_out));
-    unsigned long long *d_pairs = reinterpret_cast<unsigned long long *>(d);
-    uint8_t *d_nodes = d + 256, *d_vals = d_nodes + b_nodes, *d_chars = d_vals + b_vals, *d_out = d_chars + b_chars;
-    int rc = KC_OK;
-    cudaStream_t st = nullptr;
-    auto guard = [&](cudaError_t e, const char *what) {
-        if (e != cudaSuccess && rc == KC_OK) rc = kc_fail(KC_ECUDA, "kc_alignsim: %s: %s", what, cudaGetErrorString(e));
-    };
-    guard(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking), "stream");
-    guard(cudaMemsetAsync(d_pairs, 0, 8, st), "memset");
-    guard(cudaMemcpyAsync(d_nodes, nodes, (size_t)n_nodes * sizeof(KcAsNode), cudaMemcpyHostToDevice, st), "H2D nodes");
-    if (n_vals) guard(cudaMemcpyAsync(d_vals, vals, (size_t)n_vals * sizeof(KcAsVal), cudaMemcpyHostToDevice, st), "H2D values");
-    if (n_chars) guard(cudaMemcpyAsync(d_chars, chars, (size_t)n_chars, cudaMemcpyHostToDevice, st), "H2D chars");
+    kc::Staged st("kc_alignsim");
+    uint8_t *d[5];  // decided pairs, nodes, values, chars, matrices
+    if (const int rc = st.alloc({8, (size_t)n_nodes * sizeof(KcAsNode), (size_t)n_vals * sizeof(KcAsVal), (size_t)n_chars, (size_t)n_out * 8}, d))
+        return rc;
+    st.check(cudaMemsetAsync(d[0], 0, 8, st.stream), "memset");
+    st.check(cudaMemcpyAsync(d[1], nodes, (size_t)n_nodes * sizeof(KcAsNode), cudaMemcpyHostToDevice, st.stream), "H2D nodes");
+    if (n_vals) st.check(cudaMemcpyAsync(d[2], vals, (size_t)n_vals * sizeof(KcAsVal), cudaMemcpyHostToDevice, st.stream), "H2D values");
+    if (n_chars) st.check(cudaMemcpyAsync(d[3], chars, (size_t)n_chars, cudaMemcpyHostToDevice, st.stream), "H2D chars");
     constexpr int WARPS = 4;
     auto kernel = kc::alignsim_kernel<WARPS>;
     int grid = 0;
-    if (rc == KC_OK) rc = persistent_grid(kernel, WARPS * 32, 0, (n_nodes + WARPS - 1) / WARPS, grid);
-    if (rc == KC_OK) {
-        kernel<<<grid, WARPS * 32, 0, st>>>(reinterpret_cast<const KcAsNode *>(d_nodes), n_nodes, reinterpret_cast<const KcAsVal *>(d_vals),
-                                            d_chars, reinterpret_cast<double *>(d_out), d_pairs);
-        guard(cudaGetLastError(), "launch");
+    if (st.rc == KC_OK) st.rc = persistent_grid(kernel, WARPS * 32, 0, (n_nodes + WARPS - 1) / WARPS, grid);
+    if (st.rc == KC_OK) {
+        kernel<<<grid, WARPS * 32, 0, st.stream>>>(reinterpret_cast<const KcAsNode *>(d[1]), n_nodes, reinterpret_cast<const KcAsVal *>(d[2]),
+                                                   d[3], reinterpret_cast<double *>(d[4]), reinterpret_cast<unsigned long long *>(d[0]));
+        st.check(cudaGetLastError(), "launch");
     }
     unsigned long long decided = 0;
-    if (n_out) guard(cudaMemcpyAsync(h_out, d_out, b_out, cudaMemcpyDeviceToHost, st), "D2H matrices");
-    guard(cudaMemcpyAsync(&decided, d_pairs, 8, cudaMemcpyDeviceToHost, st), "D2H pairs");
-    if (st) {
-        guard(cudaStreamSynchronize(st), "sync");
-        cudaStreamDestroy(st);
-    }
-    cudaFree(d);
+    if (n_out) st.check(cudaMemcpyAsync(h_out, d[4], (size_t)n_out * 8, cudaMemcpyDeviceToHost, st.stream), "D2H matrices");
+    st.check(cudaMemcpyAsync(&decided, d[0], 8, cudaMemcpyDeviceToHost, st.stream), "D2H pairs");
+    const int rc = st.finish();
     if (pairs) *pairs = (int64_t)decided;
     return rc;
 }
 
 void *kc_host_alloc(uint64_t bytes) {
     void *p = nullptr;
-    if (cudaHostAlloc(&p, bytes ? bytes : 1, cudaHostAllocDefault) != cudaSuccess) {
-        cudaGetLastError();
-        return nullptr;
-    }
-    return p;
+    return kc::pinned_alloc(&p, bytes ? bytes : 1, "kc_host_alloc") ? nullptr : p;
 }
 
-void kc_host_free(void *p) {
-    if (p) cudaFreeHost(p);
-}
+void kc_host_free(void *p) { kc::pinned_free(p); }
 
 // ---------------------------------------------------------------- end-to-end with host buffers
 
