@@ -85,6 +85,13 @@ __device__ __forceinline__ void bulk_load_1d(uint32_t smem_dst, const void *src,
                  : "memory");
 }
 
+// 16 bytes from a shared-space address
+__device__ __forceinline__ int4 lds_v4(uint32_t addr) {
+    int4 r;
+    asm volatile("ld.shared.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
+    return r;
+}
+
 // ---------------------------------------------------------------- the warp-private tile pipeline of the TMA front-ends
 
 template <int ROW_BYTES>
@@ -179,6 +186,18 @@ struct WarpTiles {
 
     // swizzled offset of byte `byte` of this lane's row inside a tile
     __device__ __forceinline__ uint32_t at(uint32_t byte) const { return Swizzle<ROW_BYTES>::apply(lane * ROW_BYTES + byte); }
+
+    // this lane's row of 4-byte cells from the tile at `tile`, 16 bytes per load
+    __device__ __forceinline__ void read_row(uint32_t tile, int32_t (&raw)[ROW_BYTES / 4]) const {
+#pragma unroll
+        for (int q = 0; q < ROW_BYTES / 16; ++q) {
+            const int4 v4 = lds_v4(tile + at(q * 16));
+            raw[4 * q + 0] = v4.x;
+            raw[4 * q + 1] = v4.y;
+            raw[4 * q + 2] = v4.z;
+            raw[4 * q + 3] = v4.w;
+        }
+    }
 
     // Hands the current stage back: lane 0 requests the tile STAGES ahead into it.  Every row must be in registers first.
     // `dep` depends on every load the lane made from the tile, a warp instruction issues only when its operands are ready
@@ -312,12 +331,6 @@ __device__ __forceinline__ void store_out_f64(void *p, double v, const OutRoute 
         asm volatile("st.global.L1::no_allocate.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
         if (r.mode >= 2u) store_peers_f64(p, v, r);
     }
-}
-
-__device__ __forceinline__ int4 lds_v4(uint32_t addr) {
-    int4 r;
-    asm volatile("ld.shared.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
-    return r;
 }
 
 }  // namespace kc

@@ -490,6 +490,57 @@ __device__ __forceinline__ uint32_t wv_record_of(uint32_t x, const FieldMap &fm,
     return fm.n_fields == 1u ? x : (uint32_t)__umul64hi((uint64_t)x, inv_fields);
 }
 
+// One tile of the K3b TMA kernels, from the wait for the tile to the stores: wts = the warp's weight rows for this tile (row
+// pitch WROW, the index of the record's heaviest candidate at w[N]), g0 = the tile's first group, r0 = its record.  `extra`
+// goes to release(): what the re-arm copies next to the tile it requests.  `f` is the lane's first-pass state, declared by
+// the kernel: declared here, nvvm promotes it to registers while it optimises this function on its own, before inlining, and
+// both kernels compile to other SASS with more stack (ptxas -v: weighted_vote_rows_kernel 24/24 -> 36/36 bytes of spills,
+// weighted_vote_tma_kernel<32,...> 64 -> 72 bytes of stack).
+template <int N, int WROW, int WARPS, int STAGES, class Extra>
+__device__ __forceinline__ void wv_tma_tile(const WarpTiles<N * 4, WARPS, STAGES> &tiles, const float *wts, uint32_t g0, uint32_t r0,
+                                            uint32_t n_groups, const FieldMap &fm, bool has_nc, int32_t *win, uint32_t *meta,
+                                            float *weight, const Extra &extra, WvFirst<N> &f) {
+    const uint32_t lane = tiles.lane;
+    const uint32_t tile = tiles.wait();
+    int32_t raw[N];
+    tiles.read_row(tile, raw);
+    const uint32_t g = g0 + lane;
+    const uint32_t fpos = (g0 - r0 * fm.n_fields) + lane;  // offset inside the tile's first record: < n_fields + 32
+    const uint32_t rec_local = g < n_groups ? fm.div_small(fpos) : 0u;
+    const float *wrow = wts + rec_local * WROW;
+    // this group's cell of its record's heaviest candidate: read from the tile while the stage is still ours
+    const int imax = __float_as_int(wrow[N]);
+    int32_t graw = KC_CODE_NONE - 1;
+    if (imax < N) {
+        asm volatile("ld.shared.s32 %0, [%1];" : "=r"(graw) : "r"(tile + tiles.at((uint32_t)imax * 4u)));
+    }
+    // the release's shuffle also means that every lane has left the previous tile, whose weight slot `extra` may refill
+    const int32_t lo = min(row_min<N>(raw), graw);
+    tiles.release((uint32_t)lo, extra);
+    bool undecided = false;
+    int32_t o_code = KC_CODE_NONE;
+    uint32_t o_meta = 0;
+    float o_weight = 0.0f;
+    if (g < n_groups) {
+        const uint32_t field = fpos - rec_local * fm.n_fields;
+        const int32_t nc = has_nc ? __ldg(fm.none_code + field) : KC_CODE_NONE;
+        wv_first_pass<N>(raw, lo, nc, wrow, graw, f);
+        undecided = !f.decided;
+        if (f.decided) {
+            o_code = f.guess;
+            o_meta = pack_meta(ffs_mask(f.eq_g) - 1, popc_m(f.eq_g), f.voters, f.present, KC_FLAG_HAS_VALUE);
+            o_weight = __fdiv_rn(f.cw_g, f.total);
+        }
+    }
+    for (uint32_t todo = __ballot_sync(0xFFFFFFFFu, undecided); todo; todo &= todo - 1)
+        wv_warp_walk<N>(lane, (uint32_t)__ffs((int)todo) - 1u, f, wts, rec_local, WROW, o_code, o_meta, o_weight);
+    if (g < n_groups) {
+        win[g] = o_code;
+        meta[g] = o_meta;
+        weight[g] = o_weight;
+    }
+}
+
 // K3b with K1's TMA front-end (n in {32, 64} cells per group = 128 / 256 byte rows; WarpTiles, kc_common.cuh) instead of one
 // 128-byte row per thread straight from global memory (latency-bound at 0.39 of the HBM peak: a warp's 32 rows are 32 separate
 // lines per load instruction).  The weights of the tile's records (32 groups span 31 / n_fields + 2 records at most) are computed
@@ -559,51 +610,8 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_tma_kernel
             if (lane == 0) w[N] = __int_as_float(imax);
         }
         __syncwarp();
-        const uint32_t tile = tiles.wait();
-        int32_t raw[N];
-#pragma unroll
-        for (int q = 0; q < N / 4; ++q) {
-            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
-            raw[4 * q + 0] = v4.x;
-            raw[4 * q + 1] = v4.y;
-            raw[4 * q + 2] = v4.z;
-            raw[4 * q + 3] = v4.w;
-        }
-        const uint32_t g = g0 + lane;
-        const uint32_t fpos = (g0 - r0 * fm.n_fields) + lane;  // offset inside the tile's first record: < n_fields + 32
-        const uint32_t rec_local = g < n_groups ? fm.div_small(fpos) : 0u;
-        const float *wrow = wts + rec_local * WROW;
-        // this group's cell of its record's heaviest candidate: read from the tile while the stage is still ours
-        const int imax = __float_as_int(wrow[N]);
-        int32_t graw = KC_CODE_NONE - 1;
-        if (imax < N) {
-            asm volatile("ld.shared.s32 %0, [%1];" : "=r"(graw) : "r"(tile + tiles.at((uint32_t)imax * 4u)));
-        }
-        const int32_t lo = min(row_min<N>(raw), graw);
-        tiles.release((uint32_t)lo);
         WvFirst<N> f;
-        bool undecided = false;
-        int32_t o_code = KC_CODE_NONE;
-        uint32_t o_meta = 0;
-        float o_weight = 0.0f;
-        if (g < n_groups) {
-            const uint32_t field = fpos - rec_local * fm.n_fields;
-            const int32_t nc = has_nc ? __ldg(fm.none_code + field) : KC_CODE_NONE;
-            wv_first_pass<N>(raw, lo, nc, wrow, graw, f);
-            undecided = !f.decided;
-            if (f.decided) {
-                o_code = f.guess;
-                o_meta = pack_meta(ffs_mask(f.eq_g) - 1, popc_m(f.eq_g), f.voters, f.present, KC_FLAG_HAS_VALUE);
-                o_weight = __fdiv_rn(f.cw_g, f.total);
-            }
-        }
-        for (uint32_t todo = __ballot_sync(0xFFFFFFFFu, undecided); todo; todo &= todo - 1)
-            wv_warp_walk<N>(lane, (uint32_t)__ffs((int)todo) - 1u, f, wts, rec_local, WROW, o_code, o_meta, o_weight);
-        if (g < n_groups) {
-            win[g] = o_code;
-            meta[g] = o_meta;
-            weight[g] = o_weight;
-        }
+        wv_tma_tile<N, WROW>(tiles, wts, g0, r0, n_groups, fm, has_nc, win, meta, weight, NoExtraCopy{}, f);
         __syncwarp();  // the next tile's weights overwrite these rows
         if (prefetch) {
 #pragma unroll
@@ -667,7 +675,6 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kerne
     constexpr int WROW = kWRowBulk<N>, WSLOTS = kWSlots<STAGES>;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     WarpTiles<N * 4, WARPS, STAGES> tiles(&tmap, n_groups);
-    const uint32_t lane = tiles.lane;
     const uint32_t slot_bytes = (uint32_t)rec_cap * WROW * 4;
     const uint32_t my_rows = tiles.end() + tiles.warp * (WSLOTS * slot_bytes);                           // shared-space address
     const float *my_rows_p = reinterpret_cast<const float *>(smem_raw + (my_rows - smem_u32(smem_raw)));  // the same, generic
@@ -680,54 +687,10 @@ __global__ void __launch_bounds__(WARPS * 32, MIN_CTAS) weighted_vote_rows_kerne
     tiles.start(L2Policy::evict_first, weight_rows);
 
     for (; tiles.t < tiles.n_tiles; tiles.next()) {
-        const uint32_t g0 = tiles.t * 32, g = g0 + lane;
-        const uint32_t r0 = wv_record_of(g0, fm, inv_fields);
-        const uint32_t fpos = (g0 - r0 * fm.n_fields) + lane;  // offset inside the tile's first record: < n_fields + 32
-        const uint32_t rec_local = g < n_groups ? fm.div_small(fpos) : 0u;
+        const uint32_t g0 = tiles.t * 32;
         const float *wts = my_rows_p + (tiles.it % WSLOTS) * (slot_bytes / 4);
-        const float *wrow = wts + rec_local * WROW;
-        const uint32_t tile = tiles.wait();
-        int32_t raw[N];
-#pragma unroll
-        for (int q = 0; q < N / 4; ++q) {
-            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
-            raw[4 * q + 0] = v4.x;
-            raw[4 * q + 1] = v4.y;
-            raw[4 * q + 2] = v4.z;
-            raw[4 * q + 3] = v4.w;
-        }
-        // this group's cell of its record's heaviest candidate: read from the tile while the stage is still ours
-        const int imax = __float_as_int(wrow[N]);
-        int32_t graw = KC_CODE_NONE - 1;
-        if (imax < N) {
-            asm volatile("ld.shared.s32 %0, [%1];" : "=r"(graw) : "r"(tile + tiles.at((uint32_t)imax * 4u)));
-        }
-        // the release's shuffle also means that every lane has left the previous tile, whose weight slot it refills
-        const int32_t lo = min(row_min<N>(raw), graw);
-        tiles.release((uint32_t)lo, weight_rows);
         WvFirst<N> f;
-        bool undecided = false;
-        int32_t o_code = KC_CODE_NONE;
-        uint32_t o_meta = 0;
-        float o_weight = 0.0f;
-        if (g < n_groups) {
-            const uint32_t field = fpos - rec_local * fm.n_fields;
-            const int32_t nc = has_nc ? __ldg(fm.none_code + field) : KC_CODE_NONE;
-            wv_first_pass<N>(raw, lo, nc, wrow, graw, f);
-            undecided = !f.decided;
-            if (f.decided) {
-                o_code = f.guess;
-                o_meta = pack_meta(ffs_mask(f.eq_g) - 1, popc_m(f.eq_g), f.voters, f.present, KC_FLAG_HAS_VALUE);
-                o_weight = __fdiv_rn(f.cw_g, f.total);
-            }
-        }
-        for (uint32_t todo = __ballot_sync(0xFFFFFFFFu, undecided); todo; todo &= todo - 1)
-            wv_warp_walk<N>(lane, (uint32_t)__ffs((int)todo) - 1u, f, wts, rec_local, WROW, o_code, o_meta, o_weight);
-        if (g < n_groups) {
-            win[g] = o_code;
-            meta[g] = o_meta;
-            weight[g] = o_weight;
-        }
+        wv_tma_tile<N, WROW>(tiles, wts, g0, wv_record_of(g0, fm, inv_fields), n_groups, fm, has_nc, win, meta, weight, weight_rows, f);
     }
 }
 
@@ -747,7 +710,7 @@ __global__ void __launch_bounds__(128) weighted_vote_groups_kernel(const int8_t 
     for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_groups; g += stride) {
         const int32_t rec = __ldg(group_record + g);
         int32_t raw[NP];
-        load_row_i8<NP, VEC>(codes, g, n, raw);
+        load_row<NP, VEC>(codes, g, n, raw);
         if (rec < 0 || rec >= n_records) {
             win[g] = KC_CODE_NONE;
             meta[g] = 0u;

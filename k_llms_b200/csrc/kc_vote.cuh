@@ -6,7 +6,8 @@
 // no tensor cores.  Two front-ends feed the same register core:
 //   * vote_tma_kernel    — n in {8,16,32,64}: every WARP runs its own TMA pipeline (WarpTiles, kc_common.cuh);
 //                          no block-wide barrier anywhere.
-//   * vote_direct_kernel — any n <= 64 (and n <= 4 where a thread's cells are one coalesced vector load).
+//   * vote_direct_kernel — any n <= 64 (and n <= 4 where a thread's cells are one coalesced vector load), on int32 or
+//                          int8 cells.
 #pragma once
 
 #include "kc_common.cuh"
@@ -161,6 +162,16 @@ __device__ __forceinline__ void vote_core(const int32_t (&raw)[N], int32_t lo, i
     meta = vote_scan<N, M>(x, N, win_code);
 }
 
+// The field phase of a strided walk over groups: f is the field of the current group, and advance() moves it `step` groups
+// on with one subtraction (f and step are both < n_fields).
+struct FieldCursor {
+    uint32_t f, step, n_fields;
+    __device__ __forceinline__ void advance() {
+        f += step;
+        f = f >= n_fields ? f - n_fields : f;
+    }
+};
+
 // field of group g without a 64-bit modulo: f = x - (x*magic >> 32)*F, exact for x < 2^16 (magic = 2^32/F + 1)
 struct FieldMap {
     const int32_t *none_code;  // NULL => no field has voting Nones
@@ -169,11 +180,18 @@ struct FieldMap {
     // x / n_fields and x % n_fields for x < n_fields + a few hundred (magic = 2^32 / n_fields + 1 does not fit for n_fields = 1)
     __device__ __forceinline__ uint32_t div_small(uint32_t x) const { return n_fields == 1u ? x : __umulhi(x, magic); }
     __device__ __forceinline__ uint32_t mod_small(uint32_t x) const { return x - div_small(x) * n_fields; }
+    // a walk over units of UNIT consecutive groups that starts at unit `first` and advances `step` units at a time; these are
+    // its only divisions
+    template <int UNIT = 1, typename I>
+    __device__ __forceinline__ FieldCursor cursor(I first, I step) const {
+        return {(uint32_t)((first * UNIT) % n_fields), (uint32_t)((step * UNIT) % n_fields), n_fields};
+    }
 };
 
 // ---------------------------------------------------------------- direct front-end
 
-// NP = n rounded up to a power of two (compile-time register array); cells beyond n are padded absent.
+// Row g of n cells into registers; one overload per cell type.  NP = n rounded up to a power of two (compile-time register
+// array); cells beyond n are padded absent.
 template <int NP, bool VEC>
 __device__ __forceinline__ void load_row(const int32_t *__restrict__ codes, int64_t g, int n, int32_t (&raw)[NP]) {
     if constexpr (VEC) {  // n == NP, rows are 16-byte aligned multiples of 16 bytes
@@ -201,19 +219,48 @@ __device__ __forceinline__ void load_row(const int32_t *__restrict__ codes, int6
     }
 }
 
-// Grid-stride, one group per thread per iteration.  With PREFETCH the next iteration's row is requested before
-// the current one is processed (twice the bytes in flight per thread, for ~NP more registers).
-template <int NP, bool VEC, bool HAS_NC, bool PREFETCH>
-__global__ void __launch_bounds__(256) vote_direct_kernel(const int32_t *__restrict__ codes, int64_t n_groups, int n,
+// Compact cells (int8).  Votes only need equality INSIDE a group, so a group can always be re-coded with local codes 0..n-1
+// (< 64): one byte per cell (-1 None, -2 absent) is a lossless input format at a quarter of the bytes — what the end-to-end
+// host path ships over PCIe.  A row of n = 16 cells is ONE 16-byte load per thread (a warp reads 512 contiguous bytes).
+template <int NP, bool VEC>
+__device__ __forceinline__ void load_row(const int8_t *__restrict__ codes, int64_t g, int n, int32_t (&raw)[NP]) {
+    if constexpr (VEC && NP >= 4) {
+        const uint32_t *p = reinterpret_cast<const uint32_t *>(codes + g * NP);
+        uint32_t w[NP / 4];
+        if constexpr (NP >= 16) {
+#pragma unroll
+            for (int q = 0; q < NP / 16; ++q) {
+                const int4 t = ldg_nc_v4(reinterpret_cast<const int4 *>(p) + q);
+                w[4 * q + 0] = (uint32_t)t.x;
+                w[4 * q + 1] = (uint32_t)t.y;
+                w[4 * q + 2] = (uint32_t)t.z;
+                w[4 * q + 3] = (uint32_t)t.w;
+            }
+        } else if constexpr (NP == 8) {
+            const uint2 t = __ldg(reinterpret_cast<const uint2 *>(p));
+            w[0] = t.x;
+            w[1] = t.y;
+        } else {
+            w[0] = __ldg(p);
+        }
+#pragma unroll
+        for (int i = 0; i < NP; ++i) raw[i] = (int32_t)(int8_t)(w[i / 4] >> (8 * (i % 4)));
+    } else {
+        const int8_t *p = codes + g * n;
+#pragma unroll
+        for (int i = 0; i < NP; ++i) raw[i] = (i < n) ? (int32_t)__ldg(p + i) : KC_CODE_ABSENT;
+    }
+}
+
+// Grid-stride, one group per thread per iteration, on Cell = int32_t or int8_t cells.  With PREFETCH the next iteration's
+// row is requested before the current one is processed (twice the bytes in flight per thread, for ~NP more registers).
+template <typename Cell, int NP, bool VEC, bool HAS_NC, bool PREFETCH>
+__global__ void __launch_bounds__(256) vote_direct_kernel(const Cell *__restrict__ codes, int64_t n_groups, int n,
                                                           FieldMap fm, int32_t *__restrict__ win,
                                                           uint32_t *__restrict__ meta, const __grid_constant__ OutRoute mc) {
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t f = 0, fstep = 0;
-    if constexpr (HAS_NC) {
-        f = (uint32_t)(g % fm.n_fields);
-        fstep = (uint32_t)(stride % fm.n_fields);
-    }
+    FieldCursor field = fm.cursor(g, stride);
     int32_t raw[NP];
     if (PREFETCH && g < n_groups) load_row<NP, VEC>(codes, g, n, raw);
     for (; g < n_groups; g += stride) {
@@ -225,9 +272,8 @@ __global__ void __launch_bounds__(256) vote_direct_kernel(const int32_t *__restr
         }
         int32_t nc = KC_CODE_NONE;
         if constexpr (HAS_NC) {
-            nc = __ldg(fm.none_code + f);
-            f += fstep;
-            f = f >= fm.n_fields ? f - fm.n_fields : f;
+            nc = __ldg(fm.none_code + field.f);
+            field.advance();
         }
         int32_t w;
         uint32_t m;
@@ -297,11 +343,7 @@ __global__ void __launch_bounds__(256) vote_multi_kernel(const int32_t *__restri
     static_assert(NP * GPT == 16, "a thread's unit is 64 bytes of cells");
     const int64_t stride = (int64_t)gridDim.x * blockDim.x;
     int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t f = 0, fstep = 0;
-    if constexpr (HAS_NC) {
-        f = (uint32_t)((u * GPT) % fm.n_fields);
-        fstep = (uint32_t)((stride * GPT) % fm.n_fields);
-    }
+    FieldCursor field = fm.cursor<GPT>(u, stride);  // the field of the unit's first group
     int32_t raw[16];
     auto load = [&](int64_t unit, int32_t (&dst)[16]) {
         const int4 *p = reinterpret_cast<const int4 *>(codes) + unit * 4;
@@ -327,17 +369,14 @@ __global__ void __launch_bounds__(256) vote_multi_kernel(const int32_t *__restri
             for (int i = 0; i < NP; ++i) x[i] = raw[j * NP + i];
             int32_t nc = KC_CODE_NONE;
             if constexpr (HAS_NC) {
-                uint32_t fj = f + (uint32_t)j;  // consecutive groups are consecutive fields
+                uint32_t fj = field.f + (uint32_t)j;  // consecutive groups are consecutive fields
                 fj = fj >= fm.n_fields ? fm.mod_small(fj) : fj;
                 nc = __ldg(fm.none_code + fj);
             }
             if constexpr (NP <= 4) vote_core_small<NP, HAS_NC>(x, nc, w[j], m[j]);
             else vote_core<NP, HAS_NC>(x, row_min<NP>(x), nc, w[j], m[j]);
         }
-        if constexpr (HAS_NC) {
-            f += fstep;
-            f = f >= fm.n_fields ? f - fm.n_fields : f;
-        }
+        if constexpr (HAS_NC) field.advance();
         if constexpr (GPT >= 4) {
 #pragma unroll
             for (int q = 0; q < GPT / 4; ++q) {
@@ -357,67 +396,6 @@ __global__ void __launch_bounds__(256) vote_multi_kernel(const int32_t *__restri
     }
 }
 
-// ---------------------------------------------------------------- compact cells (int8)
-
-// Votes only need equality INSIDE a group, so a group can always be re-coded with local codes 0..n-1 (< 64): one
-// byte per cell (-1 None, -2 absent) is a lossless input format at a quarter of the bytes — what the end-to-end host
-// path ships over PCIe.  A row of n = 16 cells is ONE 16-byte load per thread (a warp reads 512 contiguous bytes).
-template <int NP, bool VEC>
-__device__ __forceinline__ void load_row_i8(const int8_t *__restrict__ codes, int64_t g, int n, int32_t (&raw)[NP]) {
-    if constexpr (VEC && NP >= 4) {
-        const uint32_t *p = reinterpret_cast<const uint32_t *>(codes + g * NP);
-        uint32_t w[NP / 4];
-        if constexpr (NP >= 16) {
-#pragma unroll
-            for (int q = 0; q < NP / 16; ++q) {
-                const int4 t = ldg_nc_v4(reinterpret_cast<const int4 *>(p) + q);
-                w[4 * q + 0] = (uint32_t)t.x;
-                w[4 * q + 1] = (uint32_t)t.y;
-                w[4 * q + 2] = (uint32_t)t.z;
-                w[4 * q + 3] = (uint32_t)t.w;
-            }
-        } else if constexpr (NP == 8) {
-            const uint2 t = __ldg(reinterpret_cast<const uint2 *>(p));
-            w[0] = t.x;
-            w[1] = t.y;
-        } else {
-            w[0] = __ldg(p);
-        }
-#pragma unroll
-        for (int i = 0; i < NP; ++i) raw[i] = (int32_t)(int8_t)(w[i / 4] >> (8 * (i % 4)));
-    } else {
-        const int8_t *p = codes + g * n;
-#pragma unroll
-        for (int i = 0; i < NP; ++i) raw[i] = (i < n) ? (int32_t)__ldg(p + i) : KC_CODE_ABSENT;
-    }
-}
-
-template <int NP, bool VEC, bool HAS_NC>
-__global__ void __launch_bounds__(256) vote_i8_kernel(const int8_t *__restrict__ codes, int64_t n_groups, int n, FieldMap fm,
-                                                      int32_t *__restrict__ win, uint32_t *__restrict__ meta, const __grid_constant__ OutRoute mc) {
-    const int64_t stride = (int64_t)gridDim.x * blockDim.x;
-    int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    uint32_t f = 0, fstep = 0;
-    if constexpr (HAS_NC) {
-        f = (uint32_t)(g % fm.n_fields);
-        fstep = (uint32_t)(stride % fm.n_fields);
-    }
-    for (; g < n_groups; g += stride) {
-        int32_t raw[NP];
-        load_row_i8<NP, VEC>(codes, g, n, raw);
-        int32_t nc = KC_CODE_NONE;
-        if constexpr (HAS_NC) {
-            nc = __ldg(fm.none_code + f);
-            f += fstep;
-            f = f >= fm.n_fields ? f - fm.n_fields : f;
-        }
-        int32_t w;
-        uint32_t m;
-        vote_core<NP, HAS_NC>(raw, row_min<NP>(raw), nc, w, m);
-        store_vote_result(win, meta, g, w, m, mc);
-    }
-}
-
 // ---------------------------------------------------------------- TMA front-end
 
 // Persistent kernel on WarpTiles (kc_common.cuh): lane l votes row l of the warp's current tile.
@@ -428,30 +406,18 @@ __global__ void __launch_bounds__(WARPS * 32) vote_tma_kernel(const __grid_const
     WarpTiles<N * 4, WARPS, STAGES> tiles(&tmap, n_groups);
     tiles.start(L2Policy::evict_first);
 
-    uint32_t f0 = 0, fstep = 0;  // field of the tile's first group, advanced without division
-    if constexpr (HAS_NC) {
-        f0 = (uint32_t)(((uint64_t)tiles.t * 32) % fm.n_fields);
-        fstep = (uint32_t)(((uint64_t)tiles.step * 32) % fm.n_fields);
-    }
+    FieldCursor field = fm.cursor<32>((uint64_t)tiles.t, (uint64_t)tiles.step);  // the field of the tile's first group
     for (; tiles.t < tiles.n_tiles; tiles.next()) {
         const uint32_t tile = tiles.wait();
         int32_t raw[N];
-#pragma unroll
-        for (int q = 0; q < N / 4; ++q) {
-            const int4 v4 = lds_v4(tile + tiles.at(q * 16));
-            raw[4 * q + 0] = v4.x;
-            raw[4 * q + 1] = v4.y;
-            raw[4 * q + 2] = v4.z;
-            raw[4 * q + 3] = v4.w;
-        }
+        tiles.read_row(tile, raw);
         const int32_t lo = row_min<N>(raw);
         tiles.release((uint32_t)lo);
         const uint32_t g = tiles.t * 32 + tiles.lane;
         int32_t nc = KC_CODE_NONE;
         if constexpr (HAS_NC) {
-            nc = __ldg(fm.none_code + fm.mod_small(f0 + tiles.lane));
-            f0 += fstep;
-            f0 = f0 >= fm.n_fields ? f0 - fm.n_fields : f0;
+            nc = __ldg(fm.none_code + fm.mod_small(field.f + tiles.lane));
+            field.advance();
         }
         if (g < n_groups) {
             int32_t w;

@@ -185,6 +185,20 @@ int with_weight_rows(int64_t n_records, int wrow, cudaStream_t st, const char *w
 
 // ---------------------------------------------------------------- K1 launchers
 
+// The argument checks of K1's entry points, `who` naming the entry in the messages.  Zero groups pass once n is valid:
+// there is nothing to launch and the buffers are not looked at.  Without a none_code table every group is field 0.
+int check_vote_args(const char *who, const void *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t &n_fields,
+                    const void *d_win_code, const void *d_meta) {
+    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "%s: n=%d outside [1,%d]", who, n, KC_MAX_CANDIDATES);
+    if (n_groups < 0) return kc_fail(KC_EINVAL, "%s: negative n_groups", who);
+    if (n_groups == 0) return KC_OK;
+    if (!d_codes || !d_win_code || !d_meta) return kc_fail(KC_EINVAL, "%s: NULL buffer", who);
+    if (d_none_code && n_fields < 1) return kc_fail(KC_EINVAL, "%s: none_code given but n_fields=%d", who, n_fields);
+    if (!d_none_code) n_fields = 1;
+    if (!aligned16(d_codes)) return kc_fail(KC_EINVAL, "%s: d_codes must be 16-byte aligned", who);
+    return KC_OK;
+}
+
 kc::FieldMap make_field_map(const int32_t *none_code, int n_fields) {
     kc::FieldMap fm;
     fm.none_code = none_code;
@@ -207,16 +221,17 @@ int launch_vote_tma(const int32_t *codes, int64_t G, const int32_t *none_code, i
     return none_code ? go(kc::vote_tma_kernel<N, WARPS, STAGES, true>) : go(kc::vote_tma_kernel<N, WARPS, STAGES, false>);
 }
 
-// VEC: n == NP, whole 16-byte rows; those up to NP = 16 request the next row before working on this one
-template <int NP, bool VEC>
-int launch_vote_direct(const int32_t *codes, int64_t G, int n, const int32_t *none_code, int n_fields, int32_t *win,
+// Cell: int32_t or int8_t cells.  VEC: n == NP, whole rows; int32 rows from NP = 4 to 16 request the next row before working
+// on this one
+template <int NP, bool VEC, typename Cell>
+int launch_vote_direct(const Cell *codes, int64_t G, int n, const int32_t *none_code, int n_fields, int32_t *win,
                        uint32_t *meta, cudaStream_t st, kc::OutRoute mc) {
-    constexpr bool kPrefetch = VEC && NP >= 4 && NP <= 16;
+    constexpr bool kPrefetch = std::is_same_v<Cell, int32_t> && VEC && NP >= 4 && NP <= 16;
     const int threads = 256;
     int grid = 0;
     int rc = stride_grid((G + threads - 1) / threads, grid);
     if (rc) return rc;
-    auto kernel = none_code ? kc::vote_direct_kernel<NP, VEC, true, kPrefetch> : kc::vote_direct_kernel<NP, VEC, false, kPrefetch>;
+    auto kernel = none_code ? kc::vote_direct_kernel<Cell, NP, VEC, true, kPrefetch> : kc::vote_direct_kernel<Cell, NP, VEC, false, kPrefetch>;
     kernel<<<grid, threads, 0, st>>>(codes, G, n, make_field_map(none_code, n_fields), win, meta, mc);
     KC_CUDA_I(cudaGetLastError());
     return KC_OK;
@@ -249,19 +264,6 @@ int launch_vote_multi(const int32_t *codes, int64_t G, const int32_t *none_code,
             if (rc) return rc;
         }
     }
-    return KC_OK;
-}
-
-template <int NP, bool VEC>
-int launch_vote_i8(const int8_t *codes, int64_t G, int n, const int32_t *none_code, int n_fields, int32_t *win, uint32_t *meta,
-                   cudaStream_t st) {
-    const int threads = 256;
-    int grid = 0;
-    int rc = stride_grid((G + threads - 1) / threads, grid);
-    if (rc) return rc;
-    auto kernel = none_code ? kc::vote_i8_kernel<NP, VEC, true> : kc::vote_i8_kernel<NP, VEC, false>;
-    kernel<<<grid, threads, 0, st>>>(codes, G, n, make_field_map(none_code, n_fields), win, meta, kc::OutRoute{});
-    KC_CUDA_I(cudaGetLastError());
     return KC_OK;
 }
 
@@ -431,13 +433,8 @@ int kc_vote_i32_peers_packed(const int32_t *d_codes, int64_t n_groups, int32_t n
 
 static int vote_i32_routed(const int32_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t n_fields,
                            int32_t *d_win_code, uint32_t *d_meta, kc::OutRoute mc, void *stream) {
-    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_vote_i32: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
-    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_vote_i32: negative n_groups");
-    if (n_groups == 0) return KC_OK;
-    if (!d_codes || !d_win_code || !d_meta) return kc_fail(KC_EINVAL, "kc_vote_i32: NULL buffer");
-    if (d_none_code && n_fields < 1) return kc_fail(KC_EINVAL, "kc_vote_i32: none_code given but n_fields=%d", n_fields);
-    if (!d_none_code) n_fields = 1;
-    if (!aligned16(d_codes)) return kc_fail(KC_EINVAL, "kc_vote_i32: d_codes must be 16-byte aligned");
+    const int rc = check_vote_args("kc_vote_i32", d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta);
+    if (rc || n_groups == 0) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     // measured on H100 SXM (400 W, 1M x 24 fields): the direct front-end wins up to n = 16 (0.59 vs 0.63 ms at n = 16), the
     // TMA pipeline from n = 32 (1.12 vs 1.30 ms at n = 32)
@@ -532,19 +529,15 @@ int kc_push_results(const int32_t *d_win_code, const uint32_t *d_vote_meta, int6
 
 int kc_vote_i8(const int8_t *d_codes, int64_t n_groups, int32_t n, const int32_t *d_none_code, int32_t n_fields,
                int32_t *d_win_code, uint32_t *d_meta, void *stream) {
-    if (n < 1 || n > KC_MAX_CANDIDATES) return kc_fail(KC_EINVAL, "kc_vote_i8: n=%d outside [1,%d]", n, KC_MAX_CANDIDATES);
-    if (n_groups < 0) return kc_fail(KC_EINVAL, "kc_vote_i8: negative n_groups");
-    if (n_groups == 0) return KC_OK;
-    if (!d_codes || !d_win_code || !d_meta) return kc_fail(KC_EINVAL, "kc_vote_i8: NULL buffer");
-    if (d_none_code && n_fields < 1) return kc_fail(KC_EINVAL, "kc_vote_i8: none_code given but n_fields=%d", n_fields);
-    if (!d_none_code) n_fields = 1;
-    if (!aligned16(d_codes)) return kc_fail(KC_EINVAL, "kc_vote_i8: d_codes must be 16-byte aligned");
+    const int rc = check_vote_args("kc_vote_i8", d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta);
+    if (rc || n_groups == 0) return rc;
     cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const kc::OutRoute local{};
     // n a power of two from 4 on: whole 16-byte rows; any other n: the next power of two, cells beyond n absent
     return with_pow2<4>(n, [&](auto np) {
         constexpr int NP = decltype(np)::value;
-        if (n == NP) return launch_vote_i8<NP, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
-        return launch_vote_i8<NP, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st);
+        if (n == NP) return launch_vote_direct<NP, true>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, local);
+        return launch_vote_direct<NP, false>(d_codes, n_groups, n, d_none_code, n_fields, d_win_code, d_meta, st, local);
     });
 }
 

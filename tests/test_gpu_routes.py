@@ -446,14 +446,15 @@ def _both(fmt):
 COVERAGE = (
     # K1, local n = 2, 4, 8: GPT groups per thread, the last < GPT groups one per thread (also the non-local n = 2, 4, 8)
     _both("vote_multi_kernel<2,8,{nc}>") + _both("vote_multi_kernel<4,4,{nc}>") + _both("vote_multi_kernel<8,2,{nc}>")
-    + _both("vote_direct_kernel<2,true,{nc},false>") + _both("vote_direct_kernel<4,true,{nc},true>")
-    + _both("vote_direct_kernel<8,true,{nc},true>")
+    + _both("vote_direct_kernel<int,2,true,{nc},false>") + _both("vote_direct_kernel<int,4,true,{nc},true>")
+    + _both("vote_direct_kernel<int,8,true,{nc},true>")
     # K1 n = 1, 16; n = 32, 64 (TMA); other n: the next power of two, cells beyond n absent
-    + _both("vote_direct_kernel<1,true,{nc},false>") + _both("vote_direct_kernel<16,true,{nc},true>")
+    + _both("vote_direct_kernel<int,1,true,{nc},false>") + _both("vote_direct_kernel<int,16,true,{nc},true>")
     + _both("vote_tma_kernel<32,8,2,{nc}>") + _both("vote_tma_kernel<64,4,2,{nc}>")
-    + [s for np_ in (4, 8, 16, 32, 64) for s in _both(f"vote_direct_kernel<{np_},false,{{nc}},false>")]
-    # K1 on int8 cells
-    + [s for np_ in (4, 8, 16, 32, 64) for vec in ("false", "true") for s in _both(f"vote_i8_kernel<{np_},{vec},{{nc}}>")]
+    + [s for np_ in (4, 8, 16, 32, 64) for s in _both(f"vote_direct_kernel<int,{np_},false,{{nc}},false>")]
+    # K1 on int8 cells (never PREFETCH)
+    + [s for np_ in (4, 8, 16, 32, 64) for vec in ("false", "true")
+       for s in _both(f"vote_direct_kernel<signedchar,{np_},{vec},{{nc}},false>")]
     # K2 local: n = 2, 4 (+ their one-group tails), 8, 16, 32 fast kernels
     + ["numeric_pairs_kernel", "numeric_quads_kernel", "numeric_direct_fast_kernel<8,128>", "numeric_tma_fast_kernel<16,4,1,6>",
        "numeric_tma_fast_kernel<32,4,1,4>"]
