@@ -661,7 +661,7 @@ int kc_weighted_vote_i32(const int32_t *d_codes, const float *d_seq_logprob, int
                                                        d_win_code + g0, d_meta + g0, d_weight + g0);
             });
         };
-        if (n == 32 && rec_cap <= 8) {  // weights by a pre-pass, fetched per tile by a bulk copy (n_fields >= 6; n = 32 only)
+        if (n == 32 && rec_cap <= 8) {  // weights by a pre-pass, fetched per tile by a bulk copy (n_fields >= 5; n = 32 only)
             constexpr int N = 32, WARPS = 8, STAGES = 2, WROW = kc::kWRowBulk<N>;
             return with_weight_rows(
                 n_records, WROW, st, "kc_weighted_vote_i32",
