@@ -7,7 +7,6 @@ record's heaviest candidate None / absent / losing / tied, clamped weights, rows
 kc_weighted_vote_groups_i8 with shuffled group_record.  Each test checks under torch.profiler that the kernels it means to
 test ran, and counts on the host how many groups wv_first_pass leaves to the warp walk, so that a generator change cannot
 quietly make the cases easy."""
-import contextlib
 import json
 
 import numpy as np
@@ -15,6 +14,7 @@ import pytest
 
 from oracle import columnar as OC
 from tests import test_weighted_edges_host as H
+from tests.helpers import assert_kernels_ran, kernels_seen, profiled
 
 pytestmark = pytest.mark.gpu
 
@@ -52,41 +52,6 @@ def i32_kernels(n, F):
 def groups_kernels(n):
     np_ = _pow2(n, 4)
     return [f"weight_rows_n_kernel<{np_}>", f"weighted_vote_groups_kernel<{np_},{'true' if n == np_ else 'false'}>"]
-
-
-def _kernel_key(name):
-    import re
-    m = re.search(r"kc::(\w+(?:<[^()]*>)?)\(", name)
-    return m.group(1).replace(" ", "") if m else None
-
-
-@contextlib.contextmanager
-def profiled():
-    """torch.profiler over the block.  In a full-suite run the kernels launched right after the profiler started were
-    missing from its record, so a few throwaway kernels go first."""
-    torch = _torch()
-    from torch.profiler import ProfilerActivity, profile
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        x = torch.zeros(1024, device="cuda")
-        for _ in range(8):
-            x.add_(1)
-        torch.cuda.synchronize()
-        yield prof
-        torch.cuda.synchronize()
-
-
-def _seen(prof):
-    torch = _torch()
-    names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
-    return {k for k in map(_kernel_key, names) if k}, bool(names)
-
-
-def _assert_ran(prof, expected):
-    seen, any_names = _seen(prof)
-    if not any_names:
-        pytest.skip("torch.profiler recorded no CUDA kernels on this machine (CUPTI unavailable)")
-    missing = sorted(set(expected) - seen)
-    assert not missing, (missing, sorted(k for k in seen if "weight" in k))
 
 
 def run_i32(codes, seq, nc):
@@ -157,7 +122,7 @@ def test_every_k3b_kernel_on_the_edge_families(n):
                         undecided[kernels[-1]] = undecided.get(kernels[-1], 0) + int(H.first_pass(*rows, ref).sum())
                     if not with_nc:
                         check_groups(rng, codes, seq, ref, what)
-    _assert_ran(prof, expected)
+    assert_kernels_ran(prof, expected)
     print(f"\nn={n}: groups with the tie flag {ties}; groups wv_first_pass leaves to the warp walk {undecided}")
     assert ties >= 500 or n == 1, ties  # one cell cannot tie
     for k, v in undecided.items():
@@ -177,7 +142,7 @@ def test_rows_kernel_cycles_weight_slots():
     nc = np.where(np.arange(F) % 2 == 0, -1, rng.integers(0, 128, F)).astype(np.int32)
     with profiled() as prof:
         got = run_i32(codes, seq, nc)
-    _assert_ran(prof, i32_kernels(n, F))
+    assert_kernels_ran(prof, i32_kernels(n, F))
     ew, em, ewt = OC.weighted_vote(codes, seq, nc)
     H.check_against(got, dict(win=ew, meta=em, weight=ewt), "rows kernel, all groups")
     c2, s2, nc2 = H.flat(codes, seq, nc)
@@ -199,7 +164,7 @@ def test_many_fields_fallback_on_the_edges(n):
     codes, seq, nc = H.make_case(rng, 3, n, 2, F, True, pool=[(None, p[1], p[2]) for p in pool])
     with profiled() as prof:
         ref, _ = check_case(codes, seq, nc, ("fallback", n))
-    _assert_ran(prof, i32_kernels(n, F))
+    assert_kernels_ran(prof, i32_kernels(n, F))
     assert i32_kernels(n, F) == [f"weighted_vote_rec_kernel<{n},128>"]
     assert int(((ref["meta"] >> 29) & 1).sum()) >= 100
 
@@ -213,7 +178,7 @@ def test_rows_kernel_switch_at_five_fields(F):
     codes, seq, nc = H.make_case(rng, 1, 32, 400, F, False)
     with profiled() as prof:
         check_case(codes, seq, nc, ("switch", F))
-    seen, any_names = _seen(prof)
+    seen, any_names = kernels_seen(prof)
     if not any_names:
         pytest.skip("torch.profiler recorded no CUDA kernels on this machine (CUPTI unavailable)")
     rows = "weighted_vote_rows_kernel<32,8,2,3>" in seen
