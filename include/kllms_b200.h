@@ -378,8 +378,8 @@ void kc_free_strings(char **arr, int64_t count);
  *            KC_JSON_UNICODE: string values may hold non-ASCII text and \uXXXX escapes (UTF-8 validated as Python's strict
  *                     decoder does).  A field decided by the similarity medoid (some value has >= 3 words) stays on the device:
  *                     it compares normalize_string forms (ASCII alphanumerics, lower-cased; every other code point dropped) and
- *                     prints the chosen original as json.dumps does (ensure_ascii).  A vote field with such a value, a non-ASCII or
- *                     escaped key, and a record of the list round with such text are declined as without it (why = 3; the list
+ *                     prints the chosen original as json.dumps does (ensure_ascii).  A vote field with such a value, a key with
+ *                     non-ASCII, DEL or escapes, and a record of the list round with such text are declined as without it (why = 3; the list
  *                     round's alignment declines non-ASCII: why = 15).  The client functions set it.
  *   *out     result handle: one text blob + per-record spans (kc_json_result_view), released with kc_json_result_free
  * status per record: 0 = consolidated on the device, 2 = consolidated by the host path, 1 = needs the Python path.

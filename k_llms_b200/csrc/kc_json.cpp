@@ -43,7 +43,7 @@ namespace {
 enum TokType : uint8_t { T_MISSING = 0, T_NULL, T_TRUE, T_FALSE, T_INT, T_FLOAT, T_STR, T_NESTED };
 
 // A token is a VIEW into the candidate text (no copies): strings keep their raw inner span and an "has escapes" flag
-// and are unescaped only where the value is needed; numbers keep their text span and the strtod value.
+// and are read character by character (each_char) where the value is needed; numbers keep their text span and the strtod value.
 struct Tok {
     TokType type = T_MISSING;
     bool esc = false;
@@ -57,51 +57,30 @@ struct Item {
     Tok tok;
 };
 
-inline bool is_ws(char c) { return c == ' ' || c == '\t' || c == '\n' || c == '\r'; }
-// str.split() / str.strip() whitespace within ASCII: \t \n \v \f \r, \x1c-\x1f and space
-inline bool is_py_space(unsigned char c) { return c == ' ' || (c >= 9 && c <= 13) || (c >= 0x1c && c <= 0x1f); }
-
-// raw inner span of a JSON string -> value (ASCII only; \uXXXX above 0x7F never gets here)
-void unescape(const char *p, uint32_t len, std::string &out) {
-    out.clear();
-    const char *e = p + len;
-    while (p < e) {
-        if (*p != '\\') {
-            out.push_back(*p++);
-            continue;
-        }
-        ++p;
-        switch (*p++) {
-            case 'b': out.push_back('\b'); break;
-            case 'f': out.push_back('\f'); break;
-            case 'n': out.push_back('\n'); break;
-            case 'r': out.push_back('\r'); break;
-            case 't': out.push_back('\t'); break;
-            case 'u': {
-                unsigned v = 0;
-                for (int i = 0; i < 4; ++i) {
-                    const char h = p[i];
-                    v = (v << 4) | (unsigned)(h <= '9' ? h - '0' : (h | 0x20) - 'a' + 10);
-                }
-                p += 4;
-                out.push_back((char)(v & 0x7F));
-                break;
-            }
-            default: out.push_back(p[-1]); break;  // \" \\ \/
-        }
+// f(c) for each character of a string given by its span: with `esc` (a raw JSON span holding escapes) each escape is decoded
+// by kc::js::decode_cp; every other byte is one character.  A span without escapes is the value itself, and it need not be
+// JSON: the {"text": ...} wrapper and the aligned tree's strings are decoded values, in which a backslash is a backslash.
+template <typename F>
+void each_char(const char *p, uint32_t len, bool esc, F f) {
+    const uint8_t *s = (const uint8_t *)p;
+    for (uint32_t i = 0; i < len;) {
+        if (esc && s[i] == '\\') f(kc::js::decode_cp(s, len, i));
+        else f((uint32_t)s[i++]);
     }
 }
 
-inline void tok_string(const Tok &t, std::string &out) {  // value of a T_STR token
-    if (t.esc) unescape(t.p, t.len, out);
-    else out.assign(t.p, t.len);
+// the value of a string from its span, one byte per character (H1 declines \uXXXX escapes above 0x7F)
+void str_value(const char *p, uint32_t len, bool esc, std::string &out) {
+    out.clear();
+    if (!esc) out.assign(p, len);
+    else each_char(p, len, true, [&](uint32_t c) { out.push_back((char)c); });
 }
 
 struct Scanner {
     const char *p, *end;
     bool non_ascii = false;
     void ws() {
-        while (p < end && is_ws(*p)) ++p;
+        while (p < end && kc::js::is_json_ws((uint8_t)*p)) ++p;
     }
     bool lit(const char *s, size_t n) {
         if ((size_t)(end - p) >= n && memcmp(p, s, n) == 0) {
@@ -132,16 +111,8 @@ struct Scanner {
             if (++p >= end) return false;
             const char k = *p++;
             if (k == 'u') {
-                if (end - p < 4) return false;
-                unsigned v = 0;
-                for (int i = 0; i < 4; ++i) {
-                    const char h = p[i];
-                    v <<= 4;
-                    if (h >= '0' && h <= '9') v |= (unsigned)(h - '0');
-                    else if (h >= 'a' && h <= 'f') v |= (unsigned)(h - 'a' + 10);
-                    else if (h >= 'A' && h <= 'F') v |= (unsigned)(h - 'A' + 10);
-                    else return false;
-                }
+                uint32_t v;
+                if (end - p < 4 || !kc::js::hex4((const uint8_t *)p, v)) return false;
                 p += 4;
                 if (v >= 0x80) non_ascii = true;  // parity for non-ASCII text is unpinned: hand the record to Python
             } else if (!(k == '"' || k == '\\' || k == '/' || k == 'b' || k == 'f' || k == 'n' || k == 'r' || k == 't')) {
@@ -319,31 +290,18 @@ void put_float(double x, std::string &out) {
     out.append((const char *)buf, (size_t)o.n);
 }
 
-// json.dumps(str) with ensure_ascii=True (input is ASCII)
-void json_string(std::string_view s, std::string &out) {
-    static const char *hex = "0123456789abcdef";
-    out.push_back('"');
-    for (unsigned char c : s) {
-        switch (c) {
-            case '"': out += "\\\""; break;
-            case '\\': out += "\\\\"; break;
-            case '\n': out += "\\n"; break;
-            case '\r': out += "\\r"; break;
-            case '\t': out += "\\t"; break;
-            case '\b': out += "\\b"; break;
-            case '\f': out += "\\f"; break;
-            default:
-                if (c < 0x20) {
-                    out += "\\u00";
-                    out.push_back(hex[c >> 4]);
-                    out.push_back(hex[c & 15]);
-                } else {
-                    out.push_back((char)c);
-                }
-        }
-    }
-    out.push_back('"');
+// json.dumps(str) with ensure_ascii=True of a string given by its span (each_char), quotes included: every character through
+// the device path's kc::js::Sink::json_char
+void json_string(const char *p, uint32_t len, bool esc, std::string &out) {
+    const size_t k = out.size();
+    out.resize(k + 6 * (size_t)len + 2);  // json_char prints at most six bytes per byte of the span (a surrogate pair: twelve for twelve)
+    kc::js::Sink o{(uint8_t *)out.data() + k, 0};
+    o.put('"');
+    each_char(p, len, esc, [&](uint32_t c) { o.json_char(c); });
+    o.put('"');
+    out.resize(k + (size_t)o.n);
 }
+void json_string(std::string_view s, std::string &out) { json_string(s.data(), (uint32_t)s.size(), false, out); }  // a decoded string
 
 // str(int) of a JSON integer token: the digits as written (JSON forbids leading zeros), except "-0" -> "0"
 void int_text(const Tok &t, std::string &out) {
@@ -351,7 +309,7 @@ void int_text(const Tok &t, std::string &out) {
     else out.append(t.p, t.len);
 }
 
-// str(v) as Python prints the value (for the enum-likeness test and for sanitising)
+// str(v) of a bool or number token as Python prints it (the vote classes sanitise it like a string)
 void py_str(const Tok &t, std::string &out) {
     switch (t.type) {
         case T_TRUE: out += "True"; break;
@@ -362,41 +320,26 @@ void py_str(const Tok &t, std::string &out) {
             else if (std::isinf(t.num)) out += t.num < 0 ? "-inf" : "inf";
             else put_float(t.num, out);
             break;
-        case T_STR: {
-            if (t.esc) {
-                std::string tmp;
-                unescape(t.p, t.len, tmp);
-                out += tmp;
-            } else {
-                out.append(t.p, t.len);
-            }
-            break;
-        }
         default: break;
     }
 }
 
-int word_count(const std::string &s) {  // len(s.strip().split())
-    int n = 0;
-    bool in = false;
-    for (unsigned char c : s) {
-        const bool sp = is_py_space(c);
-        if (!sp && !in) ++n;
-        in = !sp;
-    }
-    return n;
-}
-
-void sanitize(const std::string &s, std::string &out) {  // consensus_utils.py:925-933 on ASCII
-    out.resize(s.size());  // at most as long: written in place, trimmed once (no per-character capacity checks)
+// sanitize_value(s) (consensus_utils.py:925-933; == normalize_string, :660-673, on ASCII) of a string given by its span
+// (each_char): the characters kc::js::is_alnum_lower keeps, lower-cased.  Returns len(s).
+uint32_t sanitized(const char *p, uint32_t len, bool esc, std::string &out) {
+    out.resize(len);  // at most one character per byte: written in place, trimmed once (no per-character capacity checks)
     char *o = out.data();
     size_t k = 0;
-    for (unsigned char c : s) {
-        if (c >= 'A' && c <= 'Z') c = (unsigned char)(c + 32);
-        o[k] = (char)c;
-        k += ((c >= 'a' && c <= 'z') || (c >= '0' && c <= '9')) ? 1 : 0;
-    }
+    uint32_t chars = 0;
+    each_char(p, len, esc, [&](uint32_t c) {
+        uint8_t b = (uint8_t)c;
+        const bool keep = c < 0x80 && kc::js::is_alnum_lower(b);
+        o[k] = (char)b;
+        k += keep ? 1 : 0;
+        ++chars;
+    });
     out.resize(k);
+    return chars;
 }
 
 void json_value(const Tok &t, std::string &out) {
@@ -405,12 +348,7 @@ void json_value(const Tok &t, std::string &out) {
         case T_FALSE: out += "false"; break;
         case T_INT: int_text(t, out); break;
         case T_FLOAT: put_float(t.num, out); break;
-        case T_STR: {
-            std::string tmp;
-            tok_string(t, tmp);
-            json_string(tmp, out);
-            break;
-        }
+        case T_STR: json_string(t.p, t.len, t.esc, out); break;
         default: out += "null"; break;
     }
 }
@@ -448,7 +386,7 @@ struct Record {
 const double kF64None = [] { const uint64_t b = KC_F64_NONE_BITS; double d; memcpy(&d, &b, 8); return d; }();
 
 // Scalar field: which kernel decides it (cu:1405-1411 vote, cu:1443-1453 numeric / medoid).  False: Python path.
-bool plan_leaf(Record &rec, Group &g, const Tok *cells, int n, std::string &tmp) {
+bool plan_leaf(Record &rec, Group &g, const Tok *cells, int n) {
     const Tok *first = nullptr;
     for (int c = 0; c < n && !first; ++c)
         if (cells[c].type > T_NULL) first = &cells[c];
@@ -470,9 +408,14 @@ bool plan_leaf(Record &rec, Group &g, const Tok *cells, int n, std::string &tmp)
             }
             all_str &= t.type == T_STR;
             if (t.type == T_STR) {  // numbers and bools print as one word
-                tmp.clear();
-                py_str(t, tmp);
-                multi_word |= word_count(tmp) >= 3;
+                int words = 0;      // len(s.split())
+                bool in = false;
+                each_char(t.p, t.len, t.esc, [&](uint32_t ch) {
+                    const bool sp = kc::js::is_py_space(ch);
+                    words += (!sp && !in) ? 1 : 0;
+                    in = !sp;
+                });
+                multi_word |= words >= 3;
             }
         }
         if (multi_word) {
@@ -492,10 +435,7 @@ bool plan_leaf(Record &rec, Group &g, const Tok *cells, int n, std::string &tmp)
                 for (int c = 0; c < n; ++c) {
                     const Tok &t = cells[c];
                     if (t.type != T_STR) continue;
-                    tmp.clear();
-                    py_str(t, tmp);
-                    sanitize(tmp, norm);  // == normalize_string (cu:660-673) on ASCII text
-                    long_raw += tmp.size() > 50;
+                    long_raw += sanitized(t.p, t.len, t.esc, norm) > 50;  // len(s) > 50
                     long_norm += norm.size() > 64;
                     if (norm.size() > 2000 || long_raw > 1 || long_norm > 1) {
                         rec.status = 1;
@@ -539,7 +479,6 @@ struct LevelScratch {  // per recursion depth, reused across records (no allocat
 
 void plan_dict(Record &rec, int32_t node, const std::vector<Item> *const *items, int n, int depth) {
     thread_local std::vector<LevelScratch> levels(kMaxDepth + 1);  // sized once: references stay valid through the recursion
-    thread_local std::string tmp;
     LevelScratch &L = levels[(size_t)depth];
     std::vector<std::string_view> &keys = L.keys;
     keys.clear();
@@ -607,7 +546,7 @@ void plan_dict(Record &rec, int32_t node, const std::vector<Item> *const *items,
         const Tok *gcells = &rec.cells[base];
         Group g;
         g.key = key;
-        if (!plan_leaf(rec, g, gcells, n, tmp)) return;
+        if (!plan_leaf(rec, g, gcells, n)) return;
         const int32_t kid = (int32_t)rec.nodes.size();
         rec.nodes.emplace_back();
         rec.nodes[(size_t)kid].key = key;
@@ -680,9 +619,13 @@ void encode_vote(GroupKind kind, const Tok *toks, int n, int8_t *cells) {
             cells[c] = KC_CODE_NONE;
             continue;
         }
-        tmp.clear();
-        py_str(t, tmp);
-        sanitize(tmp, san);
+        if (t.type == T_STR) {
+            sanitized(t.p, t.len, t.esc, san);
+        } else {
+            tmp.clear();
+            py_str(t, tmp);
+            sanitized(tmp.data(), (uint32_t)tmp.size(), false, san);
+        }
         size_t k = 0;
         while (k < n_seen && seen[k] != san) ++k;
         if (k == n_seen) {
@@ -811,7 +754,7 @@ void emit_record(const Record &rec, int n, const uint32_t *vmeta, const double *
             }
             if (picked && picked->type == T_STR) {
                 content.clear();
-                tok_string(*picked, content);
+                str_value(picked->p, picked->len, picked->esc, content);
             }
         }
     }
@@ -862,7 +805,7 @@ Tok tok_of(const AVal &v) {  // a scalar of the tree as the token the leaf plann
 // The dispatcher (cu:1376-1454) over ALIGNED candidates: after the pre-pass every candidate is a dict with the same sorted
 // keys at a dict node and a list of the same width at a list node (cu:516-548, 550-613), so parent_valid_frac stays 1 and a
 // node is a dict, a list or a scalar field.  Anything the pre-pass left unaligned (mixed types) goes to the Python path.
-void plan_tree_value(Record &rec, AlignCtx &cx, int32_t node, const std::vector<int32_t> &ids, int n, int depth, std::string &tmp) {
+void plan_tree_value(Record &rec, AlignCtx &cx, int32_t node, const std::vector<int32_t> &ids, int n, int depth) {
     if (depth > 48) {
         rec.status = 1;
         return;
@@ -900,7 +843,7 @@ void plan_tree_value(Record &rec, AlignCtx &cx, int32_t node, const std::vector<
                 rec.nodes.emplace_back();
                 rec.nodes[(size_t)kid].key = key;
                 rec.nodes[(size_t)node].kids.push_back(kid);
-                plan_tree_value(rec, cx, kid, child, n, depth + 1, tmp);
+                plan_tree_value(rec, cx, kid, child, n, depth + 1);
                 if (rec.status) return;
             }
         } else {
@@ -916,7 +859,7 @@ void plan_tree_value(Record &rec, AlignCtx &cx, int32_t node, const std::vector<
                 const int32_t kid = (int32_t)rec.nodes.size();
                 rec.nodes.emplace_back();
                 rec.nodes[(size_t)node].kids.push_back(kid);
-                plan_tree_value(rec, cx, kid, child, n, depth + 1, tmp);
+                plan_tree_value(rec, cx, kid, child, n, depth + 1);
                 if (rec.status) return;
             }
         }
@@ -927,7 +870,7 @@ void plan_tree_value(Record &rec, AlignCtx &cx, int32_t node, const std::vector<
     for (int c = 0; c < n; ++c) rec.cells.push_back(tok_of(cx.tr.v[(size_t)ids[(size_t)c]]));
     Group g;
     g.key = rec.nodes[(size_t)node].key;
-    if (!plan_leaf(rec, g, &rec.cells[base], n, tmp)) return;
+    if (!plan_leaf(rec, g, &rec.cells[base], n)) return;
     rec.nodes[(size_t)node].group = (int32_t)rec.groups.size();
     rec.groups.push_back(g);
 }
@@ -979,9 +922,8 @@ void finish_record_tree(Record &rec, const std::shared_ptr<AlignCtx> &cxp, std::
         rec.status = 1;
         return;
     }
-    thread_local std::string tmp;
     rec.nodes.emplace_back();
-    plan_tree_value(rec, cx, 0, values, n, 0, tmp);
+    plan_tree_value(rec, cx, 0, values, n, 0);
     if (rec.status == 0) rec.tree = cxp;  // from here on nothing is added to the tree: cells and keys point into it
 }
 

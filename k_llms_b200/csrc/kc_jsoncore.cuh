@@ -132,7 +132,7 @@ KC_HD inline double bits_f64(uint64_t b) {
 // lists: `[` opens a list node (K_LOPEN, its elements keyless TOK_ELEM tokens one level deeper, K_LCLOSE) instead of declining
 // the record with D_NESTED; *has_list (optional): whether the text holds a list.  unicode: string VALUES may hold raw UTF-8
 // (validated), \uXXXX escapes and a raw DEL (the token gets TOK_UNICODE, its words are counted over Python's whitespace) instead
-// of declining the record with D_ESCAPE_OR_NON_ASCII; keys stay ASCII.
+// of declining the record with D_ESCAPE_OR_NON_ASCII; keys stay ASCII without DEL or escapes (json.dumps prints them as they are).
 KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, Tok *toks, int32_t stride, int32_t cap, bool *nested = nullptr,
                                  bool lists = false, bool *has_list = nullptr, bool unicode = false) {
     uint32_t p = 0;
@@ -164,7 +164,7 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
                 const uint8_t c = s[p];
                 if (c == '"') break;
                 if (c < 0x20) return -D_SYNTAX;
-                if (c >= 0x80 || c == '\\') return -D_ESCAPE_OR_NON_ASCII;
+                if (c >= 0x7F || c == '\\') return -D_ESCAPE_OR_NON_ASCII;  // the emit prints a key's bytes: DEL and escapes decline
                 ++p;
             }
             const uint32_t klen = p - kstart;
@@ -192,16 +192,15 @@ KC_HD inline int32_t scan_object(const uint8_t *s, uint32_t len, uint32_t rel, T
                 if (d < 0x20) return -D_SYNTAX;
                 bool sp = d == ' ';  // the only ASCII str.split() whitespace a raw JSON string can hold unescaped
                 if (d >= 0x7F) {
-                    if (d == 0x7F) {
-                        uni |= unicode;  // DEL: json.dumps prints it as \u007f
-                    } else {
+                    if (!unicode) return -D_ESCAPE_OR_NON_ASCII;
+                    if (d > 0x7F) {
                         uint32_t cp = 0;
-                        const uint32_t k = unicode ? utf8_decode(s + p, len - p, cp) : 0u;
+                        const uint32_t k = utf8_decode(s + p, len - p, cp);
                         if (k == 0) return -D_ESCAPE_OR_NON_ASCII;
                         sp = is_py_space(cp);
-                        uni = true;
                         p += k - 1;
                     }
+                    uni = true;  // DEL too: json.dumps prints it as \u007f
                 } else if (d == '\\') {
                     // the two-character escapes stay in the token (TOK_ESCAPED; every reader of the value skips or maps them);
                     // \uXXXX (any code point, surrogate pairs, non-ASCII) is the host path's unless `unicode`
@@ -608,31 +607,33 @@ struct Sink {
             put((uint8_t)(d < 10 ? '0' + d : 'a' + d - 10));
         }
     }
+    // json.dumps of one character of a string (ensure_ascii): `"` `\` and \n \r \t \b \f as two-character escapes, other
+    // controls and DEL as \u00xx, printable ASCII as itself, the rest of the BMP (lone surrogates included) as \uxxxx, astral
+    // code points as a surrogate pair.  The host path (kc_json.cpp) prints its strings through it as well.
+    KC_HD void json_char(uint32_t cp) {
+        if (cp == '"' || cp == '\\') {
+            put('\\');
+            put((uint8_t)cp);
+        } else if (cp >= 0x20 && cp < 0x7F) {
+            put((uint8_t)cp);
+        } else if (cp == '\n' || cp == '\r' || cp == '\t' || cp == 8 || cp == 12) {
+            put('\\');
+            put(cp == '\n' ? 'n' : (cp == '\r' ? 'r' : (cp == '\t' ? 't' : (cp == 8 ? 'b' : 'f'))));
+        } else if (cp >= 0x10000) {
+            u_escape(0xD800u + ((cp - 0x10000u) >> 10));
+            u_escape(0xDC00u + ((cp - 0x10000u) & 0x3FFu));
+        } else {
+            u_escape(cp);
+        }
+    }
     // json.dumps of a string value (ensure_ascii), quotes included, from its raw span (token flags: TOK_ESCAPED, TOK_UNICODE).
     // ASCII spans: the two-character escapes are already what json.dumps prints, except "\/", which it prints as "/".  TOK_UNICODE
-    // spans are decoded to code points and printed one by one: `"` `\` and \n \r \t \b \f as two-character escapes, other
-    // controls and DEL as \u00xx, printable ASCII as itself, the rest of the BMP (lone surrogates included) as \uxxxx, astral
-    // code points as a surrogate pair.  The length pass counts exactly what the write pass writes: it is this same code.
+    // spans are decoded to code points and printed one by one (json_char).  The length pass counts exactly what the write pass
+    // writes: it is this same code.
     KC_HD void json_string(const uint8_t *s, uint32_t len, uint8_t flags) {
         put('"');
         if (flags & TOK_UNICODE) {
-            for (uint32_t i = 0; i < len;) {
-                const uint32_t cp = decode_cp(s, len, i);
-                if (cp == '"' || cp == '\\') {
-                    put('\\');
-                    put((uint8_t)cp);
-                } else if (cp >= 0x20 && cp < 0x7F) {
-                    put((uint8_t)cp);
-                } else if (cp == '\n' || cp == '\r' || cp == '\t' || cp == 8 || cp == 12) {
-                    put('\\');
-                    put(cp == '\n' ? 'n' : (cp == '\r' ? 'r' : (cp == '\t' ? 't' : (cp == 8 ? 'b' : 'f'))));
-                } else if (cp >= 0x10000) {
-                    u_escape(0xD800u + ((cp - 0x10000u) >> 10));
-                    u_escape(0xDC00u + ((cp - 0x10000u) & 0x3FFu));
-                } else {
-                    u_escape(cp);
-                }
-            }
+            for (uint32_t i = 0; i < len;) json_char(decode_cp(s, len, i));
         } else if (!(flags & TOK_ESCAPED)) {
             put(s, len);
         } else {

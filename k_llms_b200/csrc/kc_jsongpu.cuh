@@ -35,8 +35,8 @@
 //                       leader turns them into piece offsets and record lengths          (then two exclusive scans: offsets)
 //   C1  write_kernel    lane j writes `"key": value` / `"key": confidence` at its offset of the two output blobs
 //
-// A record the device path does not model exactly (\u escapes and non-ASCII without KC_JSON_UNICODE, or with it in vote fields, escapes in
-// keys, lists without KC_JSON_LISTS, empty objects, an object in one
+// A record the device path does not model exactly (\u escapes, DEL and non-ASCII without KC_JSON_UNICODE, or with it in vote fields,
+// escapes, DEL and non-ASCII in keys, lists without KC_JSON_LISTS, empty objects, an object in one
 // candidate against a value in another, candidates of different shapes without KC_JSON_KEY_UNION, multi-word strings outside
 // K4's contract, numbers outside the exact-conversion range, ...) gets a non-zero status and is
 // consolidated by the host path (kc_consolidate_json) instead: the device path never guesses.

@@ -124,10 +124,15 @@ def test_native_similarity_matches_python():
             return {rng.choice(["a", "b", "c", "reasoning___x", "source___y", "name"]): rand_val(d + 1) for _ in range(rng.randrange(0, 4))}
         return 1
 
+    pairs = []
     for _ in range(4000):
         a, b = rand_val(), rand_val()
         if rng.random() < 0.3:
             b = json.loads(json.dumps(a))
+        pairs.append((a, b))
+    # a decoded string's backslash before a letter is a character, not an escape: "x\\ty" normalises to "xty"
+    pairs += [("x\\ty", "xty"), ("x\\ty", "x\ty"), (["a\\b c"], ["ab c"]), ({"name": "n\\nb"}, {"name": "nnb"})]
+    for a, b in pairs:
         S._cache.clear()
         exp = float(S.generic_similarity(a, b, "embeddings", raising_embeddings))
         out = ctypes.c_double()

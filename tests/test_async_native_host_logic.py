@@ -131,7 +131,7 @@ def python_async(texts):
 def test_device_phases_match_python_async_route(oracle_kernels):
     from tests.test_json_fuzz import _records
     accepted = declined = 0
-    for _n, recs in _records(600, 4242, ns=(2, 3, 5, 8, 16)).items():
+    for _n, recs in _records(1200, 4242, ns=(2, 3, 5, 8, 16)).items():
         pairs, status = jsongpu_with_oracle(recs, flags=K.JSON_NUMERIC_MEDOID)
         for texts, got, st in zip(recs, pairs, status):
             if got is None:

@@ -122,7 +122,7 @@ def test_numbers_through_the_device_json_path():
 def _fuzz_batches():
     """(label, records): the structured fuzz at n in {2, 3, 5, 8, 16} as generated and at n = 33 and 64, then the general and
     mutated records of the device JSON path's tests."""
-    for n, recs in sorted(_records(4000, 424242).items()):
+    for n, recs in sorted(_records(8000, 424242).items()):
         yield f"fuzz n={n}", recs
     yield "fuzz n=33", _records(160, 33, ns=(33,))[33]
     yield "fuzz n=64", _records(100, 64, ns=(64,))[64]

@@ -33,6 +33,18 @@ def _phrase_variant(rng, base):
 
 WORDS = ["alpha", "Bravo", "charlie", "DELTA", "echo", "fox-trot", "golf", "Hotel", "", "a b", "x\ty", 'q"uote', "back\\slash", "nl\n"]
 
+# Records at n = 3 on the edges of the text rules: DEL (json.dumps prints it as \u007f) in a vote string, a medoid string, a key
+# and free text inside the {"text": ...} wrapper; a literal backslash before a letter in free text and in a list record's string
+# (decoded values: the backslash is a character, "x\\ty" sanitises to "xty")
+TEXT_EDGES = [
+    ['{"s": "x\x7fy"}', '{"s": "x\x7fy"}', '{"s": "xy"}'],
+    ['{"p": "one two\x7f three"}', '{"p": "one two\x7f three"}', '{"p": "one two four"}'],
+    ['{"k\x7f": "x", "b": 1}', '{"k\x7f": "x", "b": 2}', '{"k\x7f": "y"}'],
+    ['x\x7fy "q" \\', '{"text": "x\x7fy \\"q\\" \\\\", "b": 1}', 'x\x7fy "q" \\'],
+    ['x\\ty', 'x\\ty', '{"text": "xty"}'],
+    ['{"s": "x\\\\ty", "l": [1]}', '{"s": "x\\\\ty", "l": [1]}', '{"s": "xty", "l": [1]}'],
+]
+
 
 def _expected(texts):
     from k_llms_b200.utils.consolidation import _format_consensus_content, _safe_parse_content
@@ -214,7 +226,7 @@ def test_native_json_matches_reference_client_order():
         ['{"p": "the big cat"}', '{"p": null}', '{}'],                                              # one non-None phrase
         ['{"p": "the big cat sat"}', '{"p": "a b"}', '{"p": ""}', '{"p": "THE BIG CAT SAT!"}'],     # short and empty members
         ['{"p": "one two three", "q": "x y z w"}', '{"p": "one two tree", "q": "x y z"}', '{"q": "x y z w"}'],
-    ]
+    ] + TEXT_EDGES
     for s in specials:
         records.append((len(s), s))
     by_n = {}

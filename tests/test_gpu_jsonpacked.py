@@ -110,12 +110,13 @@ def test_general_and_mutated_records_never_wrong():
 
 
 def test_device_only_flag_and_reasons():
-    recs = [['{"a": "x\\u0041y"}', '{"a": "x"}'], ['{"a": 1, "b": "q"}', '{"a": 1, "b": "Q!"}'], ['{"a": [1]}', '{"a": [1]}']]
+    recs = [['{"a": "x\\u0041y"}', '{"a": "x"}'], ['{"a": 1, "b": "q"}', '{"a": 1, "b": "Q!"}'], ['{"a": [1]}', '{"a": [1]}'],
+            ['{"a\x7f": "x y z"}', '{"a\x7f": "x y z"}']]  # DEL in a key: the host path prints it as \u007f
     res = run(recs, flags=K.JSON_DEVICE_ONLY)
-    assert list(res.status) == [1, 0, 1] and res.why[0] != 0 and res.why[2] != 0
+    assert list(res.status) == [1, 0, 1, 1] and res.why[0] != 0 and res.why[2] != 0 and res.why[3] != 0
     assert res.content(1) == '{"a": 1.0, "b": "q"}' and res.likelihoods(1) == '{"a": 1.0, "b": 1.0}'
     res = run(recs)
-    assert list(res.status) == [2, 0, 2]
+    assert list(res.status) == [2, 0, 2, 2]
     for r, texts in enumerate(recs):
         assert (res.content(r), res.likelihoods(r)) == _expected_with_lists(texts)
 

@@ -4,7 +4,7 @@ without a GPU: kc_json_plan -> the C oracle in the kernels' place -> kc_json_emi
 import random
 
 from tests.helpers import consolidate_json_with_oracle
-from tests.test_gpu_json import _expected, _random_nested_record, _random_record
+from tests.test_gpu_json import TEXT_EDGES, _expected, _random_nested_record, _random_record
 
 
 def test_two_phase_native_json_matches_client_order_cpu():
@@ -31,6 +31,8 @@ def test_two_phase_native_json_matches_client_order_cpu():
                 ['{"s": "00"}', '{"s": -0.0}', '{"s": 1e16}', '{"s": -0.0}'],
                 ['{"s": "1e16"}', '{"s": 1e16}', '{"s": -0.0}', '{"s": 1e16}']]
     for texts, got in zip(specials, consolidate_json_with_oracle(specials)):
+        assert got is not None and got == _expected(texts), texts
+    for texts, got in zip(TEXT_EDGES, consolidate_json_with_oracle(TEXT_EDGES)):
         assert got is not None and got == _expected(texts), texts
 
 

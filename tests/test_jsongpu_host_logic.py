@@ -310,6 +310,8 @@ def test_declines_what_it_does_not_model():
     cases = {
         "unicode escape": ['{"a": "x\\u0041y"}', '{"a": "x"}'],
         "escape in a key": ['{"a\\n": "x"}', '{"a\\n": "x"}'],
+        "DEL in a key": ['{"a\x7f": "x"}', '{"a\x7f": "x"}'],   # json.dumps prints DEL as \u007f: the emit prints a key's bytes
+        "DEL in a value": ['{"a": "x\x7fy"}', '{"a": "x"}'],  # and without KC_JSON_UNICODE a value's
         "bad escape": ['{"a": "x\\qy"}', '{"a": "x"}'],
         "non-ascii": ['{"a": "café"}', '{"a": "cafe"}'],
         "nested here, None there": ['{"a": {"b": 1}}', '{"a": null}'],

@@ -132,6 +132,7 @@ DECLINED = {
     "vote_single_live": ([{"a": "été"}, {"a": None}], D_ESCAPE_OR_NON_ASCII),
     "key_raw": ([{"é": PHRASE}, {"é": PHRASE}], D_ESCAPE_OR_NON_ASCII),
     "key_escaped": (['{"\\u0061": "x y z"}', '{"a": "x y z"}'], D_ESCAPE_OR_NON_ASCII),
+    "key_del": (['{"a\x7f": "x y z"}', '{"a\x7f": "x y z"}'], D_ESCAPE_OR_NON_ASCII),
     "bad_u_escape_short": (['{"a": "x y \\u12"}', '{"a": "x y z"}'], D_SYNTAX),
     "bad_u_escape_hex": (['{"a": "x y \\u12g4"}', '{"a": "x y z"}'], D_SYNTAX),
     "bad_u_escape_at_end": (['{"a": "x y \\u', '{"a": "x y z"}'], D_SYNTAX),
