@@ -266,6 +266,30 @@ def oracle_run(plan):
     return out
 
 
+def _fnv1a(strings_u8):
+    """32-bit FNV-1a of each row of a uint8 [S, L] array (K4's duplicate filter, kc_medoid.cuh)."""
+    h = np.full(len(strings_u8), 2166136261, dtype=np.uint32)
+    for q in range(strings_u8.shape[1]):
+        h = (h ^ strings_u8[:, q]) * np.uint32(16777619)
+    return h
+
+
+def _fnv_collision(seed=1):
+    """Two different [a-z0-9] strings of length 8 with the same 32-bit FNV-1a hash, by a birthday search."""
+    rng = np.random.default_rng(seed)
+    alphabet = np.frombuffer(b"abcdefghijklmnopqrstuvwxyz0123456789", dtype=np.uint8)
+    strs = np.zeros((0, 8), dtype=np.uint8)
+    while True:
+        strs = np.concatenate([strs, alphabet[rng.integers(0, 36, (50000, 8))]])
+        h = _fnv1a(strs)
+        order = np.argsort(h, kind="stable")
+        same = np.nonzero(h[order][1:] == h[order][:-1])[0]
+        for s in same:
+            a, b = strs[order[s]].tobytes().decode(), strs[order[s + 1]].tobytes().decode()
+            if a != b:
+                return a, b
+
+
 _WORDS = ("invoice total due amount net gross payment bank transfer within thirty days from receipt of goods and services "
           "the a an of to acme corp ltd gmbh street road avenue suite floor new york london paris berlin 2024 2025 q1 q2 "
           "ref no id number 000123 77 ab-12 x y z").split()

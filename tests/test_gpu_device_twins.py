@@ -18,7 +18,8 @@ import pytest
 
 from k_llms_b200 import _native as K
 from tests.alignsim_cases import NODE_SIZES, assert_matrices, expected_matrices, node_sets, run_nodes
-from tests.helpers import boundary_texts, general_and_mutated_records, jsongpu_with_oracle, near_halfway_texts, number_texts, repr_doubles
+from tests.helpers import (_fnv1a, _fnv_collision, boundary_texts, general_and_mutated_records, jsongpu_with_oracle, near_halfway_texts,
+                           number_texts, repr_doubles)
 from tests.test_gpu_json import _expected
 from tests.test_json_fuzz import _records
 from tests.test_jsongpu_host_logic import assert_parsed_like_cpython, parse_doubles
@@ -196,29 +197,6 @@ def test_alignsim_matrices_on_the_device():
 
 
 # ----------------------------------------------------------------------------- D. K4 under jaccard / hamming
-
-def _fnv1a(strings_u8):
-    h = np.full(len(strings_u8), 2166136261, dtype=np.uint32)
-    for q in range(strings_u8.shape[1]):
-        h = (h ^ strings_u8[:, q]) * np.uint32(16777619)
-    return h
-
-
-def _fnv_collision(seed=1):
-    """Two different [a-z0-9] strings of length 8 with the same 32-bit FNV-1a hash, by a birthday search."""
-    rng = np.random.default_rng(seed)
-    alphabet = np.frombuffer(b"abcdefghijklmnopqrstuvwxyz0123456789", dtype=np.uint8)
-    strs = np.zeros((0, 8), dtype=np.uint8)
-    while True:
-        strs = np.concatenate([strs, alphabet[rng.integers(0, 36, (50000, 8))]])
-        h = _fnv1a(strs)
-        order = np.argsort(h, kind="stable")
-        same = np.nonzero(h[order][1:] == h[order][:-1])[0]
-        for s in same:
-            a, b = strs[order[s]].tobytes().decode(), strs[order[s + 1]].tobytes().decode()
-            if a != b:
-                return a, b
-
 
 def _sim(a, b, method):
     if a == b:
