@@ -104,6 +104,20 @@ def numeric_edge_vals(rng, G, n):
     return np.ascontiguousarray(vals)
 
 
+def _up(x, k=1):
+    """The float k ulps above x."""
+    for _ in range(k):
+        x = math.nextafter(x, math.inf)
+    return x
+
+
+def _down(x, k=1):
+    """The float k ulps below x."""
+    for _ in range(k):
+        x = math.nextafter(x, -math.inf)
+    return x
+
+
 def raising_embeddings(texts):
     raise RuntimeError("no network in tests")
 

@@ -4,23 +4,11 @@ import numpy as np
 import pytest
 
 from oracle import columnar as OC
-from tests.helpers import EDGE_EPS
+from tests.helpers import EDGE_EPS, _down, _up
 
 pytestmark = pytest.mark.gpu
 
 NONE, ABSENT = OC.F64_NONE, OC.F64_ABSENT
-
-
-def _up(x, k=1):
-    for _ in range(k):
-        x = np.nextafter(x, np.inf)
-    return x
-
-
-def _down(x, k=1):
-    for _ in range(k):
-        x = np.nextafter(x, -np.inf)
-    return x
 
 
 def _extras(rng, v, rel, ab):
