@@ -53,13 +53,14 @@ struct Tok {
 };
 
 struct Item {
-    std::string_view key;
+    std::string_view key;  // raw span; empty for a list element
+    bool kesc = false;     // the key holds escapes (only aligned texts may: json.dumps escapes quotes, backslashes, controls)
     Tok tok;
 };
 
 // f(c) for each character of a string given by its span: with `esc` (a raw JSON span holding escapes) each escape is decoded
 // by kc::js::decode_cp; every other byte is one character.  A span without escapes is the value itself, and it need not be
-// JSON: the {"text": ...} wrapper and the aligned tree's strings are decoded values, in which a backslash is a backslash.
+// JSON: the {"text": ...} wrapper is a decoded value, in which a backslash is a backslash.
 template <typename F>
 void each_char(const char *p, uint32_t len, bool esc, F f) {
     const uint8_t *s = (const uint8_t *)p;
@@ -226,41 +227,43 @@ struct Scanner {
     }
 };
 
-// json.loads(text) for a flat object; anything else that json.loads would ACCEPT (top-level list, number, ...) is
-// reported through `not_object`; a parse failure means the reference wraps the text (consolidation.py:37-38).
-// `odd` is set for things this fast path does not model (escaped keys): the record goes to the Python path.
-bool parse_object(const char *s, size_t len, std::vector<Item> &out, bool &not_object, bool &non_ascii, bool &odd) {
+// json.loads(text) one level deep: an object's (key, value) items or, with `lists`, a list's elements (empty keys).  `object`
+// tells whether it was an object; anything else that json.loads would ACCEPT (top-level list, number, ...) has no members.
+// A parse failure means the reference wraps the text (consolidation.py:37-38).  `odd` is set for escaped keys.
+bool parse_members(const char *s, size_t len, bool lists, std::vector<Item> &out, bool &object, bool &non_ascii, bool &odd) {
     Scanner sc{s, s + len};
-    not_object = false;
     out.clear();
     sc.ws();
     if (sc.p >= sc.end) return false;
-    if (*sc.p != '{') {
+    const char open = *sc.p;
+    object = open == '{';
+    if (!object && (open != '[' || !lists)) {
         Tok t;
         const bool ok = sc.value(t);
         sc.ws();
-        if (ok && sc.p == sc.end) not_object = true;
         non_ascii = sc.non_ascii;
         return ok && sc.p == sc.end;
     }
+    const char close = object ? '}' : ']';
     ++sc.p;
     sc.ws();
-    if (sc.p < sc.end && *sc.p == '}') {
+    if (sc.p < sc.end && *sc.p == close) {
         ++sc.p;
     } else {
         for (;;) {
-            sc.ws();
-            if (sc.p >= sc.end || *sc.p != '"') return false;
-            const char *kp;
-            uint32_t kl;
-            bool kesc;
-            if (!sc.string(kp, kl, kesc)) return false;
-            if (kesc) odd = true;
-            sc.ws();
-            if (sc.p >= sc.end || *sc.p != ':') return false;
-            ++sc.p;
             Item it;
-            it.key = std::string_view(kp, kl);
+            if (object) {
+                sc.ws();
+                if (sc.p >= sc.end || *sc.p != '"') return false;
+                const char *kp;
+                uint32_t kl;
+                if (!sc.string(kp, kl, it.kesc)) return false;
+                odd |= it.kesc;
+                sc.ws();
+                if (sc.p >= sc.end || *sc.p != ':') return false;
+                ++sc.p;
+                it.key = std::string_view(kp, kl);
+            }
             if (!sc.value(it.tok)) return false;
             out.push_back(it);
             sc.ws();
@@ -268,7 +271,7 @@ bool parse_object(const char *s, size_t len, std::vector<Item> &out, bool &not_o
                 ++sc.p;
                 continue;
             }
-            if (sc.p < sc.end && *sc.p == '}') {
+            if (sc.p < sc.end && *sc.p == close) {
                 ++sc.p;
                 break;
             }
@@ -278,6 +281,26 @@ bool parse_object(const char *s, size_t len, std::vector<Item> &out, bool &not_o
     sc.ws();
     non_ascii = sc.non_ascii;
     return sc.p == sc.end;
+}
+
+// a.key < b.key in byte order of the decoded keys (code-point order for ASCII, consensus_utils.py:521-522)
+bool key_less(const Item &a, const Item &b) {
+    if (!a.kesc && !b.kesc) return a.key < b.key;
+    thread_local std::string x, y;
+    str_value(a.key.data(), (uint32_t)a.key.size(), a.kesc, x);
+    str_value(b.key.data(), (uint32_t)b.key.size(), b.kesc, y);
+    return x < y;
+}
+
+// "reasoning___" in key or "source___" in key (cu:1292), on the decoded key
+bool special_key(const Item &k) {
+    thread_local std::string decoded;
+    std::string_view key = k.key;
+    if (k.kesc) {
+        str_value(k.key.data(), (uint32_t)k.key.size(), true, decoded);
+        key = decoded;
+    }
+    return key.find("reasoning___") != std::string_view::npos || key.find("source___") != std::string_view::npos;
 }
 
 // ---------------------------------------------------------------- CPython text formats
@@ -359,7 +382,6 @@ enum GroupKind : uint8_t { G_ALLNULL = 0, G_VOTE_STR, G_VOTE_BOOL, G_NUMERIC, G_
 
 struct Group {
     GroupKind kind;
-    std::string_view key;
     int64_t row = -1;       // row in the vote / numeric cell matrix, or the medoid group index
     uint32_t m_first = 0;   // G_MEDOID: first string of the group in Record::mlen, and how many (the non-None cells)
     uint32_t m_count = 0;
@@ -367,20 +389,21 @@ struct Group {
 
 // Shape of the consensus object: a dict node lists its children (sorted keys), a leaf points at its group.
 struct Node {
-    std::string_view key;
+    std::string_view key;      // raw span of the key (Item::key / kesc)
+    bool kesc = false;
     int32_t group = -1;        // >= 0: leaf
     bool is_list = false;      // a list node: children are its columns, in order (no keys)
     std::vector<int32_t> kids; // dict / list: indices into Record::nodes
 };
 
 struct Record {
-    uint8_t status = 0;        // 0 native, 1 needs the Python path
+    uint8_t status = 0;        // 0 native, 1 needs the Python path, 2 (while planning) has list fields: align, then plan again
     std::vector<Node> nodes;   // nodes[0] is the root dict
     std::vector<Group> groups;
     std::vector<Tok> cells;    // groups.size() * n tokens, group-major (T_MISSING / T_NULL count as None)
     std::string mchars;        // normalize_string() of the cells of the medoid groups, back to back
     std::vector<int32_t> mlen; // their lengths
-    std::shared_ptr<void> tree;  // records with lists: the aligned value tree the cells and keys point into
+    std::vector<std::string> aligned;  // records with lists: the aligned candidate texts the cells and keys point into
 };
 
 const double kF64None = [] { const uint64_t b = KC_F64_NONE_BITS; double d; memcpy(&d, &b, 8); return d; }();
@@ -463,106 +486,119 @@ bool plan_leaf(Record &rec, Group &g, const Tok *cells, int n) {
     return true;
 }
 
-constexpr int kMaxDepth = 16;
+// Depth bounds: on the texts as given, objects nested at most 15 below the root (16 levels of objects, whose fields sit one
+// level deeper); on aligned texts, any value at most 48 below it (49 levels of the value tree, fields included).
+constexpr int kMaxObjectDepth = 15, kMaxValueDepth = 48;
 
-// One dict level of the alignment pre-pass + dispatcher (cu:516-548 then cu:1414-1426): `items[c]` is candidate c's
-// (key-sorted) dict at this node, or nullptr where it has none — the pre-pass turns None into a dict of Nones, so after
-// it EVERY candidate is a dict here and parent_valid_frac stays 1.  Keys are visited in sorted order; a key whose values
-// are all objects recurses, any list (or a mix of objects and scalars) sends the record to the Python path.
+// One node of the alignment pre-pass + dispatcher (cu:516-548, cu:550-613, then cu:1414-1426): `items[c]` is candidate c's
+// members here (an object's items sorted by key, or a list's elements), or nullptr where it holds None — the pre-pass turns
+// None into an object or list of Nones, so parent_valid_frac stays 1.  The children (keys in sorted order, or a list's
+// columns in order) whose values are all objects or all lists recurse; scalar fields go to plan_leaf; a mix of objects,
+// lists and scalars sends the record to the Python path.  On the texts as given a list sets status 2: the record goes
+// through the alignment pre-pass and is planned again on its `aligned` texts, where a list node holds lists of one width.
 struct LevelScratch {  // per recursion depth, reused across records (no allocation in the steady state)
-    std::vector<std::string_view> keys;
+    std::vector<const Item *> keys;
     std::vector<size_t> cursor;
     std::vector<Tok> cells;
     std::vector<std::vector<Item>> child_items;
     std::vector<const std::vector<Item> *> child;
 };
 
-void plan_dict(Record &rec, int32_t node, const std::vector<Item> *const *items, int n, int depth) {
-    thread_local std::vector<LevelScratch> levels(kMaxDepth + 1);  // sized once: references stay valid through the recursion
+void plan_node(Record &rec, int32_t node, const std::vector<Item> *const *items, int n, int depth, bool aligned) {
+    thread_local std::vector<LevelScratch> levels(kMaxValueDepth + 1);  // sized once: references stay valid through the recursion
     LevelScratch &L = levels[(size_t)depth];
-    std::vector<std::string_view> &keys = L.keys;
+    const bool list = rec.nodes[(size_t)node].is_list;
+    std::vector<const Item *> &keys = L.keys;
     keys.clear();
+    size_t width = 0;
     for (int c = 0; c < n; ++c)
-        if (items[c])
-            for (auto &it : *items[c]) keys.push_back(it.key);
-    std::sort(keys.begin(), keys.end());  // code-point order == byte order for ASCII (consensus_utils.py:521-522)
-    keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+        if (items[c]) {
+            if (list) {
+                width = items[c]->size();
+                break;
+            }
+            for (auto &it : *items[c]) keys.push_back(&it);
+        }
+    if (!list) {
+        std::sort(keys.begin(), keys.end(), [](const Item *a, const Item *b) { return key_less(*a, *b); });
+        keys.erase(std::unique(keys.begin(), keys.end(), [](const Item *a, const Item *b) { return a->key == b->key; }), keys.end());
+        width = keys.size();
+    }
     std::vector<size_t> &cursor = L.cursor;
     cursor.assign((size_t)n, 0);
     std::vector<Tok> &cells = L.cells;
     cells.resize((size_t)n);
-    for (size_t ki = 0; ki < keys.size(); ++ki) {
-        const std::string_view key = keys[ki];
+    for (size_t ki = 0; ki < width; ++ki) {
+        const std::string_view key = list ? std::string_view() : keys[ki]->key;
         for (int c = 0; c < n; ++c) {  // merge: both sides are sorted by key; of duplicates the last one wins
             cells[(size_t)c] = Tok();
             if (!items[c]) continue;
             const auto &its = *items[c];
             size_t &k = cursor[(size_t)c];
-            while (k < its.size() && its[k].key == key) cells[(size_t)c] = its[k++].tok;
+            if (list) cells[(size_t)c] = its[ki].tok;
+            else
+                while (k < its.size() && its[k].key == key) cells[(size_t)c] = its[k++].tok;
         }
-        if (key.find("reasoning___") != std::string_view::npos || key.find("source___") != std::string_view::npos) continue;  // cu:1292
+        if (!list && special_key(*keys[ki])) continue;
         const Tok *first = nullptr;
         for (int c = 0; c < n && !first; ++c)
             if (cells[(size_t)c].type > T_NULL) first = &cells[(size_t)c];
-        if (first && first->type == T_NESTED) {
-            if (*first->p != '{') {  // a list: the whole record goes through the alignment pre-pass (tree path below)
-                rec.status = 2;
-                return;
-            }
-            if (depth + 1 >= kMaxDepth) {
-                rec.status = 1;
-                return;
-            }
+        const bool nested = first && first->type == T_NESTED;
+        if (nested && *first->p == '[' && !aligned) {
+            rec.status = 2;
+            return;
+        }
+        if ((nested || aligned) && depth + 1 > (aligned ? kMaxValueDepth : kMaxObjectDepth)) {
+            rec.status = 1;
+            return;
+        }
+        const int32_t kid = (int32_t)rec.nodes.size();
+        rec.nodes.emplace_back();
+        rec.nodes[(size_t)kid].key = key;
+        rec.nodes[(size_t)kid].kesc = !list && keys[ki]->kesc;
+        rec.nodes[(size_t)node].kids.push_back(kid);
+        if (nested) {
             auto &child_items = L.child_items;
             if ((int)child_items.size() < n) child_items.resize((size_t)n);
             auto &child = L.child;
             child.assign((size_t)n, nullptr);
-            for (int c = 0; c < n; ++c) {
-                const Tok &t = cells[(size_t)c];
+            const size_t fc = (size_t)(first - cells.data());
+            for (size_t c = fc; c < (size_t)n; ++c) {
+                const Tok &t = cells[c];
                 if (t.type <= T_NULL) continue;
-                if (t.type != T_NESTED || *t.p != '{') {  // not all of one type: the pre-pass leaves the values alone (cu:507-512)
+                if (t.type != T_NESTED || *t.p != *first->p) {  // not all of one type: the pre-pass leaves the values alone (cu:507-512)
                     rec.status = 1;
                     return;
                 }
-                bool not_object = false, non_ascii = false, odd = false;
-                if (!parse_object(t.p, t.len, child_items[(size_t)c], not_object, non_ascii, odd) || not_object || non_ascii || odd) {
+                bool object = false, non_ascii = false, odd = false;
+                if (!parse_members(t.p, t.len, true, child_items[c], object, non_ascii, odd) || non_ascii || (odd && !aligned) ||
+                    (!object && child_items[c].size() != child_items[fc].size())) {
                     rec.status = 1;
                     return;
                 }
-                std::stable_sort(child_items[(size_t)c].begin(), child_items[(size_t)c].end(),
-                                 [](const Item &a, const Item &b) { return a.key < b.key; });
-                child[(size_t)c] = &child_items[(size_t)c];
+                std::stable_sort(child_items[c].begin(), child_items[c].end(), key_less);
+                child[c] = &child_items[c];
             }
-            const int32_t kid = (int32_t)rec.nodes.size();
-            rec.nodes.emplace_back();
-            rec.nodes[(size_t)kid].key = key;
-            rec.nodes[(size_t)node].kids.push_back(kid);
-            plan_dict(rec, kid, child.data(), n, depth + 1);
+            rec.nodes[(size_t)kid].is_list = *first->p == '[';
+            plan_node(rec, kid, child.data(), n, depth + 1, aligned);
             if (rec.status) return;
             continue;
         }
         const size_t base = rec.cells.size();
         rec.cells.insert(rec.cells.end(), cells.begin(), cells.end());
-        const Tok *gcells = &rec.cells[base];
         Group g;
-        g.key = key;
-        if (!plan_leaf(rec, g, gcells, n)) return;
-        const int32_t kid = (int32_t)rec.nodes.size();
-        rec.nodes.emplace_back();
-        rec.nodes[(size_t)kid].key = key;
+        if (!plan_leaf(rec, g, &rec.cells[base], n)) return;
         rec.nodes[(size_t)kid].group = (int32_t)rec.groups.size();
-        rec.nodes[(size_t)node].kids.push_back(kid);
         rec.groups.push_back(g);
     }
 }
 
-void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Record &rec);
-
-// defer_lists: a record with list fields keeps status 2 for the caller, which aligns it (plan_batch); else it is aligned here
-void plan_record(const char *const *texts, const int64_t *lens, int n, Record &rec, bool defer_lists) {
+// Plans a record from its n candidate texts, or (`aligned`) from the texts the alignment pre-pass made of them.
+void plan_record(const char *const *texts, const int64_t *lens, int n, Record &rec, bool aligned) {
     thread_local std::vector<std::vector<Item>> cands;
     if ((int)cands.size() < n) cands.resize((size_t)n);
     static const char kTextKey[] = "text";
+    rec.status = 0;
     for (int c = 0; c < n; ++c) {
         const char *s = texts[c];
         const size_t len = lens ? (size_t)lens[c] : strlen(s);
@@ -570,13 +606,13 @@ void plan_record(const char *const *texts, const int64_t *lens, int n, Record &r
             rec.status = 1;
             return;
         }
-        bool not_object = false, non_ascii = false, odd = false;
+        bool object = false, non_ascii = false, odd = false;
         std::vector<Item> &items = cands[(size_t)c];
-        const bool ok = parse_object(s, len, items, not_object, non_ascii, odd);
+        const bool ok = parse_members(s, len, false, items, object, non_ascii, odd);
         if (!ok || !non_ascii)  // a failed parse may have stopped early: look at every byte
             for (size_t i = 0; i < len && !non_ascii; ++i)
                 if ((unsigned char)s[i] >= 0x80) non_ascii = true;
-        if (non_ascii || odd || (ok && not_object)) {
+        if (non_ascii || (odd && !aligned) || (ok && !object)) {
             rec.status = 1;
             return;
         }
@@ -590,7 +626,7 @@ void plan_record(const char *const *texts, const int64_t *lens, int n, Record &r
             items.push_back(it);
         }
         // sort by key; of duplicates the LAST one in the text wins (dict construction)
-        std::stable_sort(items.begin(), items.end(), [](const Item &a, const Item &b) { return a.key < b.key; });
+        std::stable_sort(items.begin(), items.end(), key_less);
     }
     rec.groups.clear();
     rec.cells.clear();
@@ -601,8 +637,7 @@ void plan_record(const char *const *texts, const int64_t *lens, int n, Record &r
     thread_local std::vector<const std::vector<Item> *> top;
     top.assign((size_t)n, nullptr);
     for (int c = 0; c < n; ++c) top[(size_t)c] = &cands[(size_t)c];
-    plan_dict(rec, 0, top.data(), n, 0);
-    if (rec.status == 2 && !defer_lists) plan_record_tree(texts, lens, n, rec);  // list fields: align first (H2), then plan on the aligned tree
+    plan_node(rec, 0, top.data(), n, 0, aligned);
 }
 
 void encode_vote(GroupKind kind, const Tok *toks, int n, int8_t *cells) {
@@ -719,9 +754,9 @@ void emit_node(const EmitCtx &cx, int32_t ni, std::string &content, std::string 
         }
         first = false;
         if (!node.is_list) {
-            const std::string_view key = cx.rec.nodes[(size_t)kid].key;
-            json_string(key, content);
-            json_string(key, lik);
+            const Node &k = cx.rec.nodes[(size_t)kid];
+            json_string(k.key.data(), (uint32_t)k.key.size(), k.kesc, content);
+            json_string(k.key.data(), (uint32_t)k.key.size(), k.kesc, lik);
             content += ": ";
             lik += ": ";
         }
@@ -786,151 +821,23 @@ void parallel_for(int64_t n, int threads, F fn) {
 
 #include "kc_align.inl"  // H2: value tree, similarities, assignment, lists_alignment, recursive_list_alignments
 
-// ---------------------------------------------------------------- H1 for records with list fields: plan on the aligned tree
-
-Tok tok_of(const AVal &v) {  // a scalar of the tree as the token the leaf planner / encoders / emitters work on
-    static const char kBrace[] = "{";
-    Tok t;
-    switch (v.t) {
-        case A_NONE: t.type = T_NULL; break;
-        case A_BOOL: t.type = v.b ? T_TRUE : T_FALSE; break;
-        case A_INT: t.type = T_INT; t.p = v.s.data(); t.len = (uint32_t)v.s.size(); t.num = v.num; break;
-        case A_FLOAT: t.type = T_FLOAT; t.num = v.num; break;
-        case A_STR: t.type = T_STR; t.p = v.s.data(); t.len = (uint32_t)v.s.size(); break;  // already unescaped
-        default: t.type = T_NESTED; t.p = kBrace; t.len = 1; break;
-    }
-    return t;
-}
-
-// The dispatcher (cu:1376-1454) over ALIGNED candidates: after the pre-pass every candidate is a dict with the same sorted
-// keys at a dict node and a list of the same width at a list node (cu:516-548, 550-613), so parent_valid_frac stays 1 and a
-// node is a dict, a list or a scalar field.  Anything the pre-pass left unaligned (mixed types) goes to the Python path.
-void plan_tree_value(Record &rec, AlignCtx &cx, int32_t node, const std::vector<int32_t> &ids, int n, int depth) {
-    if (depth > 48) {
+// A record with list fields, planned again on the n texts the alignment pre-pass made of its candidates (status: the
+// pre-pass's; non-zero sends the record to the Python path).  The record keeps the texts: its cells and keys point into them.
+void plan_aligned(Record &rec, int status, std::vector<std::string> &aligned, int n) {
+    if (status) {
         rec.status = 1;
         return;
     }
-    const AVal *first = nullptr;
-    for (int c = 0; c < n && !first; ++c)
-        if (cx.tr.v[(size_t)ids[(size_t)c]].t != A_NONE) first = &cx.tr.v[(size_t)ids[(size_t)c]];
-    if (first && (first->t == A_DICT || first->t == A_LIST)) {
-        const AType ft = first->t;
-        for (int c = 0; c < n; ++c)
-            if (cx.tr.v[(size_t)ids[(size_t)c]].t != ft) {  // not what the pre-pass produces from uniform input
-                rec.status = 1;
-                return;
-            }
-        std::vector<int32_t> child((size_t)n);
-        if (ft == A_DICT) {
-            const size_t width = first->kv.size();
-            for (int c = 0; c < n; ++c)
-                if (cx.tr.v[(size_t)ids[(size_t)c]].kv.size() != width) {
-                    rec.status = 1;
-                    return;
-                }
-            for (size_t k = 0; k < width; ++k) {
-                const std::string &key = cx.tr.v[(size_t)ids[0]].kv[k].first;
-                for (int c = 0; c < n; ++c) {
-                    const auto &e = cx.tr.v[(size_t)ids[(size_t)c]].kv[k];
-                    if (e.first != key) {
-                        rec.status = 1;
-                        return;
-                    }
-                    child[(size_t)c] = e.second;
-                }
-                if (key.find("reasoning___") != std::string::npos || key.find("source___") != std::string::npos) continue;  // cu:1292
-                const int32_t kid = (int32_t)rec.nodes.size();
-                rec.nodes.emplace_back();
-                rec.nodes[(size_t)kid].key = key;
-                rec.nodes[(size_t)node].kids.push_back(kid);
-                plan_tree_value(rec, cx, kid, child, n, depth + 1);
-                if (rec.status) return;
-            }
-        } else {
-            rec.nodes[(size_t)node].is_list = true;
-            const size_t width = first->items.size();
-            for (int c = 0; c < n; ++c)
-                if (cx.tr.v[(size_t)ids[(size_t)c]].items.size() != width) {
-                    rec.status = 1;
-                    return;
-                }
-            for (size_t k = 0; k < width; ++k) {
-                for (int c = 0; c < n; ++c) child[(size_t)c] = cx.tr.v[(size_t)ids[(size_t)c]].items[k];
-                const int32_t kid = (int32_t)rec.nodes.size();
-                rec.nodes.emplace_back();
-                rec.nodes[(size_t)node].kids.push_back(kid);
-                plan_tree_value(rec, cx, kid, child, n, depth + 1);
-                if (rec.status) return;
-            }
-        }
-        return;
+    rec.aligned = std::move(aligned);
+    thread_local std::vector<const char *> texts;
+    thread_local std::vector<int64_t> lens;
+    texts.resize((size_t)n);
+    lens.resize((size_t)n);
+    for (int c = 0; c < n; ++c) {
+        texts[(size_t)c] = rec.aligned[(size_t)c].data();
+        lens[(size_t)c] = (int64_t)rec.aligned[(size_t)c].size();
     }
-    // a scalar field (or all None)
-    const size_t base = rec.cells.size();
-    for (int c = 0; c < n; ++c) rec.cells.push_back(tok_of(cx.tr.v[(size_t)ids[(size_t)c]]));
-    Group g;
-    g.key = rec.nodes[(size_t)node].key;
-    if (!plan_leaf(rec, g, &rec.cells[base], n)) return;
-    rec.nodes[(size_t)node].group = (int32_t)rec.groups.size();
-    rec.groups.push_back(g);
-}
-
-// The candidate texts of a record with list fields as a value tree; false: the record takes the Python path (status 1).
-bool parse_record_tree(const char *const *texts, const int64_t *lens, int n, Record &rec, AlignCtx &cx, std::vector<int32_t> &values) {
-    rec.status = 0;
-    rec.groups.clear();
-    rec.cells.clear();
-    rec.mchars.clear();
-    rec.mlen.clear();
-    rec.nodes.clear();
-    values.assign((size_t)n, -1);
-    {
-        size_t bytes = 0;
-        for (int c = 0; c < n; ++c) bytes += lens ? (size_t)lens[c] : strlen(texts[c]);
-        cx.tr.v.reserve(bytes / 6 + 16);  // a value per ~6 bytes of JSON, plus what the alignment adds: no regrowth (moves of every node) while parsing
-    }
-    for (int c = 0; c < n; ++c) {  // _safe_parse_content (consolidation.py:25-38); the caller already ruled out empty / non-ASCII text
-        const size_t len = lens ? (size_t)lens[c] : strlen(texts[c]);
-        Scanner sc{texts[c], texts[c] + len};
-        const size_t mark = cx.tr.v.size();
-        bool ok = aparse(sc, cx.tr, values[(size_t)c], 0);
-        if (ok) {
-            sc.ws();
-            ok = sc.p == sc.end;
-        }
-        if (ok && cx.tr.v[(size_t)values[(size_t)c]].t != A_DICT) {  // valid JSON but not an object: Python path (as the flat planner does)
-            rec.status = 1;
-            return false;
-        }
-        if (!ok) {  // {"text": content}
-            cx.tr.v.resize(mark);
-            const int32_t str = cx.tr.add(A_STR);
-            cx.tr.v[(size_t)str].s.assign(texts[c], len);
-            const int32_t d = cx.tr.add(A_DICT);
-            cx.tr.v[(size_t)d].kv.emplace_back("text", str);
-            values[(size_t)c] = d;
-        }
-    }
-    return true;
-}
-
-// The alignment pre-pass, then the plan on the aligned tree
-void finish_record_tree(Record &rec, const std::shared_ptr<AlignCtx> &cxp, std::vector<int32_t> &values, int n) {
-    AlignCtx &cx = *cxp;
-    align_values(cx, values, /*min_support_ratio=*/0.51, 0);  // ConsensusSettings default (cu:41); other settings: Python path
-    if (cx.decline) {
-        rec.status = 1;
-        return;
-    }
-    rec.nodes.emplace_back();
-    plan_tree_value(rec, cx, 0, values, n, 0);
-    if (rec.status == 0) rec.tree = cxp;  // from here on nothing is added to the tree: cells and keys point into it
-}
-
-void plan_record_tree(const char *const *texts, const int64_t *lens, int n, Record &rec) {
-    auto cxp = std::make_shared<AlignCtx>();
-    std::vector<int32_t> values;
-    if (parse_record_tree(texts, lens, n, rec, *cxp, values)) finish_record_tree(rec, cxp, values, n);
+    plan_record(texts.data(), lens.data(), n, rec, true);
 }
 
 // ---------------------------------------------------------------- a batch of records: plan, encode, emit
@@ -946,35 +853,35 @@ struct Batch {
 
 int default_threads() { return (int)std::min(32u, std::max(1u, std::thread::hardware_concurrency())); }  // parsing saturates memory / malloc beyond ~32
 
-// sim_device >= 0: the element similarities of the records with list fields come from one kc_alignsim pass on that device
-// (the records are aligned after it); < 0: every similarity is computed on the host while aligning.
+// Records with list fields are aligned (H2, under the ConsensusSettings default min_support_ratio 0.51, cu:41) and planned again
+// on their aligned texts.  sim_device >= 0: the element similarities of their list nodes come from one kc_alignsim pass on that
+// device (the records are aligned after it); < 0: each similarity is computed on the host when the alignment asks for it.
 int plan_batch(Batch &b, const char *const *texts, const int64_t *lens, int64_t n_records, int n, int threads, int sim_device) {
     b.n = n;
     b.recs.assign((size_t)n_records, Record());
-    const bool defer = sim_device >= 0;
-    parallel_for(n_records, threads, [&](int64_t r) { plan_record(texts + r * n, lens ? lens + r * n : nullptr, n, b.recs[(size_t)r], defer); });
-    if (defer) {
-        std::vector<int64_t> idx;  // the records with list fields
-        for (int64_t r = 0; r < n_records; ++r)
-            if (b.recs[(size_t)r].status == 2) idx.push_back(r);
-        std::vector<std::shared_ptr<AlignCtx>> cxs(idx.size());
-        std::vector<std::vector<int32_t>> values(idx.size());
-        std::vector<AlignCtx *> tabs(idx.size(), nullptr);
-        parallel_for((int64_t)idx.size(), threads, [&](int64_t i) {
-            const int64_t r = idx[(size_t)i];
-            cxs[(size_t)i] = std::make_shared<AlignCtx>();
-            if (!parse_record_tree(texts + r * n, lens ? lens + r * n : nullptr, n, b.recs[(size_t)r], *cxs[(size_t)i], values[(size_t)i])) {
-                cxs[(size_t)i].reset();
-                return;
+    parallel_for(n_records, threads, [&](int64_t r) { plan_record(texts + r * n, lens ? lens + r * n : nullptr, n, b.recs[(size_t)r], false); });
+    std::vector<int64_t> idx;  // the records with list fields; a candidate that is not JSON is aligned as {"text": content}
+    for (int64_t r = 0; r < n_records; ++r)
+        if (b.recs[(size_t)r].status == 2) idx.push_back(r);
+    const int64_t m = (int64_t)idx.size();
+    if (sim_device >= 0 && m) {
+        std::vector<const char *> sub_texts((size_t)(m * n));
+        std::vector<int64_t> sub_lens(lens ? (size_t)(m * n) : 0);
+        for (int64_t i = 0; i < m; ++i)
+            for (int c = 0; c < n; ++c) {
+                sub_texts[(size_t)(i * n + c)] = texts[idx[(size_t)i] * n + c];
+                if (lens) sub_lens[(size_t)(i * n + c)] = lens[idx[(size_t)i] * n + c];
             }
-            sim_collect(*cxs[(size_t)i], values[(size_t)i], 0);
-            tabs[(size_t)i] = cxs[(size_t)i].get();
-        });
-        const int rc = sim_batch(tabs, sim_device, threads, nullptr, [&](int64_t i) {
-            if (cxs[(size_t)i]) finish_record_tree(b.recs[(size_t)idx[(size_t)i]], cxs[(size_t)i], values[(size_t)i], n);
-            cxs[(size_t)i].reset();  // a planned record keeps its tree through Record::tree
-        });
+        const int rc = align_batch(sub_texts.data(), lens ? sub_lens.data() : nullptr, m, n, 0.51, true, sim_device, threads,
+                                   nullptr, [&](int64_t i, int status, std::vector<std::string> &aligned) { plan_aligned(b.recs[(size_t)idx[(size_t)i]], status, aligned, n); });
         if (rc) return rc;
+    } else if (m) {
+        parallel_for(m, threads, [&](int64_t i) {
+            const int64_t r = idx[(size_t)i];
+            std::vector<std::string> aligned;
+            const int status = align_record(texts + r * n, lens ? lens + r * n : nullptr, n, 0.51, true, aligned);
+            plan_aligned(b.recs[(size_t)r], status, aligned, n);
+        });
     }
     for (auto &rec : b.recs) {
         if (rec.status) continue;
@@ -1136,27 +1043,10 @@ void kc_json_free(kc_json_batch *h) { delete h; }
 // would be compared through embeddings, cu:813; non-ASCII text); negative for invalid JSON.
 int kc_align_json(const char *const *texts, const int64_t *lens, int32_t n, double min_support_ratio, char **out_texts) {
     if (!texts || !out_texts || n < 1) return KC_EINVAL;
-    AlignCtx cx;
-    std::vector<int32_t> values((size_t)n);
-    for (int32_t c = 0; c < n; ++c) {
-        out_texts[c] = nullptr;
-        const size_t len = lens ? (size_t)lens[c] : strlen(texts[c]);
-        Scanner sc{texts[c], texts[c] + len};
-        if (!aparse(sc, cx.tr, values[(size_t)c], 0)) return KC_EINVAL;
-        sc.ws();
-        if (sc.p != sc.end) return KC_EINVAL;
-        if (sc.non_ascii) return 1;
-        for (size_t i = 0; i < len; ++i)
-            if ((unsigned char)texts[c][i] >= 0x80) return 1;
-    }
-    align_values(cx, values, min_support_ratio, 0);
-    if (cx.decline) return 1;
-    std::string out;
-    for (int32_t c = 0; c < n; ++c) {
-        out.clear();
-        adump(cx.tr, values[(size_t)c], out);
-        out_texts[c] = dup_string(out);
-    }
+    for (int32_t c = 0; c < n; ++c) out_texts[c] = nullptr;
+    std::vector<std::string> aligned;
+    if (const int status = align_record(texts, lens, n, min_support_ratio, false, aligned)) return status;
+    for (int32_t c = 0; c < n; ++c) out_texts[c] = dup_string(aligned[(size_t)c]);
     return 0;
 }
 
@@ -1166,66 +1056,15 @@ int kc_align_json_batch(const char *const *texts, const int64_t *lens, int64_t n
                         int32_t threads, char **out_texts, int32_t *out_status, int64_t *out_counts) {
     if (!texts || !out_texts || !out_status || n < 1 || n_records < 0) return kc_fail(KC_EINVAL, "kc_align_json_batch: bad arguments");
     if (threads <= 0) threads = default_threads();
-    std::vector<std::unique_ptr<AlignCtx>> cxs((size_t)n_records);
-    std::vector<std::vector<int32_t>> values((size_t)n_records);
-    std::vector<AlignCtx *> tabs((size_t)n_records, nullptr);
-    parallel_for(n_records, threads, [&](int64_t r) {  // parse as kc_align_json does, then flatten the list nodes
-        for (int32_t c = 0; c < n; ++c) out_texts[r * n + c] = nullptr;
-        auto cx = std::make_unique<AlignCtx>();
-        std::vector<int32_t> &vals = values[(size_t)r];
-        vals.assign((size_t)n, -1);
-        out_status[r] = 0;
-        for (int32_t c = 0; c < n && !out_status[r]; ++c) {
-            const char *t = texts[r * n + c];
-            const size_t len = lens ? (size_t)lens[r * n + c] : strlen(t);
-            Scanner sc{t, t + len};
-            if (!aparse(sc, cx->tr, vals[(size_t)c], 0)) {
-                out_status[r] = KC_EINVAL;
-                break;
-            }
-            sc.ws();
-            if (sc.p != sc.end) out_status[r] = KC_EINVAL;
-            else if (sc.non_ascii) out_status[r] = 1;
-            for (size_t i = 0; i < len && !out_status[r]; ++i)
-                if ((unsigned char)t[i] >= 0x80) out_status[r] = 1;
-        }
-        if (out_status[r]) return;
-        sim_collect(*cx, vals, 0);
-        tabs[(size_t)r] = cx.get();
-        cxs[(size_t)r] = std::move(cx);
-    });
-    int64_t device_pairs = 0;
-    std::atomic<int64_t> host_pairs{0};
-    const int rc = sim_batch(tabs, device, threads, &device_pairs, [&](int64_t r) {
-        if (!cxs[(size_t)r]) return;
-        AlignCtx &cx = *cxs[(size_t)r];
-        std::vector<int32_t> &vals = values[(size_t)r];
-        align_values(cx, vals, min_support_ratio, 0);
-        host_pairs += cx.host_pairs;
-        if (cx.decline) {
-            out_status[r] = 1;
-        } else {
-            std::string out;
-            for (int32_t c = 0; c < n; ++c) {
-                out.clear();
-                adump(cx.tr, vals[(size_t)c], out);
-                out_texts[r * n + c] = dup_string(out);
-            }
-        }
-        cxs[(size_t)r].reset();
-    });
-    if (rc) {
-        for (int64_t i = 0; i < n_records * n; ++i) {
-            free(out_texts[i]);
-            out_texts[i] = nullptr;
-        }
-        return rc;
-    }
-    if (out_counts) {
-        out_counts[0] = device_pairs;
-        out_counts[1] = host_pairs.load();
-    }
-    return KC_OK;
+    for (int64_t i = 0; i < n_records * n; ++i) out_texts[i] = nullptr;
+    const int rc = align_batch(texts, lens, n_records, n, min_support_ratio, false, device, threads, out_counts,
+                               [&](int64_t r, int status, const std::vector<std::string> &aligned) {
+                                   out_status[r] = status;
+                                   if (!status)
+                                       for (int32_t c = 0; c < n; ++c) out_texts[r * n + c] = dup_string(aligned[(size_t)c]);
+                               });
+    if (rc) kc_free_strings(out_texts, n_records * n);
+    return rc;
 }
 
 // The similarity phase of kc_align_json_batch instantiated on the host for one node whose T elements are given as JSON

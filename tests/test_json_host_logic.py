@@ -37,8 +37,9 @@ def test_two_phase_native_json_matches_client_order_cpu():
 
 
 def test_two_phase_native_json_list_records_cpu():
-    """Records with list fields through the native path (H2 alignment on the parsed tree + element-wise merge), the oracle in
-    the kernels' place: the reference's client-order goldens and random list records."""
+    """Records with list fields through the native path (H2 alignment, then the plan of the aligned texts with an
+    element-wise merge), the oracle in the kernels' place: the reference's client-order goldens, random list records and
+    list records with escaped keys."""
     import json
 
     from oracle.gen_golden import random_list_records
@@ -56,6 +57,20 @@ def test_two_phase_native_json_list_records_cpu():
             assert got == (_format_consensus_content(case["value"]), json.dumps(case["conf"])), (texts, got)
     assert native > 100
     recs = [[json.dumps(v) for v in r] for r in random_list_records(78, 200)]
+    by_n = {}
+    for r in recs:
+        by_n.setdefault(len(r), []).append(r)
+    for _n, rs in by_n.items():
+        for texts, got in zip(rs, consolidate_json_with_oracle(rs)):
+            assert got is not None and got == _expected_with_lists(texts), texts
+    # escaped keys inside list elements and objects: decoded keys decide the order and the special-key skip
+    keys = ["\reasoning___x", "x\"source___", "reasoning___q", 'q"', "q#", "q\\", "q\n", "Q"]
+    rng = random.Random(5)
+    recs = []
+    for _ in range(60):
+        n = rng.choice([2, 3])
+        recs.append([json.dumps({"items": [{k: rng.choice([1, 2, None]) for k in rng.sample(keys, 3)} for _ in range(rng.randrange(1, 3))],
+                                 "o": {k: rng.choice(["a", "b"]) for k in rng.sample(keys, 3)}}) for _ in range(n)])
     by_n = {}
     for r in recs:
         by_n.setdefault(len(r), []).append(r)

@@ -2,7 +2,7 @@
 fields are marked by the first round, aligned by the native pre-pass H2 on the host, and consolidated from the aligned texts with
 list nodes.  The host instantiation of the phases (kc_debug_jsongpu_plan_flags with KC_JSON_LISTS) runs both rounds lane by lane
 with the oracle in the kernels' place; its texts must equal the reference's client-order goldens, the host path H1 (which
-consolidates from the aligned tree) and the Python pre-pass + oracle, byte for byte.  Without the flag nothing changes."""
+consolidates from the aligned texts too) and the Python pre-pass + oracle, byte for byte.  Without the flag nothing changes."""
 import json
 import random
 
